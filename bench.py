@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- Llama-3-8B AWQ-INT4 batch-1 decode on B200 (BASELINE.json configs[1] at N = 1, configs[4] = tensor-parallel decode at
+"""bench.py -- Llama-3-8B AWQ-INT4 batch-1 decode on H100 (BASELINE.json configs[1] at N = 1, configs[4] = tensor-parallel decode at
 N > 1), the reference's own CPU path beside it.
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path (one rank per GPU under torchrun)
@@ -12,6 +12,10 @@ entry point (tce_llama_decode_host): token id/position copied from pinned host m
 back, every step, inside the timed region.  N > 1 defaults to tensor-parallel decode of ONE sequence (column/row sharded linears,
 two all-reduces per layer over NVLink peer memory inside the persistent kernel); `tp_parity_rel_err` compares its logits with a
 single-GPU run of the same weights before timing.  One JSON line on stdout (rank 0).  See DESIGN.md "Measurement".
+
+    --dump-outputs DIR   write what the last timed step computed as DIR/<name>.npy (float32): `logits` (last tce_llama_decode),
+                         `logits_host` / `next_token_host` (last tce_llama_decode_host), `prefill_13b_2048_logits` (last position of
+                         the prompt pass, when the extras run).  All inputs are seeded: two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -63,7 +67,7 @@ def env_rank():
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# clocks: sample NVML during the timed region (B200_PROFILING.md timing hygiene)
+# clocks: sample NVML during the timed region (a power-capped card lowers its clocks under sustained load)
 # ------------------------------------------------------------------------------------------------------------------
 class ClockSampler:
     REASONS = {0x1: "gpu_idle", 0x2: "applications_clocks_setting", 0x4: "sw_power_cap", 0x8: "hw_slowdown", 0x10: "sync_boost",
@@ -117,7 +121,7 @@ def load_peaks():
     if p.exists():
         d = json.loads(p.read_text())
         return d, float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return {}, 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return {}, 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -439,7 +443,7 @@ def run_reference(args):
 # secondary configs measured in the same run (BASELINE.json configs[2], configs[3]) and the reference's CUDA kernel on this GPU
 # ------------------------------------------------------------------------------------------------------------------
 def gpu_reference_gemv(model, geom, dev):
-    """The reference's own gemv_kernel_g128 (kernels/cuda/gemv_cuda.cu, compiled unchanged for sm_100a into oracle/_ref) over every
+    """The reference's own gemv_kernel_g128 (kernels/cuda/gemv_cuda.cu, compiled unchanged for sm_90a into oracle/_ref) over every
     GEMV of one decode step on the model's real weights: the GPU-side baseline SURVEY.md 8(d) config 2 names."""
     import torch
 
@@ -478,17 +482,18 @@ def gpu_reference_gemv(model, geom, dev):
         e1.record(ds)
         torch.cuda.synchronize(dev)
     ms = e0.elapsed_time(e1) / reps
-    return {"kernel": "reference gemv_kernel_g128 (kernels/cuda/gemv_cuda.cu:140-194) built for sm_100a, all GEMVs of one step, eager launches",
+    return {"kernel": "reference gemv_kernel_g128 (kernels/cuda/gemv_cuda.cu:140-194) built for sm_90a, all GEMVs of one step, eager launches",
             "ms_per_token_gemvs_only": ms, "tok_s_gemvs_only": 1e3 / ms}
 
 
-def run_extras(ctx, dev, stream, peaks):
+def run_extras(ctx, dev, stream, peaks, outputs):
     """configs[3] (Llama-2-13B 2048-token prefill) and configs[2] (Llama-2-7B-shaped W8A8 decoder layer) on this GPU, CUDA events."""
     out = {}
     try:
         from tools.prefill_bench import prefill_once
 
-        out["prefill_13b_2048"] = prefill_once(ctx, dev, stream, "llama2-13b", 2048, peaks)
+        out["prefill_13b_2048"] = prefill_once(ctx, dev, stream, "llama2-13b", 2048, peaks, logits_out=(lg := []))
+        outputs["prefill_13b_2048_logits"] = lg[0].numpy()
     except Exception as ex:  # a secondary number must never hide the headline
         out["prefill_13b_2048"] = {"error": repr(ex)}
     try:
@@ -538,13 +543,14 @@ def run_ours(args):
             torch.cuda.synchronize(dev)
 
         def fill_cache(m, g):
-            # random-filled KV cache so every context length is "already generated"
+            # random-filled KV cache so every context length is "already generated" (seeded: the same fill in every run)
+            torch.manual_seed(4321)
             for l in range(g.num_layers):
                 m.kv_cache(l, 0).normal_(0, 0.5)
                 m.kv_cache(l, 1).normal_(0, 0.5)
 
         def timed(m, vocab_local):
-            """(device-resident ms, host entry point ms, clocks) over the K timed steps of model m"""
+            """(device-resident ms, host entry point ms, clocks, outputs of the last timed step) over the K timed steps of model m"""
             tokpos_all = torch.tensor(list(zip(toks, pos_list)), dtype=torch.int32, device=dev)
             tokpos = torch.zeros(2, dtype=torch.int32, device=dev)
             logits_pinned = torch.empty(vocab_local, dtype=torch.float32).pin_memory()
@@ -561,16 +567,19 @@ def run_ours(args):
                 e1.record(stream)
                 barrier()
             ms_dev = e0.elapsed_time(e1)
+            outputs = {"logits": m.logits().float().cpu().numpy()}
             for i in range(W):
                 m.decode_host(toks[i], pos_list[i], logits_pinned)
             barrier()
             e2, e3 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e2.record(stream)
             for i in range(W, W + K):
-                m.decode_host(toks[i], pos_list[i], logits_pinned)
+                nxt = m.decode_host(toks[i], pos_list[i], logits_pinned)
             e3.record(stream)
             barrier()
-            return ms_dev, e2.elapsed_time(e3), clk.summary()
+            outputs["logits_host"] = logits_pinned.numpy().copy()
+            outputs["next_token_host"] = [float(nxt)]
+            return ms_dev, e2.elapsed_time(e3), clk.summary(), outputs
 
         if tp:
             # tensor-parallel decode of ONE sequence: every rank generates the same full weights (same seed) and keeps its 1/N shard
@@ -600,10 +609,10 @@ def run_ours(args):
                 extra["tp_parity_rel_err"] = parity
                 extra["tp_parity_note"] = "max |logits_tp - logits_1gpu| / max |logits_1gpu| over 4 decode steps of the same weights (rank 0 runs the single-GPU model)"
             fill_cache(model, gl)
-            ms_dev, ms_e2e, clocks = timed(model, gl.vocab_size)
+            ms_dev, ms_e2e, clocks, outputs = timed(model, gl.vocab_size)
             if args.replicas_too:
                 fill_cache(single, geom)
-                r_dev, _, _ = timed(single, geom.vocab_size)
+                r_dev, _, _, _ = timed(single, geom.vocab_size)
                 rt = torch.tensor([r_dev], dtype=torch.float64, device=dev)
                 dist.all_reduce(rt, op=dist.ReduceOp.MAX)
                 extra["replicas_tok_s"] = world * K / (rt.item() * 1e-3)
@@ -614,7 +623,7 @@ def run_ours(args):
             gl = geom
             model = LL.LlamaModel(ctx, geom, max_ctx=args.max_ctx, seed=1234 + rank)
             fill_cache(model, geom)
-            ms_dev, ms_e2e, clocks = timed(model, geom.vocab_size)
+            ms_dev, ms_e2e, clocks, outputs = timed(model, geom.vocab_size)
             vocab_local = geom.vocab_size
         kernels_per_step = model.kernels_per_step
         if rank == 0 and world == 1 and not args.no_extras:
@@ -625,7 +634,7 @@ def run_ours(args):
                 extra["gpu_reference"] = {"error": repr(ex)}
         model.close()
         if rank == 0 and world == 1 and not args.no_extras:
-            extra.update(run_extras(ctx, dev, stream, peaks))
+            extra.update(run_extras(ctx, dev, stream, peaks, outputs))
         if world > 1 and not args.no_extras:
             # configs[3] at N GPUs.  The prompt pass is tensor-bound and a 2048-token prompt of the 13B model fits one GPU, so it scales as N
             # independent prompts (data parallel, no collective on the data path): aggregate = N x FLOPs / the slowest rank's time.
@@ -673,7 +682,7 @@ def run_ours(args):
             "data": "synthetic",
             "config": workload_config(geom, args, world, tp),
             "mean_ctx": mean_ctx,
-            "l2": "inputs larger than L2: 3.9 GB of weights stream per step vs 126 MB L2",
+            "l2": "inputs larger than L2: 3.9 GB of weights stream per step vs 50 MB L2",
             "clocks": clocks,
             "e2e": {"value": e2e_tok_s, "unit": UNIT, "h2d_bytes_per_step": 12, "d2h_bytes_per_step": vocab_local * 4 + 4},
             "gpu_launches": K * kernels_per_step,
@@ -709,6 +718,13 @@ def run_ours(args):
                             line["extra"][key]["cpu_baseline"] = fn()
                         except Exception as ex:
                             line["extra"][key]["cpu_baseline"] = {"error": repr(ex)}
+        if args.dump_outputs:
+            import numpy as np
+
+            out_dir = Path(args.dump_outputs)
+            out_dir.mkdir(parents=True, exist_ok=True)
+            for name, arr in outputs.items():  # rank 0's view: under tensor parallelism its vocabulary shard
+                np.save(out_dir / f"{name}.npy", np.asarray(arr, dtype=np.float32))
         print(json.dumps(line), flush=True)
     ctx.close()
     if world > 1:
@@ -719,7 +735,7 @@ def run_ours(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=128)
+    ap.add_argument("--steps", type=int, default=None, help="timed steps (default 128; 8 with --impl reference)")
     ap.add_argument("--warmup", type=int, default=8)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--model", default="llama3-8b")
@@ -732,6 +748,7 @@ def main():
     # N > 1 default = tensor-parallel decode of ONE sequence (BASELINE config 5, strong scaling); "replicas" = one independent batch-1
     # sequence per GPU (no data-path collective, weak scaling), also reported as `replicas_tok_s` beside the tensor-parallel value
     ap.add_argument("--parallel", default="tp", choices=["tp", "replicas"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
     ap.add_argument("--no-replicas", dest="replicas_too", action="store_false", help="N>1 tp: skip the secondary replicas measurement")
     args = ap.parse_args()
     if args.warmup < 3:
@@ -739,9 +756,13 @@ def main():
     if args.probe_threads:
         probe_threads(args)
         return
+    if args.steps is None:
+        args.steps = 8 if args.impl == "reference" else 128  # a full token costs seconds on the host: keep the default invocation within minutes
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
-        if args.steps == 128:
-            args.steps = 8  # a full token costs seconds on the host: keep the default invocation within minutes
+        if args.dump_outputs:
+            ap.error("--dump-outputs belongs to the CUDA path; the reference arm times the host kernels only")
         run_reference(args)
     else:
         run_ours(args)

@@ -1,5 +1,5 @@
 /*
- * tce_b200.h -- C ABI of libtce_b200.so: the B200 (sm_100a) implementation of TinyChatEngine's quantized-linear
+ * tce_b200.h -- C ABI of libtce_b200.so: the H100 (sm_90a) implementation of TinyChatEngine's quantized-linear
  * hot path (W4A16 AWQ GEMV/GEMM, W8A8 SmoothQuant GEMM, per-token KV-cache attention).
  *
  * Boundary contract (SURVEY.md 8(b)): plain pointers and sizes, no C++/torch types.  Every data pointer is a
@@ -180,7 +180,7 @@ TCE_API int tce_llama_decode_host(tce_llama *m, int token, int pos, float *logit
 /* Prompt processing (the reference's Int4LlamaForCausalLM::forward with sqlen = n > 1, cuda/Int4llamaForCausalLM.cu:20-47): n host
  * token ids at positions pos0..pos0+n-1 in one pass -- KV cache rows written, logits of the LAST position (the only row the
  * sampler reads, LLaMAGenerate.cu:160-166) copied to logits_host (may be NULL), greedy token to next_token (may be NULL).
- * Linears run as tcgen05 GEMMs, attention as a causal flash kernel.  Synchronous.  Single GPU (tp_size == 1).                */
+ * Linears run as wgmma GEMMs, attention as a causal flash kernel.  Synchronous.  Single GPU (tp_size == 1).                */
 TCE_API int tce_llama_prefill(tce_llama *m, const int *tokens_host, int n, int pos0, float *logits_host, int *next_token);
 /* ---- sampling + generate loop on the device (SURVEY.md 8(f)3) -------------------------------------------------------------
  * The reference copies n_vocab logits to the host every token and samples there (llm/src/nn_modules/cuda/LLaMAGenerate.cu:112-166 with

@@ -223,7 +223,7 @@ _REF_CUDA = None
 
 
 def ref_cuda():
-    """oracle/_ref/libtce_ref_cuda.so: the reference's own kernels/cuda/gemv_cuda.cu compiled for sm_100a (GPU-side baseline and
+    """oracle/_ref/libtce_ref_cuda.so: the reference's own kernels/cuda/gemv_cuda.cu compiled for sm_90a (GPU-side baseline and
     second oracle).  Takes raw DEVICE pointers; launches on the legacy default stream like the reference."""
     global _REF_CUDA
     if _REF_CUDA is None:

@@ -1,6 +1,6 @@
 // ref_cuda_shim.cu -- TEST / BENCH INFRASTRUCTURE ONLY.  Thin entry into the reference's own CUDA GEMV so that it can run on the same
-// B200 as a GPU-side baseline and as a second oracle (SURVEY.md 8(c), 8(d) config 2: "the reference gemv_kernel_g128 compiled for
-// sm_100a as reference CUDA on this box").  oracle/Makefile compiles /root/reference/kernels/cuda/gemv_cuda.cu where it lies, unchanged,
+// GPU as a GPU-side baseline and as a second oracle (SURVEY.md 8(c), 8(d) config 2: "the reference gemv_kernel_g128 compiled for
+// sm_90a as reference CUDA on the same GPU").  oracle/Makefile compiles /root/reference/kernels/cuda/gemv_cuda.cu where it lies, unchanged,
 // next to this file; nothing of the reference is copied.  The only code here fills `matmul_params` exactly like the reference call
 // site Linear_half_int4::forward (llm/src/ops/cuda/linear.cu:20-33) and calls MatmulOperator::gemv_forward_cuda.
 #include <cuda_runtime.h>

@@ -12,7 +12,7 @@ GOLDEN = Path(__file__).resolve().parent / "golden"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "slow: bigger CPU cases (still part of the default CPU suite)")
 
 
@@ -25,7 +25,7 @@ def pytest_collection_modifyitems(config, items):
         has_gpu = False
     if has_gpu:
         return
-    skip = pytest.mark.skip(reason="no CUDA device in this container")
+    skip = pytest.mark.skip(reason="no CUDA device")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

@@ -1,5 +1,5 @@
 """bench.py's CPU legs (the reference's own kernels timed beside the GPU numbers) run on any host: shapes of what they return, bounded run time.
-The GPU arm itself needs a B200 (tests/test_gpu_*.py); the reference arm under torchrun is covered by tests/test_dist_gloo.py."""
+The GPU arm itself needs an H100 (tests/test_gpu_*.py); the reference arm under torchrun is covered by tests/test_dist_gloo.py."""
 import importlib.util
 import json
 import time

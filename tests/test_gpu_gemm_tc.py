@@ -1,4 +1,4 @@
-"""The tcgen05 GEMMs (large-M slots of the path) on the GPU.
+"""The wgmma GEMMs (large-M slots of the path) on the GPU.
 W4A16 prefill slot (tce_w4a16_gemm, M >= 16): vs the CPU oracle, <= 1e-2 relative (contract) and the 2e-3 internal bar.
 W8A8 (tce_w8a8_matmul, M >= 16, K % 128 == 0): BIT-EXACT vs the oracle, and identical to the DP4A kernel."""
 import numpy as np
@@ -79,5 +79,5 @@ def test_w8a8_tc_bit_exact(ctx, M, N, K):
     want = [capi.int8_matmul(0, A, B, b8, None, ALPHA, BETA, -128, 127), capi.int8_matmul(0, A, B, b8, None, ALPHA, BETA, 0, 127),
             capi.int8_matmul(2, A, B, alpha=ALPHA), capi.int8_matmul(4, A, B, biasf=bf, alpha=ALPHA), capi.int8_matmul(6, A, B, alpha=ALPHA)]
     for i, (t, d, w_) in enumerate(zip(tc, dp, want)):
-        assert np.array_equal(t, w_), f"tcgen05 variant #{i}"
+        assert np.array_equal(t, w_), f"wgmma variant #{i}"
         assert np.array_equal(d, w_), f"dp4a variant #{i}"

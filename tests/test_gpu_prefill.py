@@ -1,4 +1,4 @@
-"""Prompt processing (tce_llama_prefill: tcgen05 GEMMs + causal flash attention) vs the oracle-composed decode steps, vs the
+"""Prompt processing (tce_llama_prefill: wgmma GEMMs + causal flash attention) vs the oracle-composed decode steps, vs the
 decode path on the same weights, and chunked against one-shot."""
 import numpy as np
 import pytest

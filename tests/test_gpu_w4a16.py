@@ -120,7 +120,7 @@ def test_gemv_tiny_and_mixed_magnitudes(ctx):
 
 @pytest.mark.parametrize("oc,ic", [(4096, 4096), (1024, 14336), (11008, 4096)])
 def test_reference_cuda_kernel_on_this_gpu(ctx, oc, ic):
-    """The reference's own gemv_kernel_g128 (kernels/cuda/gemv_cuda.cu:140-194), compiled unchanged for sm_100a (oracle/_ref), on the
+    """The reference's own gemv_kernel_g128 (kernels/cuda/gemv_cuda.cu:140-194), compiled unchanged for sm_90a (oracle/_ref), on the
     same device buffers: a second, independent oracle on the GPU.  Its arithmetic is fp32 FMA of exactly converted fp16 inputs."""
     from oracle import capi
 

@@ -1,6 +1,6 @@
 """CPU: the drop-in matmul.h keeps the reference's struct layout (field order / offsets) so reference call sites
-link against it unchanged.  Checked by compiling a probe against both headers when /root/reference is present,
-else against recorded offsets."""
+link against it unchanged.  Checked by compiling a probe against this header and comparing with the sizes and offsets the
+same probe printed for the reference's kernels/matmul.h (-DQM_CUDA), stored in tests/golden/matmul_h_layout.txt."""
 import subprocess
 import tempfile
 from pathlib import Path
@@ -33,8 +33,6 @@ def probe(header: str, extra):
 
 def test_struct_layout_matches_reference():
     ours = probe(str(ROOT / "tinychatengine_b200/host/matmul.h"), [])
-    ref_h = Path("/root/reference/kernels/matmul.h")
-    if ref_h.exists():
-        ref = probe(str(ref_h), ["-DQM_CUDA", "-I/root/reference/llm/half-2.2.0/include"])
-        assert ours == ref, (ours, ref)
+    ref = (ROOT / "tests" / "golden" / "matmul_h_layout.txt").read_text().strip()
+    assert ours == ref, (ours, ref)
     assert len(ours.split()) == 16

@@ -3,7 +3,7 @@
 exact integer dot products with the nibbles -> one fp32 FMA per group.  The model restates that arithmetic in numpy with the SAME integer widths and checks,
 without a GPU, the properties DESIGN.md 4.1 claims: the digits reconstruct X, nothing overflows 32 bits at the extreme inputs, and the result stays inside
 the parity contract (<= 1e-2 per element wherever |y| > 1e-3 max|y|, SURVEY.md 8(d) config 1) on the heavy-tailed activations that broke round 1's 15-bit
-scheme (VERDICT.md, What's weak 3).  The CUDA kernel itself is checked against the oracle on the same cases in tests/test_gpu_w4a16.py; this file guards
+scheme.  The CUDA kernel itself is checked against the oracle on the same cases in tests/test_gpu_w4a16.py; this file guards
 the DESIGN of the number format."""
 import numpy as np
 import pytest

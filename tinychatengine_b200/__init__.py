@@ -1,4 +1,4 @@
-"""tinychatengine_b200 -- B200 (sm_100a) implementation of TinyChatEngine's quantized-linear hot path.
+"""tinychatengine_b200 -- H100 (sm_90a) implementation of TinyChatEngine's quantized-linear hot path.
 
 The product is ``lib/libtce_b200.so`` (hand-written CUDA behind the C ABI in ``include/tce_b200.h``); this
 package is the thin host layer: the ctypes binding (:mod:`._lib`), the reference's on-disk INT4 formats

@@ -88,7 +88,7 @@ def lib() -> C.CDLL:
     global _lib
     if _lib is None:
         if not Path(LIB).exists():
-            raise TceError(f"{LIB} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_100a). "
+            raise TceError(f"{LIB} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a). "
                            "tinychatengine_b200 has no CPU fallback.")
         L = C.CDLL(str(LIB))
         for name, (res, args) in SIGNATURES.items():

@@ -1,4 +1,4 @@
-"""In-tree build of libtce_b200.so (nvcc, sm_100a only)."""
+"""In-tree build of libtce_b200.so (nvcc, sm_90a only)."""
 from __future__ import annotations
 
 import os
@@ -10,7 +10,7 @@ LIB = PKG / "lib" / "libtce_b200.so"
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every CUDA source of the package for sm_100a (cross-compiles without a GPU)."""
+    """Compile every CUDA source of the package for sm_90a (cross-compiles without a GPU)."""
     if force:
         subprocess.run(["make", "-C", str(PKG / "csrc"), "clean"], check=True, capture_output=not verbose)
     jobs = str(max(1, min(8, os.cpu_count() or 1)))

@@ -1,4 +1,4 @@
-// attention.cu -- per-token KV-cache attention for decode (fp16 cache, GQA aware) on sm_100a.
+// attention.cu -- per-token KV-cache attention for decode (fp16 cache, GQA aware) on sm_90a.
 //
 // Replaces the attention part of Int4llamaAttention::forward between qkv_proj and o_proj
 // (reference llm/src/nn_modules/cuda/Int4llamaAttention.cu:128-217: shape_qkv -> RotaryPosEmb_cuda_forward ->

@@ -1,5 +1,5 @@
 // capi.cu -- extern "C" surface of libtce_b200.so (include/tce_b200.h): argument checking, context and
-// workspace management, dispatch to the sm_100a kernels.  No CPU fallback anywhere in this file.
+// workspace management, dispatch to the sm_90a kernels.  No CPU fallback anywhere in this file.
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -69,7 +69,7 @@ int tce_ctx_create(int device, tce_ctx **out) {
     CK(cudaSetDevice(device), "cudaSetDevice");
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties");
-    if (prop.major < 10) return fail(TCE_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+    if (prop.major != 9) return fail(TCE_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
     tce_ctx *ctx = new tce_ctx();
     Ctx &c = ctx->c;
     c.device = device;
@@ -79,10 +79,10 @@ int tce_ctx_create(int device, tce_ctx **out) {
     c.gemv_impl = env_int("TCE_GEMV_IMPL", 1);
     c.gemv_ctas_per_sm = env_int("TCE_GEMV_CTAS_PER_SM", 1);
     c.gemv_consumer_warps = env_int("TCE_GEMV_CONSUMER_WARPS", 8);  // 8, 16, or 0 = per shape (16 for long rows: faster alone, not in the step)
-    c.gemv_stages = env_int("TCE_GEMV_STAGES", 8);  // 8 vs 4: +3 % on the decode step once the consumers outran HBM (profiles/README.md)
+    c.gemv_stages = env_int("TCE_GEMV_STAGES", 8);  // deep ring: the consumers outrun HBM on the decode step
     c.pdl_early = env_int("TCE_PDL_EARLY", 1);
-    c.use_pdl = env_int("TCE_USE_PDL", 1) != 0;  // programmatic dependent launch, dependents resident from kernel entry: +3 % (profiles/r01_pdl_matrix.txt)
-    ctx->attn_chunk = env_int("TCE_ATTN_CHUNK", 256);  // cached rows per CTA: 256 measured best (64: -8 %, 128: -2 %; profiles/README.md)
+    c.use_pdl = env_int("TCE_USE_PDL", 1) != 0;  // programmatic dependent launch, dependents resident from kernel entry
+    ctx->attn_chunk = env_int("TCE_ATTN_CHUNK", 256);  // cached rows per CTA
     c.gemv_max_ctas = c.num_sms * 4;
     c.gemv_max_tiles = 32768;
     c.attn_ws_bytes = (size_t)128 * 1024 * 130 * sizeof(float);  // heads * splits * (128 + 2): 128 heads x 1024 splits
@@ -160,7 +160,7 @@ int tce_ctx_set_option(tce_ctx *ctx, const char *name, int value) {
         }
     } else if (!strcmp(name, "use_pdl"))
         ctx->c.use_pdl = value != 0;
-    else if (!strcmp(name, "gemm_min_m"))  // smallest M served by the tcgen05 GEMMs (W4A16 prefill slot, W8A8); below it the weight-streaming kernels run
+    else if (!strcmp(name, "gemm_min_m"))  // smallest M served by the wgmma GEMMs (W4A16 prefill slot, W8A8); below it the weight-streaming kernels run
         ctx->c.gemm_min_m = value < 1 ? 1 : value;
     else if (!strcmp(name, "attn_cluster"))
         (void)value;  // accepted and ignored: the cluster flavour of the stand-alone decode attention was removed (measured slower)
@@ -286,7 +286,7 @@ int tce_w8a8_matmul(tce_ctx *ctx, int variant, int batch, const void *A, const v
     a.variant = variant;
     a.batch = batch ? 1 : 0;
     if (!a.batch && M >= ctx->c.gemm_min_m && K % 128 == 0 && !(((uintptr_t)A | (uintptr_t)B | (uintptr_t)C) & 15)) {
-        CK(launch_w8a8_tc(&ctx->c, a), "tce_w8a8_matmul (tcgen05)");
+        CK(launch_w8a8_tc(&ctx->c, a), "tce_w8a8_matmul (wgmma)");
         return TCE_OK;
     }
     CK(launch_w8a8_dp4a(&ctx->c, a), "tce_w8a8_matmul");

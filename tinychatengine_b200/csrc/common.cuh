@@ -1,4 +1,4 @@
-// common.cuh -- device-side building blocks shared by the sm_100a kernels of libtce_b200.
+// common.cuh -- device-side building blocks shared by the sm_90a kernels of libtce_b200.
 // Raw PTX wrappers only (mbarrier, bulk async copy = TMA 1-D, mma.sync, PDL); no CUTLASS, no Triton.
 #pragma once
 #include <cuda.h>

@@ -1,4 +1,4 @@
-// decode_persistent.cu -- one persistent cooperative kernel per decoded token (Llama, AWQ-INT4, batch 1) on sm_100a.
+// decode_persistent.cu -- one persistent cooperative kernel per decoded token (Llama, AWQ-INT4, batch 1) on sm_90a.
 //
 // Call sites restated (reference, CUDA build): Int4LlamaForCausalLM::forward (cuda/Int4llamaForCausalLM.cu:17-50) ->
 // Int4llamaDecoder::forward (cuda/Int4llamaDecoder.cu:57-112) -> 32 x Int4llamaDecoderLayer::forward (cuda/Int4llamaDecoderLayer.cu:73-115)
@@ -66,7 +66,7 @@ TCE_DEVINL uint2 ld_ll1(const uint2 *p, bool sys) {
     return r;
 }
 // A failed poll waits this long before it asks L2 again: thousands of threads spinning without a pause fill the L2 request queues and
-// stretch every round trip (their own and the producers' stores) to ~0.5 us (profiles/README.md, run 11).
+// stretch every round trip (their own and the producers' stores).
 __constant__ unsigned g_poll_ns = 100;  // TCE_PK_POLL_NS (set_poll_backoff)
 #define kPollBackoffNs g_poll_ns
 constexpr long long kSpinLimit = 20000000000LL;  // ~10 s: a peer rank may legitimately start its kernel later
@@ -297,8 +297,7 @@ TCE_DEVINL AttnSplit attn_split(int cta, int ncta, int KVH, int pos) {
 // ------------------------------------------------------------------------------------------------------------ producer
 // The same walk over (tile, stage, box) serves two warps: the loader (PF = false) moves stages into the ring as slots free up; the
 // prefetcher (PF = true) runs `kPrefetchAhead` stages ahead of it and only asks L2 for the same boxes, so that the bytes in flight
-// towards HBM are not bounded by the ring (4 x 32 KiB per SM x ~3 us loaded HBM latency = ~40 GB/s per SM, the ceiling measured without
-// it, profiles/README.md) and a ring slot waits one L2 round trip instead of one DRAM round trip.
+// towards HBM are not bounded by the ring (4 x 32 KiB per SM per loaded HBM round trip) and a ring slot waits one L2 round trip instead of one DRAM round trip.
 constexpr int kPrefetchAhead = 10;
 struct ProdState {
     Ring rs;
@@ -477,7 +476,7 @@ TCE_DEVINL void rx_wait(const PSmem &sm, PairCtx &pc) {
 }
 
 // ------------------------------------------------------------------------------------------------------------ consumers: staging
-// unit rotation: CTA c starts its walk over the input vector `rot` groups further on, so that the 148 CTAs do not all pull the same
+// unit rotation: CTA c starts its walk over the input vector `rot` groups further on, so that the CTAs do not all pull the same
 // L2 lines at the same moment.  Whole groups (16 units) keep the half-warp amax shuffles of emit_unit intact.
 TCE_DEVINL int rot_unit(int u, int units, int cta) {
     const int ng = units >> 4;
@@ -725,7 +724,7 @@ TCE_DEVINL void locate(const BoxPlan &pl, int gi, int g, int t, uint32_t &off, u
 
 // Fast path for dense boxes of 16 groups (NG >= 16: every Llama width): within a stage every operand address is a per-lane constant
 // plus the slot base, and the second unit of a warp sits at fixed distances (+16 KiB weights, +4 KiB planes, +512 B scales ...), so the
-// inner loop carries almost no address arithmetic (the ALU pipe is what bounds this loop, profiles/README.md).
+// inner loop carries almost no address arithmetic (the ALU pipe is what bounds this loop).
 TCE_DEVINL void consume_gemv_dense(const GemvOp &op, const PSmem &sm, Ring &rs, Red &cs, float inv, int cta, int ncta, int cw, int lane) {
     const int g = lane >> 2, t = lane & 3;
     int t0, t1;
@@ -1363,7 +1362,7 @@ BoxPlan make_box_plan(int n, int *widths, int *nwidths) {
     BoxPlan pl{};
     int w[kMaxBoxes], nb = 0;
     // Dense boxes of up to 16 groups.  (Odd widths -- 9+9+7+7 -- make the weight LDS.128 conflict free, but rows of 576 / 448 bytes are
-    // not multiples of the 128-byte L2 line: measured 25 % SLOWER end to end, profiles/README.md; kept selectable for the record.)
+    // not multiples of the 128-byte L2 line: slower end to end when last measured; kept selectable.)
     const bool odd = getenv("TCE_PK_ODD_BOXES") != nullptr;
     if (!odd) {
         w[nb++] = n < 16 ? n : 16;

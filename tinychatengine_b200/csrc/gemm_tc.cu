@@ -1,9 +1,9 @@
-// gemm_tc.cu -- instantiations of the tcgen05 GEMM for the two large-M slots of the path:
+// gemm_tc.cu -- instantiations of the wgmma GEMM for the two large-M slots of the path:
 //   * W4A16 prefill (MatmulOperator::gemm_forward_cuda, declared-but-undefined in the reference, kernels/matmul.h:142-145): the
 //     QM_CUDA int4 weights are expanded once per call to fp16 ((q - z) * s, one rounding) into an L2-resident scratch by a
-//     bandwidth-bound kernel, then C = X * W16^T runs on the tensor cores with fp32 accumulation in TMEM.  Expanding once per call
+//     bandwidth-bound kernel, then C = X * W16^T runs on the tensor cores with fp32 accumulation.  Expanding once per call
 //     instead of once per M tile keeps the CUDA-core dequant work at OC*IC instead of OC*IC*ceil(M/128).
-//   * W8A8 (mat_mul_accelerator_int8_fast_2x2_32unroll* at M >= 16, kernels/ref/matmul_ref_int8.cc:11-159): tcgen05 kind::i8 with
+//   * W8A8 (mat_mul_accelerator_int8_fast_2x2_32unroll* at M >= 16, kernels/ref/matmul_ref_int8.cc:11-159): wgmma s8 x s8 with
 //     int32 accumulation is exact, the float epilogue keeps the reference's evaluation order -> bit-identical int8 / fp32 outputs.
 #include "gemm_tc.cuh"
 #include "kernels.h"
@@ -12,84 +12,29 @@
 namespace tce {
 namespace {
 
+using tc::EpiAddF32;
+using tc::EpiHalf;
 using tc::GemmArgs;
 
 // ------------------------------------------------------------------------------------------------ epilogues
-struct EpiHalf {  // fp32 accumulator -> fp16 C
-    TCE_DEVINL static void apply(const GemmArgs &a, int row, int col0, int n, const uint32_t (&v)[32]) {
-        __half *dst = reinterpret_cast<__half *>(a.C) + (size_t)row * a.ldc + col0;
-        if (n == 32 && (a.ldc & 7) == 0) {
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                uint4 o;
-                o.x = pack_half2(__uint_as_float(v[8 * i + 0]), __uint_as_float(v[8 * i + 1]));
-                o.y = pack_half2(__uint_as_float(v[8 * i + 2]), __uint_as_float(v[8 * i + 3]));
-                o.z = pack_half2(__uint_as_float(v[8 * i + 4]), __uint_as_float(v[8 * i + 5]));
-                o.w = pack_half2(__uint_as_float(v[8 * i + 6]), __uint_as_float(v[8 * i + 7]));
-                reinterpret_cast<uint4 *>(dst)[i] = o;
-            }
-        } else {
-#pragma unroll
-            for (int i = 0; i < 32; i++)
-                if (i < n) dst[i] = __float2half_rn(__uint_as_float(v[i]));
-        }
-    }
-};
-
-struct EpiAddF32 {  // fp32 accumulator added into an fp32 C (residual stream)
-    TCE_DEVINL static void apply(const GemmArgs &a, int row, int col0, int n, const uint32_t (&v)[32]) {
-        float *dst = reinterpret_cast<float *>(a.C) + (size_t)row * a.ldc + col0;
-        if (n == 32 && (a.ldc & 3) == 0) {
-#pragma unroll
-            for (int i = 0; i < 8; i++) {
-                float4 c = reinterpret_cast<float4 *>(dst)[i];
-                c.x += __uint_as_float(v[4 * i + 0]);
-                c.y += __uint_as_float(v[4 * i + 1]);
-                c.z += __uint_as_float(v[4 * i + 2]);
-                c.w += __uint_as_float(v[4 * i + 3]);
-                reinterpret_cast<float4 *>(dst)[i] = c;
-            }
-        } else {
-#pragma unroll
-            for (int i = 0; i < 32; i++)
-                if (i < n) dst[i] += __uint_as_float(v[i]);
-        }
-    }
-};
-
 template <int VARIANT>
 struct EpiW8 {  // int32 accumulator -> the four W8A8 epilogues (same float op order as w8a8.cu / kernels/ref)
-    TCE_DEVINL static void apply(const GemmArgs &a, int row, int col0, int n, const uint32_t (&v)[32]) {
-        const size_t o = (size_t)row * a.ldc + col0;
-        if constexpr (VARIANT == W8_BIAS8_O8 || VARIANT == W8_NOBIAS_O8) {
-            int8_t *dst = reinterpret_cast<int8_t *>(a.C) + o;
-            uint32_t packed[8];
+    static constexpr bool kSilu = false;
+    TCE_DEVINL static void apply(const GemmArgs &a, int row, int col, int v0, int v1) {
+        const size_t o = (size_t)row * a.ldc + col;
+        const int v[2] = {v0, v1};
 #pragma unroll
-            for (int i = 0; i < 32; i++) {
-                float f = __fmul_rn((float)(int)v[i], a.alpha);
-                if constexpr (VARIANT == W8_BIAS8_O8) f = __fadd_rn(f, __fmul_rn((float)(i < n ? a.bias8[col0 + i] : (int8_t)0), a.beta));
+        for (int i = 0; i < 2; i++) {
+            if (col + i >= a.N) break;
+            float f = __fmul_rn((float)v[i], a.alpha);
+            if constexpr (VARIANT == W8_BIAS8_O8 || VARIANT == W8_NOBIAS_O8) {
+                if constexpr (VARIANT == W8_BIAS8_O8) f = __fadd_rn(f, __fmul_rn((float)a.bias8[col + i], a.beta));
                 int qv = (int)roundf(f);
                 qv = min(max(qv, a.q_min), a.q_max);
-                if ((i & 3) == 0) packed[i >> 2] = 0;
-                packed[i >> 2] |= (uint32_t)(qv & 0xff) << (8 * (i & 3));
-            }
-            if (n == 32 && (a.ldc & 15) == 0) {
-                reinterpret_cast<uint4 *>(dst)[0] = make_uint4(packed[0], packed[1], packed[2], packed[3]);
-                reinterpret_cast<uint4 *>(dst)[1] = make_uint4(packed[4], packed[5], packed[6], packed[7]);
+                reinterpret_cast<int8_t *>(a.C)[o + i] = (int8_t)qv;
             } else {
-#pragma unroll
-                for (int i = 0; i < 32; i++)
-                    if (i < n) dst[i] = (int8_t)((packed[i >> 2] >> (8 * (i & 3))) & 0xff);
-            }
-        } else {
-            float *dst = reinterpret_cast<float *>(a.C) + o;
-#pragma unroll
-            for (int i = 0; i < 32; i++) {
-                if (i < n) {
-                    float f = __fmul_rn((float)(int)v[i], a.alpha);
-                    if constexpr (VARIANT == W8_BIASF_OF32) f = __fadd_rn(f, a.biasf[col0 + i]);
-                    dst[i] = f;
-                }
+                if constexpr (VARIANT == W8_BIASF_OF32) f = __fadd_rn(f, a.biasf[col + i]);
+                reinterpret_cast<float *>(a.C)[o + i] = f;
             }
         }
     }
@@ -121,60 +66,25 @@ __global__ void w4_expand_kernel(const uint32_t *__restrict__ w, const uint32_t 
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
-                             const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-cudaError_t encode_kmajor(CUtensorMap *out, const void *base, bool i8, long long rows, long long K, long long ld_elems, int box_rows) {
-    static EncodeFn fn = nullptr;
-    if (!fn) {
-        void *sym = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &q);
-        if (e != cudaSuccess || !sym) return e != cudaSuccess ? e : cudaErrorNotSupported;
-        fn = reinterpret_cast<EncodeFn>(sym);
-    }
-    const int es = i8 ? 1 : 2;
-    const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-    const cuuint64_t gstride[1] = {(cuuint64_t)(ld_elems * es)};
-    const cuuint32_t box[2] = {(cuuint32_t)(tc::kAtomBytes / es), (cuuint32_t)box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = fn(out, i8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void *>(base), gdim, gstride, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
-}
-
 template <int BLOCK_N, int STAGES, bool I8, class Epi>
 cudaError_t launch(Ctx *ctx, GemmArgs &a, const void *A, long long lda, const void *B, long long ldb, long long K) {
-    cudaError_t e = encode_kmajor(&a.tmA, A, I8, a.M, K, lda, tc::kBlockM);
+    cudaError_t e = tc::encode_kmajor(&a.tmA, A, I8, a.M, K, lda, tc::kBlockM);
     if (e != cudaSuccess) return e;
-    e = encode_kmajor(&a.tmB, B, I8, a.N, K, ldb, BLOCK_N);
+    e = tc::encode_kmajor(&a.tmB, B, I8, a.N, K, ldb, BLOCK_N / 2);
     if (e != cudaSuccess) return e;
     a.k_blocks = (int)(K * (I8 ? 1 : 2) / tc::kAtomBytes);
-    a.m_blocks = (a.M + tc::kBlockM - 1) / tc::kBlockM;
-    a.n_blocks = (a.N + BLOCK_N - 1) / BLOCK_N;
-    auto kern = tc::gemm_tc_kernel<BLOCK_N, STAGES, I8, Epi>;
-    constexpr size_t smem = tc::smem_bytes<BLOCK_N, STAGES>();
-    static DeviceOnce attr_once;  // per instantiation
-    if (attr_once.pending(ctx->device)) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        attr_once.done(ctx->device);
-    }
-    const int tiles = a.m_blocks * a.n_blocks;
-    const int grid = tiles < ctx->num_sms ? tiles : ctx->num_sms;
-    kern<<<grid, tc::kThreads, smem, ctx->stream>>>(a);
-    return cudaGetLastError();
+    return tc::launch_wg<BLOCK_N, STAGES, I8, false, 1, Epi>(ctx, a);
 }
 
 // Tile width by wave quantisation: a persistent grid of `sms` CTAs needs ceil(tiles / sms) rounds, each costing ~BLOCK_N (the MMA
-// time of one tile) times a small penalty for the narrower tiles (the 128-row A tile is re-read once per N block).
+// time of one tile) times a penalty for the narrower tile (the 128-row A tile is re-read once per N block); the 1.12 is a guess, not measured on H100.
 int pick_block_n(int M, int N, int sms) {
     const long long mb = (M + 127) / 128;
-    const int bn[3] = {256, 192, 128};
-    const double pen[3] = {1.00, 1.04, 1.12};
+    const int bn[2] = {256, 128};
+    const double pen[2] = {1.00, 1.12};
     int best = 256;
     double best_cost = 1e30;
-    for (int i = 0; i < 3; i++) {
+    for (int i = 0; i < 2; i++) {
         const long long tiles = mb * ((N + bn[i] - 1) / bn[i]);
         const double cost = (double)((tiles + sms - 1) / sms) * bn[i] * pen[i];
         if (cost < best_cost) {
@@ -187,11 +97,8 @@ int pick_block_n(int M, int N, int sms) {
 
 template <class Epi, bool I8>
 cudaError_t dispatch(Ctx *ctx, GemmArgs &a, const void *A, long long lda, const void *B, long long ldb, long long K) {
-    switch (pick_block_n(a.M, a.N, ctx->num_sms)) {
-        case 256: return launch<256, 4, I8, Epi>(ctx, a, A, lda, B, ldb, K);
-        case 192: return launch<192, 5, I8, Epi>(ctx, a, A, lda, B, ldb, K);
-        default: return launch<128, 6, I8, Epi>(ctx, a, A, lda, B, ldb, K);
-    }
+    if (pick_block_n(a.M, a.N, ctx->num_sms) == 256) return launch<256, 4, I8, Epi>(ctx, a, A, lda, B, ldb, K);
+    return launch<128, 6, I8, Epi>(ctx, a, A, lda, B, ldb, K);
 }
 
 }  // namespace

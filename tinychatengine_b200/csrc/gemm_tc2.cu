@@ -1,17 +1,9 @@
-// gemm_tc2.cu -- the prefill GEMM on CTA pairs:  C[M][N] = X[M][K] (fp16) * W[N][K]^T, tcgen05.mma.cta_group::2.
+// gemm_tc2.cu -- the prefill GEMM on CTA pairs:  C[M][N] = X[M][K] (fp16) * W[N][K]^T, the CL = 2 instantiations of gemm_tc.cuh.
 //
-// Two CTAs of a cluster (one TPC) own one 256 x 256 output tile.  Each CTA stages ITS 128 activation rows and ITS 128 weight rows of
-// every 64-k block; one thread of the leader CTA issues M = 256 MMAs that read both CTAs' shared memory, so per CTA and k-block the
-// tensor core pulls 32 KiB of operands for 128 x 256 x 64 MACs -- half of what a single-CTA 128 x 256 tile needs, which is what bounds
-// the single-CTA kernel (gemm_tc.cuh): there the operand reads + TMA writes (+ dequant traffic when fused) exceed the 128 B/clk of one SM's
-// shared memory long before the tensor pipe is busy (profiles/README.md, round 2).
-//
-// FUSED = false: W is fp16 (the expanded scratch): both operands arrive by TMA (cta_group::2 flavour: completion bytes are counted on the
-//                leader's mbarrier).
-// FUSED = true:  W is the packed QM_CUDA int4 matrix: each CTA's TMA brings 128 rows x 32 bytes of nibbles per k-block, four dequant warps turn
-//                them into the fp16 K-major SWIZZLE_128B operand tile ((q - z) * s, exact subtraction, one rounding), fence.proxy.async, and
-//                arrive on the LEADER's barrier (remote arrive from the peer).  Nothing but the nibbles crosses HBM for the weights.
-// Epilogue: every CTA reads its own 128 accumulator rows from its own TMEM (double-buffered accumulators), fp16 store or fp32 accumulate.
+// Two CTAs of a cluster own two vertically adjacent 128-row tiles of the same N block; each fetches half of the weight rows of every 64-k
+// block and multicasts them to both (see gemm_tc.cuh, CL = 2).  W is fp16 (the expanded scratch) or packed QM_CUDA int4 (dequantised by
+// each CTA's own warps).  SiLU variant: W = [gate (F rows); up (F rows)]; tile columns 0..127 are 128 channels of gate (fetched by CTA 0),
+// 128..255 the same channels of up (CTA 1), so a thread holds both accumulators of a channel and writes act = SiLU(gate) * up.
 #include <cstdlib>
 #include <string>
 
@@ -19,443 +11,30 @@
 #include "kernels.h"
 
 namespace tce {
+
+cudaError_t fill_w4_gemm_args(tc::GemmArgs &a, const __half *X, long long ldx, const uint32_t *w, const uint32_t *zeros, const __half *scales, void *C, long long ldc,
+                              int M, int N, int K);  // gemm_w4_tc.cu
+
 namespace {
 
-using namespace tc;
+using tc::GemmArgs;
 
-constexpr int kPairN = 256;                 // output columns per tile (each CTA stages half of the weight rows)
-constexpr int kHalfN = 128;
-constexpr int kBHalfBytes = kHalfN * 128;   // 16 KiB fp16 operand tile per CTA and k-block
-constexpr int kRawHalf = kHalfN * 32;       // 4 KiB of packed nibbles
-constexpr int kDq = 4;                      // dequant warps per k-block and CTA (FUSED): one thread per weight row
-constexpr int kDqGroups = 2;                // groups of kDq warps working on alternate k-blocks (hides the per-block barrier / fence latencies)
-constexpr uint32_t kPeerMask = 0xFEFFFFFFu; // clears the CTA-rank bit of a shared::cluster address: "the same location in CTA 0"
-constexpr uint64_t kEvictNormal = 0x1000000000000000ull;
-
-template <bool FUSED>
-struct Cfg {
-    static constexpr int kAStages = 6;               // ring of activation tiles (not FUSED: + this CTA's fp16 weight tile in the same slot)
-    static constexpr int kOpStages = FUSED ? 4 : 0;  // ring of dequantised operand tiles
-    static constexpr int kRawStages = FUSED ? 12 : 0;  // ring of packed weight tiles: its own, deeper ring -- 4 KiB per k-block buys the look-ahead
-                                                       // that hides the load latency in front of the dequant warps (a shared 5-slot ring left the
-                                                       // tensor pipe at 42 %: a slot was only re-requested after its MMA had retired)
-    static constexpr int kSlotBytes = kABytes + (FUSED ? 0 : kBHalfBytes);
-    static constexpr int kThreads = 32 * (6 + (FUSED ? kDq * kDqGroups + 1 : 0));  // FUSED: + one warp that loads the packed tiles
-    static constexpr size_t kSmem = 1024 + (size_t)kAStages * kSlotBytes + (size_t)kOpStages * kBHalfBytes + (size_t)kRawStages * kRawHalf;
+struct EpiSiluMul {  // act[M][F] = SiLU(gate) * up (SiLuMul_half, llm/src/nn_modules/cuda/Int4llamaDecoderLayer.cu:12-30; fp32 math)
+    static constexpr bool kSilu = true;
+    TCE_DEVINL static void apply(const GemmArgs &a, int row, int col, float g0, float g1, float u0, float u1) {
+        __half *dst = reinterpret_cast<__half *>(a.C) + (size_t)row * a.ldc + col;  // F % 128 == 0, ldc % 8 == 0: both columns exist, 4-byte aligned
+        *reinterpret_cast<uint32_t *>(dst) = pack_half2((g0 / (1.f + __expf(-g0))) * u0, (g1 / (1.f + __expf(-g1))) * u1);
+    }
 };
 
-struct PairArgs {
-    alignas(64) CUtensorMap tmA;  // fp16 [M][K], box {64, 128}, SWIZZLE_128B
-    alignas(64) CUtensorMap tmB;  // FUSED: uint32 [N][K/8], box {8, 128}, no swizzle; else fp16 [N][K], box {64, 128}, SWIZZLE_128B
-    const __half *scales;
-    const uint32_t *zeros;
-    int sf_w, zeros_w;
-    int M, N, k_blocks, m_blocks, n_blocks;  // blocks of 256
-    void *C;
-    long long ldc;
-    int add_f32;
-    int pn;      // output columns per tile of the fp16-weight kernel: 256, or 128 where 256-wide tiles quantise badly onto the 74 clusters (N = 5120:
-                 // 160 tiles = 2.16 waves); each CTA stages pn / 2 weight rows.  The fused and SiLU variants use 256.
-    int silu_F;  // > 0: W = [gate (F rows); up (F rows)], the pair's two halves are the SAME 128 channels of gate (CTA 0) and up (CTA 1), and the
-                 // epilogue writes act[M][F] = SiLU(gate) * up (SiLuMul_half, llm/src/nn_modules/cuda/Int4llamaDecoderLayer.cu:12-30; fp32 math)
-};
-
-TCE_DEVINL uint32_t cluster_rank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-TCE_DEVINL uint32_t cluster_id_x() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
-    return r;
-}
-TCE_DEVINL uint32_t num_clusters_x() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
-    return r;
-}
-TCE_DEVINL void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster
-TCE_DEVINL void mbar_arrive_cluster(uint64_t *bar, uint32_t rank) {
-    uint32_t remote;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
-    // default semantics (release at CTA scope), as for a local arrive: the operand tile was already published to the async proxy by
-    // fence.proxy.async; a cluster-scope release costs MEMBAR.ALL.GPU + ERRBAR per arrive and halved the kernel (profiles/README.md)
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-// wait on a barrier whose arrivals come from both CTAs (plain try_wait: an acquire.cluster wait invalidates L1 on every poll)
-TCE_DEVINL void mbar_wait_cl(uint64_t *bar, uint32_t parity) {
-    const long long t0 = clock64();
-    while (true) {
-        uint32_t ok;
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(ok)
-                     : "r"(smem_u32(bar)), "r"(parity)
-                     : "memory");
-        if (ok) return;
-        if (clock64() - t0 > 6000000000LL) __trap();  // a protocol bug surfaces as a launch failure, not as a hung GPU
-    }
-}
-// TMA load whose completion bytes are counted on the LEADER's barrier (same offset in CTA 0); the data lands in this CTA
-TCE_DEVINL void tma_load_2d_pair(void *dst_smem, const void *tmap, int x, int y, uint64_t *bar) {
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3}], [%4], %5;" ::"r"(
-                     smem_u32(dst_smem)),
-                 "l"(tmap), "r"(x), "r"(y), "r"(smem_u32(bar) & kPeerMask), "l"(kEvictNormal)
-                 : "memory");
-}
-TCE_DEVINL void tmem_alloc_pair(uint32_t *dst_smem, uint32_t ncols) {  // the same warp of BOTH CTAs
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-TCE_DEVINL void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// all MMAs issued so far by this thread complete -> one arrival on `bar` in BOTH CTAs
-TCE_DEVINL void umma_commit_pair(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)), "h"((unsigned short)3)
-                 : "memory");
-}
-TCE_DEVINL void umma_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc),
-                 "r"(idesc), "r"(accumulate)
-                 : "memory");
-}
-
-TCE_DEVINL uint32_t lop3_and_or2(uint32_t a, uint32_t b, uint32_t c) {
-    uint32_t r;
-    asm("lop3.b32 %0, %1, %2, %3, 0xEA;" : "=r"(r) : "r"(a), "r"(b), "r"(c));
-    return r;
-}
-TCE_DEVINL uint4 dequant_word2(uint32_t w, uint32_t zmagic, __half2 s2) {  // 8 nibbles -> 8 fp16 (q - z) * s in k order
-    constexpr uint32_t Mk = 0x000F000Fu, MG = 0x64006400u;
-    const __half2 zm = *reinterpret_cast<const __half2 *>(&zmagic);
-    uint32_t q[4] = {lop3_and_or2(w, Mk, MG), lop3_and_or2(w >> 4, Mk, MG), lop3_and_or2(w >> 8, Mk, MG), lop3_and_or2(w >> 12, Mk, MG)};
-    uint32_t p[4];
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        const __half2 v = __hmul2(__hsub2(*reinterpret_cast<const __half2 *>(&q[i]), zm), s2);
-        p[i] = *reinterpret_cast<const uint32_t *>(&v);
-    }
-    return make_uint4(__byte_perm(p[0], p[1], 0x5410), __byte_perm(p[2], p[3], 0x5410), __byte_perm(p[0], p[1], 0x7632), __byte_perm(p[2], p[3], 0x7632));
-}
-
-template <bool FUSED>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(Cfg<FUSED>::kThreads, 1) gemm_pair_kernel(const __grid_constant__ PairArgs a) {
-    using C = Cfg<FUSED>;
-    constexpr int AS = C::kAStages, OS = FUSED ? C::kOpStages : 1, RS = FUSED ? C::kRawStages : 1;
-    extern __shared__ uint8_t smem_raw[];
-    // barriers live at identical offsets in both CTAs (multicast commits and remote arrives address "the same barrier in the other CTA")
-    __shared__ __align__(8) uint64_t a_full[AS], a_empty[AS], raw_full[RS], raw_empty[RS], op_full[OS], op_empty[OS], tfull_bar[2], tempty_bar[2];
-    __shared__ uint32_t tmem_base_s;
-    const uint32_t raw = smem_u32(smem_raw);
-    uint8_t *base = smem_raw + (((raw + 1023u) & ~1023u) - raw);
-    uint8_t *sSlot = base;                                    // [AS][A 16 KiB (| B half fp16 16 KiB when not FUSED)]
-    uint8_t *sOp = base + (size_t)AS * C::kSlotBytes;         // FUSED: [OS][16 KiB] dequantised operand tiles
-    uint8_t *sRaw = sOp + (size_t)(FUSED ? OS : 0) * kBHalfBytes;  // FUSED: [RS][4 KiB] packed tiles
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_rank();
-    const bool leader = rank == 0;
-    const int tiles_total = a.m_blocks * a.n_blocks;
-    const int cl = (int)cluster_id_x(), ncl = (int)num_clusters_x();
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < AS; s++) {
-            mbar_init(&a_full[s], 1);                          // leader: its own expect_tx arrival; bytes from both CTAs
-            mbar_init(&a_empty[s], 1);                         // multicast MMA commit
-        }
-        for (int s = 0; s < RS; s++) {
-            mbar_init(&raw_full[s], 1);                        // FUSED: this CTA's packed tile (local TMA)
-            mbar_init(&raw_empty[s], kDq);                     // the dequant warps of the group that owns the k-block
-        }
-        for (int s = 0; s < OS; s++) {
-            mbar_init(&op_full[s], 2 * kDq);                   // leader: dequant warps of both CTAs
-            mbar_init(&op_empty[s], 1);                        // multicast MMA commit
-        }
-        for (int s = 0; s < 2; s++) {
-            mbar_init(&tfull_bar[s], 1);                       // multicast MMA commit
-            mbar_init(&tempty_bar[s], 256);                    // leader: the epilogue threads of both CTAs
-        }
-        mbar_fence_init();
-    }
-    cluster_sync_all();  // barriers of both CTAs exist before anyone signals across
-    if (warp == 1) tmem_alloc_pair(&tmem_base_s, 512);
-    tc_fence_before();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_s;
-
-    if (warp == 0) {
-        // ------------------------------------------------------------------------------- TMA producer (both CTAs)
-        if (lane == 0) {
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&a.tmA) : "memory");
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&a.tmB) : "memory");
-            int s = 0;
-            uint32_t ph = 0;
-            for (int t = cl; t < tiles_total; t += ncl) {
-                const int mb = t % a.m_blocks, nb = t / a.m_blocks;
-                const int row0 = mb * 256 + (int)rank * kBlockM;
-                const int pn = FUSED ? kPairN : a.pn, hn = pn >> 1;
-                const int wrow0 = a.silu_F > 0 ? nb * kHalfN + (int)rank * a.silu_F : nb * pn + (int)rank * hn;
-                for (int kb = 0; kb < a.k_blocks; kb++) {
-                    mbar_wait(&a_empty[s], ph ^ 1u);
-                    uint8_t *dst = sSlot + (size_t)s * C::kSlotBytes;
-                    if (FUSED) {
-                        if (leader) mbar_arrive_expect_tx(&a_full[s], 2 * kABytes);
-                        tma_load_2d_pair(dst, &a.tmA, kb * 64, row0, &a_full[s]);
-                    } else {
-                        if (leader) mbar_arrive_expect_tx(&a_full[s], 2 * (kABytes + hn * 128));
-                        tma_load_2d_pair(dst, &a.tmA, kb * 64, row0, &a_full[s]);
-                        tma_load_2d_pair(dst + kABytes, &a.tmB, kb * 64, wrow0, &a_full[s]);
-                    }
-                    if (++s == AS) {
-                        s = 0;
-                        ph ^= 1u;
-                    }
-                }
-            }
-        }
-        __syncwarp();
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------------------- MMA issuer (leader CTA only)
-        if (leader && lane == 0) {
-            const uint32_t idesc = (1u << 4) | ((uint32_t)((FUSED ? kPairN : a.pn) >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);  // F32 acc, f16 x f16, K-major, N, M 256
-            int s = 0, os = 0, it = 0;
-            uint32_t ph = 0, oph = 0;
-            for (int t = cl; t < tiles_total; t += ncl, it++) {
-                const int acc = it & 1;
-                const uint32_t acc_ph = (uint32_t)(it >> 1) & 1u;
-                mbar_wait_cl(&tempty_bar[acc], acc_ph ^ 1u);
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(acc * kPairN);
-                for (int kb = 0; kb < a.k_blocks; kb++) {
-                    mbar_wait(&a_full[s], ph);
-                    if (FUSED) mbar_wait_cl(&op_full[os], oph);
-                    tc_fence_after();
-                    const uint64_t adesc = make_sw128_desc(smem_u32(sSlot + (size_t)s * C::kSlotBytes));
-                    const uint64_t bdesc = make_sw128_desc(FUSED ? smem_u32(sOp + (size_t)os * kBHalfBytes) : smem_u32(sSlot + (size_t)s * C::kSlotBytes + kABytes));
-#pragma unroll
-                    for (int k = 0; k < 4; k++) umma_pair(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (kb | k) != 0 ? 1u : 0u);
-                    umma_commit_pair(&a_empty[s]);
-                    if (FUSED) umma_commit_pair(&op_empty[os]);
-                    if (++s == AS) {
-                        s = 0;
-                        ph ^= 1u;
-                    }
-                    if (FUSED && ++os == OS) {
-                        os = 0;
-                        oph ^= 1u;
-                    }
-                }
-                umma_commit_pair(&tfull_bar[acc]);
-            }
-        }
-        __syncwarp();
-    } else if (warp < 6) {
-        // ------------------------------------------------------------------------------- epilogue (both CTAs, own accumulator rows)
-        const int q = warp & 3;
-        int it = 0;
-        for (int t = cl; t < tiles_total; t += ncl, it++) {
-            const int mb = t % a.m_blocks, nb = t / a.m_blocks;
-            const int acc = it & 1;
-            const uint32_t acc_ph = (uint32_t)(it >> 1) & 1u;
-            mbar_wait(&tfull_bar[acc], acc_ph);
-            tc_fence_after();
-            const int row = mb * 256 + (int)rank * kBlockM + q * 32 + lane;
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * kPairN);
-            if (a.silu_F > 0) {
-                // accumulator columns 0..127 = gate, 128..255 = up of output channels nb * 128 ..: act = SiLU(gate) * up
-#pragma unroll 1
-                for (int c = 0; c < kHalfN / 32; c++) {
-                    uint32_t g[32], u[32];
-                    tmem_ld32(taddr + (uint32_t)(c * 32), g);
-                    tmem_ld32(taddr + (uint32_t)(kHalfN + c * 32), u);
-                    tmem_ld_wait();
-                    const int col0 = nb * kHalfN + c * 32;
-                    if (row < a.M && col0 < a.silu_F) {
-                        __half *dst = reinterpret_cast<__half *>(a.C) + (size_t)row * a.ldc + col0;
-                        uint32_t o[16];
-#pragma unroll
-                        for (int i = 0; i < 16; i++) {
-                            const float g0 = __uint_as_float(g[2 * i]), g1 = __uint_as_float(g[2 * i + 1]);
-                            o[i] = pack_half2((g0 / (1.f + __expf(-g0))) * __uint_as_float(u[2 * i]), (g1 / (1.f + __expf(-g1))) * __uint_as_float(u[2 * i + 1]));
-                        }
-#pragma unroll
-                        for (int i = 0; i < 4; i++) reinterpret_cast<uint4 *>(dst)[i] = make_uint4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]);
-                    }
-                }
-                tc_fence_before();
-                mbar_arrive_cluster(&tempty_bar[acc], 0);
-                continue;
-            }
-            const int pn = FUSED ? kPairN : a.pn;
-#pragma unroll 1
-            for (int c = 0; c < pn / 32; c++) {
-                uint32_t v[32];
-                tmem_ld32(taddr + (uint32_t)(c * 32), v);
-                tmem_ld_wait();
-                const int col0 = nb * pn + c * 32;
-                if (row < a.M && col0 < a.N) {
-                    const int n = min(32, a.N - col0);
-                    if (a.add_f32) {
-                        float *dst = reinterpret_cast<float *>(a.C) + (size_t)row * a.ldc + col0;
-                        if (n == 32 && (a.ldc & 3) == 0) {
-#pragma unroll
-                            for (int i = 0; i < 8; i++) {
-                                float4 cc = reinterpret_cast<float4 *>(dst)[i];
-                                cc.x += __uint_as_float(v[4 * i + 0]);
-                                cc.y += __uint_as_float(v[4 * i + 1]);
-                                cc.z += __uint_as_float(v[4 * i + 2]);
-                                cc.w += __uint_as_float(v[4 * i + 3]);
-                                reinterpret_cast<float4 *>(dst)[i] = cc;
-                            }
-                        } else {
-#pragma unroll
-                            for (int i = 0; i < 32; i++)
-                                if (i < n) dst[i] += __uint_as_float(v[i]);
-                        }
-                    } else {
-                        __half *dst = reinterpret_cast<__half *>(a.C) + (size_t)row * a.ldc + col0;
-                        if (n == 32 && (a.ldc & 7) == 0) {
-#pragma unroll
-                            for (int i = 0; i < 4; i++) {
-                                uint4 o;
-                                o.x = pack_half2(__uint_as_float(v[8 * i + 0]), __uint_as_float(v[8 * i + 1]));
-                                o.y = pack_half2(__uint_as_float(v[8 * i + 2]), __uint_as_float(v[8 * i + 3]));
-                                o.z = pack_half2(__uint_as_float(v[8 * i + 4]), __uint_as_float(v[8 * i + 5]));
-                                o.w = pack_half2(__uint_as_float(v[8 * i + 6]), __uint_as_float(v[8 * i + 7]));
-                                reinterpret_cast<uint4 *>(dst)[i] = o;
-                            }
-                        } else {
-#pragma unroll
-                            for (int i = 0; i < 32; i++)
-                                if (i < n) dst[i] = __float2half_rn(__uint_as_float(v[i]));
-                        }
-                    }
-                }
-            }
-            tc_fence_before();
-            mbar_arrive_cluster(&tempty_bar[acc], 0);  // the leader's MMA thread may overwrite this accumulator (in both CTAs)
-        }
-    } else if (FUSED && warp == 6 + kDq * kDqGroups) {
-        // ------------------------------------------------------------------------------- packed-weight producer (both CTAs, local barriers)
-        if (lane == 0) {
-            int s = 0;
-            uint32_t ph = 0;
-            for (int t = cl; t < tiles_total; t += ncl) {
-                const int nb = t / a.m_blocks;
-                const int wrow0 = nb * kPairN + (int)rank * kHalfN;
-                for (int kb = 0; kb < a.k_blocks; kb++) {
-                    mbar_wait(&raw_empty[s], ph ^ 1u);
-                    mbar_arrive_expect_tx(&raw_full[s], kRawHalf);
-                    tma_load_2d(sRaw + (size_t)s * kRawHalf, &a.tmB, kb * 8, wrow0, &raw_full[s]);
-                    if (++s == RS) {
-                        s = 0;
-                        ph ^= 1u;
-                    }
-                }
-            }
-        }
-        __syncwarp();
-    } else if (FUSED) {
-        // ------------------------------------------------------------------------------- dequant warps: thread r owns weight row r of this CTA's half;
-        // group `grp` takes the k-blocks kb = grp (mod kDqGroups).  K % 128 == 0 makes k_blocks even, so a group sees the same half of every
-        // 128-k scale group in every tile.
-        const int dt = threadIdx.x - 32 * 6;
-        const int r = dt & (kHalfN - 1), grp = dt >> 7;
-        const uint32_t row_off = (uint32_t)(r >> 3) * 1024u + (uint32_t)(r & 7) * 128u;
-        const uint32_t sw = (uint32_t)(r & 7);
-        long long kbase = 0;  // k-blocks of the tiles processed so far: ring slot = (kbase + kb) % depth
-        for (int t = cl; t < tiles_total; t += ncl) {
-            const int nb = t / a.m_blocks;
-            const int grow = nb * kPairN + (int)rank * kHalfN + r;
-            const bool live = grow < a.N;
-            const __half *srow = a.scales + (size_t)(live ? grow : 0) * a.sf_w;
-            const uint32_t *zrow = a.zeros + (size_t)(live ? grow : 0) * a.zeros_w;
-            // scale / zero point of a 128-k group are requested one group before they are used (an L2 round trip on this critical path otherwise)
-            const int ngroups = a.k_blocks >> 1;
-            uint32_t zword = 0u, zword_nxt = live ? zrow[0] : 0u;
-            __half s_nxt = live ? srow[0] : __float2half(0.f);
-            for (int kb = grp; kb < a.k_blocks; kb += kDqGroups) {
-                const int g = kb >> 1;  // kDqGroups == 2: every iteration of a group is a new scale group
-                if ((g & 7) == 0) {
-                    zword = zword_nxt;
-                    if (live && g + 8 < ngroups) zword_nxt = zrow[(g >> 3) + 1];
-                }
-                const uint32_t z = (zword >> (4 * (g & 7))) & 0xFu;
-                const uint32_t zmagic = 0x64006400u | z | (z << 16);
-                const __half2 s2 = __half2half2(s_nxt);
-                if (live && g + 1 < ngroups) s_nxt = srow[g + 1];
-                const long long kk = kbase + kb;
-                const int s = (int)(kk % RS), os = (int)(kk % OS);
-                const uint32_t ph = (uint32_t)((kk / RS) & 1), oph = (uint32_t)((kk / OS) & 1);
-                mbar_wait(&raw_full[s], ph);
-                const uint8_t *src = sRaw + (size_t)s * kRawHalf + (size_t)r * 32;
-                const uint4 w0 = *reinterpret_cast<const uint4 *>(src), w1 = *reinterpret_cast<const uint4 *>(src + 16);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&raw_empty[s]);  // the packed tile is in registers
-                const uint32_t ww[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
-                uint4 o[8];
-#pragma unroll
-                for (int c = 0; c < 8; c++) o[c] = dequant_word2(ww[c], zmagic, s2);
-                mbar_wait(&op_empty[os], oph ^ 1u);
-                uint8_t *dst = sOp + (size_t)os * kBHalfBytes + row_off;
-#pragma unroll
-                for (int c = 0; c < 8; c++) *reinterpret_cast<uint4 *>(dst + (((uint32_t)c ^ sw) << 4)) = o[c];
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(&op_full[os], 0);
-            }
-            kbase += a.k_blocks;
-        }
-    }
-    tc_fence_before();
-    cluster_sync_all();  // both CTAs are done with TMEM and with each other's shared memory
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc_pair(tmem_base, 512);
-    }
-}
-
-typedef CUresult (*EncodeFn2)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
-                              const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeFn2 encoder2() {
-    static EncodeFn2 fn = nullptr;
-    if (!fn) {
-        void *sym = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &q) == cudaSuccess && sym) fn = reinterpret_cast<EncodeFn2>(sym);
-    }
-    return fn;
-}
-
-bool encode_f16(CUtensorMap *out, const void *base, long long rows, long long K, long long ld, int box_rows = 128) {
-    const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-    const cuuint64_t gstride[1] = {(cuuint64_t)(ld * 2)};
-    const cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    return encoder2()(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void *>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-template <bool FUSED>
-cudaError_t launch_pair(Ctx *ctx, PairArgs &a) {
-    using C = Cfg<FUSED>;
-    auto kern = gemm_pair_kernel<FUSED>;
-    static DeviceOnce attr_once;
-    if (attr_once.pending(ctx->device)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::kSmem);
-        if (e != cudaSuccess) return e;
-        attr_once.done(ctx->device);
-    }
-    const int tiles = a.m_blocks * a.n_blocks;
-    int clusters = ctx->num_sms / 2;
-    if (clusters > tiles) clusters = tiles;
-    kern<<<2 * clusters, C::kThreads, C::kSmem, ctx->stream>>>(a);
-    return cudaGetLastError();
+cudaError_t fill_f16(GemmArgs &a, const __half *X, long long ldx, const __half *W, long long ldw, long long w_rows, int box_rows, int M, int K) {
+    cudaError_t e = tc::encode_kmajor(&a.tmA, X, false, M, K, ldx, tc::kBlockM);
+    if (e != cudaSuccess) return e;
+    e = tc::encode_kmajor(&a.tmB, W, false, w_rows, K, ldw, box_rows);
+    if (e != cudaSuccess) return e;
+    a.M = M;
+    a.k_blocks = K / 64;
+    return cudaSuccess;
 }
 
 }  // namespace
@@ -463,7 +42,7 @@ cudaError_t launch_pair(Ctx *ctx, PairArgs &a) {
 int w4_gemm_mode() {
     static const int mode = [] {
         const char *e = getenv("TCE_W4_GEMM");
-        if (!e) return (int)W4G_PAIR_OVERLAP;  // measured best on B200 (profiles/README.md): CTA-pair GEMM, expansion of the next linear overlapped
+        if (!e) return (int)W4G_PAIR_OVERLAP;  // CTA-pair GEMM, expansion of the next linear overlapped
         const std::string v(e);
         if (v == "fused") return (int)W4G_FUSED;
         if (v == "pair") return (int)W4G_PAIR;
@@ -477,75 +56,50 @@ int w4_gemm_mode() {
 
 // W fp16 [N][K] (ldw elements between rows)
 cudaError_t launch_gemm_f16_pair(Ctx *ctx, const __half *X, long long ldx, const __half *W, long long ldw, void *C, long long ldc, int M, int N, int K, int add_f32) {
-    if (M < 1 || N < 1 || K < 64 || (K % 64) || (ldx % 8) || (ldw % 8) || !encoder2()) return cudaErrorInvalidValue;
-    PairArgs a = {};
-    a.M = M;
-    a.N = N;
-    a.k_blocks = K / 64;
-    a.m_blocks = (M + 255) / 256;
-    // tile width by wave quantisation over the clusters: rounds x width (x a small penalty for the narrower tile: the activation tile is re-read per N block)
+    if (M < 1 || N < 1 || K < 64 || (K % 64) || (ldx % 8) || (ldw % 8)) return cudaErrorInvalidValue;
+    // tile width by wave quantisation over the clusters: rounds x width (x a penalty for the narrower tile, the activation tile being re-read per N block: 1.12 is a guess, not measured on H100)
     const int clusters = ctx->num_sms / 2;
+    const long long mb = (M + 255) / 256;
     auto cost = [&](int pn, double pen) {
-        const long long tiles = (long long)a.m_blocks * ((N + pn - 1) / pn);
+        const long long tiles = mb * ((N + pn - 1) / pn);
         return (double)((tiles + clusters - 1) / clusters) * pn * pen;
     };
-    // measured: 128-wide tiles run at 0.70 of the 256-wide rate per FLOP (the activation tile is read twice as often from shared memory), which
-    // costs more than the wave quantisation it removes (13B o / down: 919 / 973 -> 640 / 673 TFLOP/s): a penalty of 1.45 keeps them for tiny N only
-    a.pn = cost(128, 1.45) < cost(256, 1.0) ? 128 : 256;
-    if (!encode_f16(&a.tmA, X, M, K, ldx) || !encode_f16(&a.tmB, W, N, K, ldw, a.pn / 2)) return cudaErrorInvalidValue;
-    a.n_blocks = (N + a.pn - 1) / a.pn;
+    const int pn = cost(128, 1.12) < cost(256, 1.0) ? 128 : 256;
+    GemmArgs a = {};
+    cudaError_t e = fill_f16(a, X, ldx, W, ldw, N, pn / 2, M, K);
+    if (e != cudaSuccess) return e;
+    a.N = N;
     a.C = C;
     a.ldc = ldc;
-    a.add_f32 = add_f32;
-    return launch_pair<false>(ctx, a);
+    if (pn == 256) {
+        if (add_f32) return tc::launch_wg<256, 4, false, false, 2, tc::EpiAddF32>(ctx, a);
+        return tc::launch_wg<256, 4, false, false, 2, tc::EpiHalf>(ctx, a);
+    }
+    if (add_f32) return tc::launch_wg<128, 6, false, false, 2, tc::EpiAddF32>(ctx, a);
+    return tc::launch_wg<128, 6, false, false, 2, tc::EpiHalf>(ctx, a);
 }
 
 // act[M][F] = SiLU(X Wg^T) * (X Wu^T), W = fp16 [2F][K] with the gate rows first; F % 128 == 0, ldc % 8 == 0
 cudaError_t launch_gemm_f16_pair_silu(Ctx *ctx, const __half *X, long long ldx, const __half *W, long long ldw, __half *act, long long ldc, int M, int F, int K) {
-    if (M < 1 || F < 128 || (F % kHalfN) || K < 64 || (K % 64) || (ldx % 8) || (ldw % 8) || (ldc % 8) || !encoder2()) return cudaErrorInvalidValue;
-    PairArgs a = {};
-    if (!encode_f16(&a.tmA, X, M, K, ldx) || !encode_f16(&a.tmB, W, 2LL * F, K, ldw)) return cudaErrorInvalidValue;
-    a.M = M;
+    if (M < 1 || F < 128 || (F % 128) || K < 64 || (K % 64) || (ldx % 8) || (ldw % 8) || (ldc % 8)) return cudaErrorInvalidValue;
+    GemmArgs a = {};
+    cudaError_t e = fill_f16(a, X, ldx, W, ldw, 2LL * F, 128, M, K);
+    if (e != cudaSuccess) return e;
     a.N = F;
-    a.k_blocks = K / 64;
-    a.m_blocks = (M + 255) / 256;
-    a.n_blocks = F / kHalfN;
+    a.silu_F = F;
     a.C = act;
     a.ldc = ldc;
-    a.pn = kPairN;
-    a.silu_F = F;
-    return launch_pair<false>(ctx, a);
+    return tc::launch_wg<256, 4, false, false, 2, EpiSiluMul>(ctx, a);
 }
 
 // W packed QM_CUDA int4
 cudaError_t launch_gemm_w4_pair(Ctx *ctx, const __half *X, long long ldx, const uint32_t *w, const uint32_t *zeros, const __half *scales, void *C, long long ldc,
                                 int M, int N, int K, int add_f32) {
-    if (M < 1 || N < 1 || K < 128 || (K % 128) || (ldx % 8) || !encoder2()) return cudaErrorInvalidValue;
-    PairArgs a = {};
-    if (!encode_f16(&a.tmA, X, M, K, ldx)) return cudaErrorInvalidValue;
-    {
-        const cuuint64_t gdim[2] = {(cuuint64_t)(K / 8), (cuuint64_t)N};
-        const cuuint64_t gstride[1] = {(cuuint64_t)(K / 8) * 4};
-        const cuuint32_t box[2] = {8u, (cuuint32_t)kHalfN};
-        const cuuint32_t estr[2] = {1, 1};
-        if (encoder2()(&a.tmB, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, const_cast<uint32_t *>(w), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return cudaErrorInvalidValue;
-    }
-    a.scales = scales;
-    a.zeros = zeros;
-    a.zeros_w = zeros_width(K, kW4Group);
-    a.sf_w = a.zeros_w * 8;
-    a.M = M;
-    a.N = N;
-    a.k_blocks = K / 64;
-    a.m_blocks = (M + 255) / 256;
-    a.n_blocks = (N + kPairN - 1) / kPairN;
-    a.pn = kPairN;
-    a.C = C;
-    a.ldc = ldc;
-    a.add_f32 = add_f32;
-    return launch_pair<true>(ctx, a);
+    GemmArgs a = {};
+    cudaError_t e = fill_w4_gemm_args(a, X, ldx, w, zeros, scales, C, ldc, M, N, K);
+    if (e != cudaSuccess) return e;
+    if (add_f32) return tc::launch_wg<128, 5, false, true, 2, tc::EpiAddF32>(ctx, a);
+    return tc::launch_wg<128, 5, false, true, 2, tc::EpiHalf>(ctx, a);
 }
 
 }  // namespace tce

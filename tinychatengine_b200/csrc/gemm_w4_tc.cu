@@ -2,333 +2,32 @@
 // MatmulOperator::gemm_forward_cuda, kernels/matmul.h:142-145, declared and never defined by the reference).
 //
 //   C[M][N] = X[M][K] (fp16) * dequant(W)[N][K]^T,   W = QM_CUDA int4 (uint32 [N][K/8], 8 sequential nibbles per word; fp16 scale and
-//   4-bit zero per 128-k group), fp32 accumulation in TMEM.
+//   4-bit zero per 128-k group), fp32 accumulation in the wgmma register fragment.
 //
 // Nothing but the packed nibbles ever leaves HBM for the weights (0.5 B per weight + scales, against 4.5 B per weight for an expansion
-// pass to an fp16 scratch followed by a plain GEMM):
-//   warp 0        TMA producer: per k-block (64 k) one 128 x 64 fp16 activation tile (SWIZZLE_128B) and one 256-row x 32-byte tile of
-//                 packed nibbles into a 5-deep ring
-//   warps 6-13    dequant: thread t owns weight row t of the tile; reads its 32 bytes, (q - z) * s in half2 (exact subtraction through the
-//                 1024 + q trick, one rounding in the multiply: the same values w4_expand_kernel / the reference's dequantisation
-//                 gemv_cuda.cu:181-184 produce), and writes the row as 64 fp16 into the K-major SWIZZLE_128B operand layout of a
-//                 3-deep operand ring; fence.proxy.async, then one mbarrier arrival per warp
-//   warp 1        one elected thread issues tcgen05.mma (cta_group::1, 128 x 256 x 16 per instruction) from the two rings through
-//                 shared-memory descriptors; tcgen05.commit releases the ring slots
-//   warps 2-5     epilogue: tcgen05.ld of their TMEM lane quarter, fp32 -> fp16 store or fp32 accumulate (residual), double-buffered
-//                 accumulators so that the epilogue of tile i overlaps the main loop of tile i + 1
+// pass to an fp16 scratch followed by a plain GEMM).  The kernel is the FUSED instantiation of gemm_tc.cuh:
+//   warp 8 = TMA producer (128 x 64 fp16 activation tile + 128 rows x 32 bytes of nibbles per k-block, 5-deep ring); warps 9-12 = dequant
+//   (one thread per weight row, the values w4_expand_kernel / the reference's gemv_cuda.cu:181-184 produce, 3-deep operand ring);
+//   warps 0-7 = two consumer warpgroups (wgmma from both rings, then fp16 store or fp32 residual accumulate from the fragment).
 // Persistent, one CTA per SM, tiles walked m-fastest so that the CTAs running concurrently share weight tiles in L2.
 #include "gemm_tc.cuh"
 #include "kernels.h"
 
 namespace tce {
+
 namespace {
-
-using namespace tc;
-
-constexpr int kBN = 256;                       // weight rows per tile (MMA N)
-constexpr int kLdStages = 5;                   // ring of {activation tile, packed weight tile}
-constexpr int kOpStages = 3;                   // ring of dequantised fp16 weight tiles
-constexpr int kRawBytes = kBN * 32;            // 64 nibbles per row
-constexpr int kLdBytes = kABytes + kRawBytes;  // 24 KiB
-constexpr int kOpBytes = kBN * kAtomBytes;     // 32 KiB
-constexpr int kDqWarps = 8;
-constexpr int kW4Threads = 32 * (6 + kDqWarps);  // 448
-constexpr size_t kW4Smem = 1024 + (size_t)kLdStages * kLdBytes + (size_t)kOpStages * kOpBytes;
-
-struct W4GemmArgs {
-    alignas(64) CUtensorMap tmA;  // fp16 [M][K], box {64, 128}, SWIZZLE_128B
-    alignas(64) CUtensorMap tmW;  // uint32 [N][K/8], box {8, 256}, no swizzle
-    const __half *scales;         // [N][sf_w]
-    const uint32_t *zeros;        // [N][zeros_w]
-    int sf_w, zeros_w;
-    int M, N, k_blocks, m_blocks, n_blocks;
-    void *C;
-    long long ldc;
-    int add_f32;
-};
-
-TCE_DEVINL uint32_t lop3_and_or_(uint32_t a, uint32_t b, uint32_t c) {
-    uint32_t r;
-    asm("lop3.b32 %0, %1, %2, %3, 0xEA;" : "=r"(r) : "r"(a), "r"(b), "r"(c));
-    return r;
-}
-
-// 8 nibbles -> 8 fp16 (q - z) * s in k order
-TCE_DEVINL uint4 dequant_word(uint32_t w, uint32_t zmagic, __half2 s2) {
-    constexpr uint32_t M = 0x000F000Fu, MG = 0x64006400u;
-    const __half2 zm = *reinterpret_cast<const __half2 *>(&zmagic);
-    uint32_t q[4];
-    q[0] = lop3_and_or_(w, M, MG);        // (1024 + e0, 1024 + e4)
-    q[1] = lop3_and_or_(w >> 4, M, MG);   // (e1, e5)
-    q[2] = lop3_and_or_(w >> 8, M, MG);   // (e2, e6)
-    q[3] = lop3_and_or_(w >> 12, M, MG);  // (e3, e7)
-    uint32_t p[4];
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        const __half2 v = __hmul2(__hsub2(*reinterpret_cast<const __half2 *>(&q[i]), zm), s2);  // exact difference, one rounding
-        p[i] = *reinterpret_cast<const uint32_t *>(&v);
-    }
-    uint4 o;
-    o.x = __byte_perm(p[0], p[1], 0x5410);  // (e0, e1)
-    o.y = __byte_perm(p[2], p[3], 0x5410);  // (e2, e3)
-    o.z = __byte_perm(p[0], p[1], 0x7632);  // (e4, e5)
-    o.w = __byte_perm(p[2], p[3], 0x7632);  // (e6, e7)
-    return o;
-}
-
-__global__ void __launch_bounds__(kW4Threads, 1) gemm_w4_tc_kernel(const __grid_constant__ W4GemmArgs a) {
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t ld_full[kLdStages], ld_empty[kLdStages], op_full[kOpStages], op_empty[kOpStages], tfull_bar[2], tempty_bar[2];
-    __shared__ uint32_t tmem_base_s;
-    const uint32_t raw = smem_u32(smem_raw);
-    uint8_t *base = smem_raw + (((raw + 1023u) & ~1023u) - raw);
-    uint8_t *sLd = base;                                   // [kLdStages][A 16 KiB | packed W 8 KiB]
-    uint8_t *sOp = base + (size_t)kLdStages * kLdBytes;    // [kOpStages][32 KiB]
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int tiles_total = a.m_blocks * a.n_blocks;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kLdStages; s++) {
-            mbar_init(&ld_full[s], 1);
-            mbar_init(&ld_empty[s], 1 + kDqWarps);  // the MMA commit + every dequant warp
-        }
-        for (int s = 0; s < kOpStages; s++) {
-            mbar_init(&op_full[s], kDqWarps);
-            mbar_init(&op_empty[s], 1);
-        }
-        for (int s = 0; s < 2; s++) {
-            mbar_init(&tfull_bar[s], 1);
-            mbar_init(&tempty_bar[s], 128);
-        }
-        mbar_fence_init();
-    }
-    if (warp == 1) tmem_alloc(&tmem_base_s, 512);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_s;
-
-    if (warp == 0) {
-        // ------------------------------------------------------------------------------- TMA producer
-        if (lane == 0) {
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&a.tmA) : "memory");
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&a.tmW) : "memory");
-            int s = 0;
-            uint32_t ph = 0;
-            for (int t = blockIdx.x; t < tiles_total; t += gridDim.x) {
-                const int mb = t % a.m_blocks, nb = t / a.m_blocks;
-                for (int kb = 0; kb < a.k_blocks; kb++) {
-                    mbar_wait(&ld_empty[s], ph ^ 1u);
-                    mbar_arrive_expect_tx(&ld_full[s], kLdBytes);
-                    uint8_t *dst = sLd + (size_t)s * kLdBytes;
-                    tma_load_2d(dst, &a.tmA, kb * 64, mb * kBlockM, &ld_full[s]);
-                    tma_load_2d(dst + kABytes, &a.tmW, kb * 8, nb * kBN, &ld_full[s]);
-                    if (++s == kLdStages) {
-                        s = 0;
-                        ph ^= 1u;
-                    }
-                }
-            }
-        }
-        __syncwarp();
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------------------- MMA issuer
-        if (lane == 0) {
-            constexpr uint32_t idesc = make_idesc<kBN, false>();
-            int ls = 0, os = 0, it = 0;
-            uint32_t lph = 0, oph = 0;
-            for (int t = blockIdx.x; t < tiles_total; t += gridDim.x, it++) {
-                const int acc = it & 1;
-                const uint32_t acc_ph = (uint32_t)(it >> 1) & 1u;
-                mbar_wait(&tempty_bar[acc], acc_ph ^ 1u);
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(acc * kBN);
-                for (int kb = 0; kb < a.k_blocks; kb++) {
-                    mbar_wait(&ld_full[ls], lph);  // the activation tile (already observed by the dequant warps)
-                    mbar_wait(&op_full[os], oph);  // the dequantised weight tile
-                    tc_fence_after();
-                    const uint64_t adesc = make_sw128_desc(smem_u32(sLd + (size_t)ls * kLdBytes));
-                    const uint64_t bdesc = make_sw128_desc(smem_u32(sOp + (size_t)os * kOpBytes));
-#pragma unroll
-                    for (int k = 0; k < 4; k++) umma<false>(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (kb | k) != 0 ? 1u : 0u);
-                    umma_commit(&ld_empty[ls]);
-                    umma_commit(&op_empty[os]);
-                    if (++ls == kLdStages) {
-                        ls = 0;
-                        lph ^= 1u;
-                    }
-                    if (++os == kOpStages) {
-                        os = 0;
-                        oph ^= 1u;
-                    }
-                }
-                umma_commit(&tfull_bar[acc]);
-            }
-        }
-        __syncwarp();
-    } else if (warp < 6) {
-        // ------------------------------------------------------------------------------- epilogue
-        const int q = warp & 3;
-        int it = 0;
-        for (int t = blockIdx.x; t < tiles_total; t += gridDim.x, it++) {
-            const int mb = t % a.m_blocks, nb = t / a.m_blocks;
-            const int acc = it & 1;
-            const uint32_t acc_ph = (uint32_t)(it >> 1) & 1u;
-            mbar_wait(&tfull_bar[acc], acc_ph);
-            tc_fence_after();
-            const int row = mb * kBlockM + q * 32 + lane;
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * kBN);
-#pragma unroll 1
-            for (int c = 0; c < kBN / 32; c++) {
-                uint32_t v[32];
-                tmem_ld32(taddr + (uint32_t)(c * 32), v);
-                tmem_ld_wait();
-                const int col0 = nb * kBN + c * 32;
-                if (row < a.M && col0 < a.N) {
-                    const int n = min(32, a.N - col0);
-                    if (a.add_f32) {
-                        float *dst = reinterpret_cast<float *>(a.C) + (size_t)row * a.ldc + col0;
-                        if (n == 32 && (a.ldc & 3) == 0) {
-#pragma unroll
-                            for (int i = 0; i < 8; i++) {
-                                float4 cc = reinterpret_cast<float4 *>(dst)[i];
-                                cc.x += __uint_as_float(v[4 * i + 0]);
-                                cc.y += __uint_as_float(v[4 * i + 1]);
-                                cc.z += __uint_as_float(v[4 * i + 2]);
-                                cc.w += __uint_as_float(v[4 * i + 3]);
-                                reinterpret_cast<float4 *>(dst)[i] = cc;
-                            }
-                        } else {
-                            for (int i = 0; i < n; i++) dst[i] += __uint_as_float(v[i]);
-                        }
-                    } else {
-                        __half *dst = reinterpret_cast<__half *>(a.C) + (size_t)row * a.ldc + col0;
-                        if (n == 32 && (a.ldc & 7) == 0) {
-#pragma unroll
-                            for (int i = 0; i < 4; i++) {
-                                uint4 o;
-                                o.x = pack_half2(__uint_as_float(v[8 * i + 0]), __uint_as_float(v[8 * i + 1]));
-                                o.y = pack_half2(__uint_as_float(v[8 * i + 2]), __uint_as_float(v[8 * i + 3]));
-                                o.z = pack_half2(__uint_as_float(v[8 * i + 4]), __uint_as_float(v[8 * i + 5]));
-                                o.w = pack_half2(__uint_as_float(v[8 * i + 6]), __uint_as_float(v[8 * i + 7]));
-                                reinterpret_cast<uint4 *>(dst)[i] = o;
-                            }
-                        } else {
-                            for (int i = 0; i < n; i++) dst[i] = __float2half_rn(__uint_as_float(v[i]));
-                        }
-                    }
-                }
-            }
-            tc_fence_before();
-            mbar_arrive(&tempty_bar[acc]);
-        }
-    } else {
-        // ------------------------------------------------------------------------------- dequant warps: thread r owns weight row r of the tile
-        const int r = threadIdx.x - 32 * 6;  // 0..255
-        int ls = 0, os = 0;
-        uint32_t lph = 0, oph = 0;
-        // destination of chunk c (8 fp16) of row r inside a 128B-swizzled K-major tile: 8-row groups of 1024 B, chunk index XOR (row & 7)
-        const uint32_t row_off = (uint32_t)(r >> 3) * 1024u + (uint32_t)(r & 7) * 128u;
-        const uint32_t sw = (uint32_t)(r & 7);
-        for (int t = blockIdx.x; t < tiles_total; t += gridDim.x) {
-            const int nb = t / a.m_blocks;
-            const int grow = nb * kBN + r;
-            const bool live = grow < a.N;
-            const __half *srow = a.scales + (size_t)(live ? grow : 0) * a.sf_w;
-            const uint32_t *zrow = a.zeros + (size_t)(live ? grow : 0) * a.zeros_w;
-            // scale / zero point of a 128-k group are requested one group (two k-blocks) before they are used: an L2 round trip per group on
-            // the dequant warps' critical path halves the whole kernel (measured, profiles/README.md)
-            const int ngroups = a.k_blocks >> 1;
-            uint32_t zword = 0u, zword_nxt = live ? zrow[0] : 0u, zmagic = 0x64006400u;
-            __half s_nxt = live ? srow[0] : __float2half(0.f);
-            __half2 s2 = __float2half2_rn(0.f);
-            for (int kb = 0; kb < a.k_blocks; kb++) {
-                if ((kb & 1) == 0) {  // a new group (rows past N: scale 0 -> zero weights)
-                    const int g = kb >> 1;
-                    if ((g & 7) == 0) {
-                        zword = zword_nxt;
-                        if (live && g + 8 < ngroups) zword_nxt = zrow[(g >> 3) + 1];
-                    }
-                    const uint32_t z = (zword >> (4 * (g & 7))) & 0xFu;
-                    zmagic = 0x64006400u | z | (z << 16);
-                    s2 = __half2half2(s_nxt);
-                    if (live && g + 1 < ngroups) s_nxt = srow[g + 1];
-                }
-                mbar_wait(&ld_full[ls], lph);
-                const uint8_t *src = sLd + (size_t)ls * kLdBytes + kABytes + (size_t)r * 32;
-                const uint4 w0 = *reinterpret_cast<const uint4 *>(src), w1 = *reinterpret_cast<const uint4 *>(src + 16);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&ld_empty[ls]);  // the packed tile is in registers
-                if (++ls == kLdStages) {
-                    ls = 0;
-                    lph ^= 1u;
-                }
-                const uint32_t ww[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
-                uint4 o[8];
-#pragma unroll
-                for (int c = 0; c < 8; c++) o[c] = dequant_word(ww[c], zmagic, s2);
-                mbar_wait(&op_empty[os], oph ^ 1u);
-                uint8_t *dst = sOp + (size_t)os * kOpBytes + row_off;
-#pragma unroll
-                for (int c = 0; c < 8; c++) *reinterpret_cast<uint4 *>(dst + (((uint32_t)c ^ sw) << 4)) = o[c];
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes, read by the tensor core (async proxy)
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&op_full[os]);
-                if (++os == kOpStages) {
-                    os = 0;
-                    oph ^= 1u;
-                }
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
-    }
-}
-
-typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
-                             const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeFn encoder() {
-    static EncodeFn fn = nullptr;
-    if (!fn) {
-        void *sym = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &q) == cudaSuccess && sym) fn = reinterpret_cast<EncodeFn>(sym);
-    }
-    return fn;
-}
-
+constexpr int kBN = 128;       // weight rows per tile
+constexpr int kLdStages = 5;   // ring of {activation tile, packed weight tile}
 }  // namespace
 
-// C[M][N] (fp16, or fp32 accumulated into when add_f32) = X[M][K] fp16 * dequant(W)^T; W rows [N], K % 128 == 0, ldx % 8 == 0.
-cudaError_t launch_gemm_w4_tc(Ctx *ctx, const __half *X, long long ldx, const uint32_t *w, const uint32_t *zeros, const __half *scales, void *C,
-                              long long ldc, int M, int N, int K, int add_f32) {
+// shared by the single-CTA and the CTA-pair launch (gemm_tc2.cu)
+cudaError_t fill_w4_gemm_args(tc::GemmArgs &a, const __half *X, long long ldx, const uint32_t *w, const uint32_t *zeros, const __half *scales, void *C, long long ldc,
+                              int M, int N, int K) {
     if (M < 1 || N < 1 || K < 128 || (K % 128) || (ldx % 8)) return cudaErrorInvalidValue;
-    EncodeFn fn = encoder();
-    if (!fn) return cudaErrorNotSupported;
-    W4GemmArgs a = {};
-    {
-        const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)M};
-        const cuuint64_t gstride[1] = {(cuuint64_t)(ldx * 2)};
-        const cuuint32_t box[2] = {64u, (cuuint32_t)kBlockM};
-        const cuuint32_t estr[2] = {1, 1};
-        if (fn(&a.tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half *>(X), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return cudaErrorInvalidValue;
-    }
-    {
-        const cuuint64_t gdim[2] = {(cuuint64_t)(K / 8), (cuuint64_t)N};
-        const cuuint64_t gstride[1] = {(cuuint64_t)(K / 8) * 4};
-        const cuuint32_t box[2] = {8u, (cuuint32_t)kBN};
-        const cuuint32_t estr[2] = {1, 1};
-        if (fn(&a.tmW, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, const_cast<uint32_t *>(w), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return cudaErrorInvalidValue;
-    }
+    cudaError_t e = tc::encode_kmajor(&a.tmA, X, false, M, K, ldx, tc::kBlockM);
+    if (e != cudaSuccess) return e;
+    e = tc::encode_w4_packed(&a.tmB, w, N, K, kBN / 2);
+    if (e != cudaSuccess) return e;
     a.scales = scales;
     a.zeros = zeros;
     a.zeros_w = zeros_width(K, kW4Group);
@@ -336,21 +35,19 @@ cudaError_t launch_gemm_w4_tc(Ctx *ctx, const __half *X, long long ldx, const ui
     a.M = M;
     a.N = N;
     a.k_blocks = K / 64;
-    a.m_blocks = (M + kBlockM - 1) / kBlockM;
-    a.n_blocks = (N + kBN - 1) / kBN;
     a.C = C;
     a.ldc = ldc;
-    a.add_f32 = add_f32;
-    static DeviceOnce attr_once;
-    if (attr_once.pending(ctx->device)) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_w4_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kW4Smem);
-        if (e != cudaSuccess) return e;
-        attr_once.done(ctx->device);
-    }
-    const int tiles = a.m_blocks * a.n_blocks;
-    const int grid = tiles < ctx->num_sms ? tiles : ctx->num_sms;
-    gemm_w4_tc_kernel<<<grid, kW4Threads, kW4Smem, ctx->stream>>>(a);
-    return cudaGetLastError();
+    return cudaSuccess;
+}
+
+// C[M][N] (fp16, or fp32 accumulated into when add_f32) = X[M][K] fp16 * dequant(W)^T; W rows [N], K % 128 == 0, ldx % 8 == 0.
+cudaError_t launch_gemm_w4_tc(Ctx *ctx, const __half *X, long long ldx, const uint32_t *w, const uint32_t *zeros, const __half *scales, void *C,
+                              long long ldc, int M, int N, int K, int add_f32) {
+    tc::GemmArgs a = {};
+    cudaError_t e = fill_w4_gemm_args(a, X, ldx, w, zeros, scales, C, ldc, M, N, K);
+    if (e != cudaSuccess) return e;
+    if (add_f32) return tc::launch_wg<kBN, kLdStages, false, true, 1, tc::EpiAddF32>(ctx, a);
+    return tc::launch_wg<kBN, kLdStages, false, true, 1, tc::EpiHalf>(ctx, a);
 }
 
 }  // namespace tce

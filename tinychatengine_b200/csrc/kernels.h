@@ -35,7 +35,7 @@ struct Ctx {
     int gemv_stages = 8;           // TMA ring depth (16 KiB stages, capped by the per-CTA shared-memory share); 0 = deepest that fits
     bool use_pdl = false;
     int pdl_early = 0;  // with use_pdl: 1 = dependents may become resident from the first instruction of each GEMV (2: and no 2-CTA/SM mode)
-    // large-M (prefill) path: fp16 expansion of one int4 weight matrix, grown on demand; M >= gemm_min_m goes to the tcgen05 GEMM
+    // large-M (prefill) path: fp16 expansion of one int4 weight matrix, grown on demand; M >= gemm_min_m goes to the wgmma GEMM
     __half *w16_scratch = nullptr;
     size_t w16_scratch_elems = 0;
     int gemm_min_m = 16;
@@ -117,10 +117,10 @@ cudaError_t launch_gemm_f16_tc(Ctx *ctx, const __half *A, long long lda, const _
 // fused variant (gemm_w4_tc.cu): the nibbles are unpacked inside the tile pipeline, no fp16 copy of the weights in HBM
 cudaError_t launch_gemm_w4_tc(Ctx *ctx, const __half *X, long long ldx, const uint32_t *w, const uint32_t *zeros, const __half *scales, void *C, long long ldc,
                               int M, int N, int K, int add_f32);
-// which W4A16 large-M GEMM runs (TCE_W4_GEMM=expand|fused|pair|pair_fused; the default is the measured best, profiles/README.md)
+// which W4A16 large-M GEMM runs (TCE_W4_GEMM=expand|fused|pair|pair_fused; see gemm_tc2.cu)
 enum W4GemmMode : int { W4G_EXPAND = 0, W4G_FUSED = 1, W4G_PAIR = 2, W4G_PAIR_FUSED = 3, W4G_PAIR_OVERLAP = 4 };
 int w4_gemm_mode();
-// CTA-pair variants (gemm_tc2.cu): tcgen05.mma.cta_group::2 on 256 x 256 tiles, W as fp16 or as packed int4 (unpack fused)
+// CTA-pair variants (gemm_tc2.cu): 2-CTA clusters on 256-row tiles, weight tiles multicast, W as fp16 or as packed int4 (unpack fused)
 cudaError_t launch_gemm_f16_pair(Ctx *ctx, const __half *X, long long ldx, const __half *W, long long ldw, void *C, long long ldc, int M, int N, int K, int add_f32);
 cudaError_t launch_gemm_f16_pair_silu(Ctx *ctx, const __half *X, long long ldx, const __half *W, long long ldw, __half *act, long long ldc, int M, int F, int K);
 cudaError_t launch_gemm_w4_pair(Ctx *ctx, const __half *X, long long ldx, const uint32_t *w, const uint32_t *zeros, const __half *scales, void *C, long long ldc,

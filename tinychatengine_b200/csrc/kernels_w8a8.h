@@ -26,7 +26,7 @@ struct W8A8Args {
 };
 
 cudaError_t launch_w8a8_dp4a(Ctx *ctx, const W8A8Args &a);
-cudaError_t launch_w8a8_tc(Ctx *ctx, const W8A8Args &a);  // tcgen05 kind::i8, non-batched, K % 128 == 0
+cudaError_t launch_w8a8_tc(Ctx *ctx, const W8A8Args &a);  // wgmma s8 x s8, non-batched, K % 128 == 0
 
 // int8 attention core of Int8OPTAttention::forward (llm/src/nn_modules/Int8OPTAttention.cc:183-284)
 struct OptAttnParams {

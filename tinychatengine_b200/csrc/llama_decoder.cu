@@ -462,7 +462,7 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         for (int k = 0; k < pk::kMaxBoxes; k++)
             if ((k < a.op[i].plan[0].nbox && a.op[i].plan[0].map[k] < 0) || (k < a.op[i].plan[1].nbox && a.op[i].plan[1].map[k] < 0)) return no("too many box widths");
         // unit boxes ([group][row][64 B], conflict-free LDS.128) where the dense consumer applies (every stage made of 16-group boxes)
-        static const bool want_units = !getenv("TCE_PK_UNIT_BOXES") || atoi(getenv("TCE_PK_UNIT_BOXES")) != 0;  // default on: +1.3 % (profiles/README.md)
+        static const bool want_units = !getenv("TCE_PK_UNIT_BOXES") || atoi(getenv("TCE_PK_UNIT_BOXES")) != 0;  // default on
         a.op[i].unit = (want_units && a.op[i].plan[0].bw[0] == 16 && (NG & 15) == 0) ? 1 : 0;
         if (a.op[i].IC > max_ic) max_ic = a.op[i].IC;
         if (a.op[i].NG > max_ng) max_ng = a.op[i].NG;
@@ -606,7 +606,7 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
     }
     if ((int)pk::smem_bytes(a) > ctx_->smem_optin) return no("shared memory");
     // pair staging (clusters of two CTAs share the activation staging over DSMEM): on unless switched off or the device cannot co-schedule
-    // num_sms / 2 such clusters (+3 % on one B200, profiles/README.md)
+    // num_sms / 2 such clusters
     a.pair = (!getenv("TCE_PK_PAIR") || atoi(getenv("TCE_PK_PAIR")) != 0) && pk::pair_supported(ctx_, a) ? 1 : 0;
     pargs_ = a;
     return cudaSuccess;

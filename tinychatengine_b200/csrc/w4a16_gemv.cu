@@ -1,4 +1,4 @@
-// w4a16_gemv.cu -- stand-alone W4A16 group-128 GEMV launch (batch 1..8 decode) on sm_100a.
+// w4a16_gemv.cu -- stand-alone W4A16 group-128 GEMV launch (batch 1..8 decode) on sm_90a.
 //
 // Replaces MatmulOperator::gemv_forward_cuda + gemv_kernel_g128 (reference kernels/cuda/gemv_cuda.cu:140-260).
 // The device-side roles live in w4a16_gemv_impl.cuh (shared with the persistent decode kernel); this file is the
@@ -267,8 +267,8 @@ cudaError_t launch_mma(Ctx *ctx, const KArgs &a_in, bool pdl) {
         attr_once.done(ctx->device);
     }
     const long long U = (long long)a.num_tiles * a.NG;
-    // Two co-resident CTAs per SM (two independent TMA rings, 16 consumer warps) stream ~25 % faster than one on large
-    // matrices (profiles/r01_gemv_microbench.jsonl: lm_head 5.1 vs 4.0 TB/s) but double the per-launch activation
+    // Two co-resident CTAs per SM (two independent TMA rings, 16 consumer warps) stream faster than one on large
+    // matrices but double the per-launch activation
     // staging, which dominates small launches and long rows: only used when every CTA still gets >= 128 units and the
     // activation vector is short.  "gemv_ctas_per_sm" > 1 forces it.
     int per_sm = ctx->gemv_ctas_per_sm;
@@ -280,10 +280,10 @@ cudaError_t launch_mma(Ctx *ctx, const KArgs &a_in, bool pdl) {
     const long long cuts = a.full ? U / kStageGroups : U;  // stream-K cuts fall on whole stages when every stage is full
     if ((long long)nc > cuts) nc = (int)cuts;
     // Epilogues that need a single ordered writer per output (stores, SiLU*mul, deterministic residual) avoid split
-    // tiles altogether when there is at least one whole tile per CTA: the fix-up protocol costs ~2.5 us of tail per
-    // launch (profiles/r01_gemv_phase_timeline.txt), more than the <= 1/tiles_per_cta imbalance it removes.
+    // tiles altogether when there is at least one whole tile per CTA: the fix-up protocol adds a tail to every
+    // launch, more than the <= 1/tiles_per_cta imbalance it removes.
     a.aligned = (!a.atomic_add && a.num_tiles >= nc) ? 1 : 0;
-    // Ring depth = bytes in flight per SM.  HBM latency under load (~1.2 us) x 6.5 TB/s / 148 SMs = ~55 KB must be in flight per SM
+    // Ring depth = bytes in flight per SM.  HBM latency under load (~1.2 us) x 3.35 TB/s / 132 SMs = ~30 KB must be in flight per SM
     // all the time, and a slot is only re-requested after it was consumed: the deepest ring that fits the per-CTA share of shared
     // memory (1 KiB per CTA is reserved by the driver), at most kMaxStages and no more stages than the CTA has work for.
     {
@@ -337,8 +337,8 @@ cudaError_t launch_w4a16_gemv(Ctx *ctx, const W4GemvParams &p) {
         cudaError_t e = encode_w4_tmap(&a.tmap[i], p.seg[i].w, p.seg[i].rows, p.IC, a.sg, p.pair_mode ? 8 : 16);
         if (e != cudaSuccess) return e;
     }
-    // 16 consumer warps pay off on long rows (down_proj, IC = 14336: 10.4 vs 12.1 us), where one CTA per SM stages a long activation
-    // vector and the 2-CTA mode is off; 8 warps (x 2 CTAs on large launches) everywhere else (profiles/r01_gemv_microbench_v5.jsonl)
+    // 16 consumer warps pay off on long rows (down_proj, IC = 14336), where one CTA per SM stages a long activation
+    // vector and the 2-CTA mode is off; 8 warps (x 2 CTAs on large launches) everywhere else
     const int cw = ctx->gemv_consumer_warps == 16 ? 16 : (ctx->gemv_consumer_warps == 8 ? 8 : (p.IC > 8192 && p.M == 1 ? 16 : 8));
     if (p.M > 1 && (int)w4a16_gemv_smem_bytes(8, cw, p.IC) > ctx->smem_optin) {
         // the 8-column activation tile does not fit next to the weight ring: one pass per activation row

@@ -1,4 +1,4 @@
-// w8a8.cu -- W8A8 (SmoothQuant) INT8 x INT8 -> INT32 linear / batched-matmul family on sm_100a.
+// w8a8.cu -- W8A8 (SmoothQuant) INT8 x INT8 -> INT32 linear / batched-matmul family on sm_90a.
 //
 // Replaces the eight MatmulOperator::mat_mul_accelerator_int8_fast_* methods
 // (reference kernels/ref/matmul_ref_int8.cc:11-192, AVX: kernels/avx/matmul_avx_int8.cc).  Integer
@@ -11,7 +11,7 @@
 // `batch` flavours: row i of A uses its own B slab B[i][N][K] (per-head QK^T / PV at sqlen 1).
 //
 // This file holds the DP4A kernel: one warp per output column, 128-bit loads, up to 8 activation rows per
-// pass -- HBM-bound for the M<=8 decode case.  Large-M prefill goes to the tcgen05 kind::i8 GEMM (w8a8_gemm.cu).
+// pass -- HBM-bound for the M<=8 decode case.  Large-M prefill goes to the wgmma s8 x s8 GEMM (gemm_tc.cu).
 #include "common.cuh"
 #include "kernels.h"
 #include "kernels_w8a8.h"
@@ -97,8 +97,7 @@ __global__ void __launch_bounds__(kWarps * 32) w8a8_dp4a_kernel(const W8A8Args a
 
 // Decode flavour (M <= 4 rows, one B for all rows, K % 16 == 0, K >= 512): HBM-bound weight streaming.  Persistent warps walk the output
 // columns interleaved (neighbouring warps stream neighbouring weight rows), the activation rows sit in shared memory, and every
-// lane keeps UNR 128-bit weight loads in flight (the simple kernel above has one load per warp in flight and short-lived warps:
-// 2.0-2.8 TB/s; this one is measured in profiles/).  Integer sums in any order are exact, the epilogue is the shared one.
+// lane keeps UNR 128-bit weight loads in flight (the simple kernel above has one load per warp in flight and short-lived warps).  Integer sums in any order are exact, the epilogue is the shared one.
 template <int MR, int UNR>
 __global__ void __launch_bounds__(kWarps * 32) w8a8_stream_kernel(const W8A8Args a) {
     extern __shared__ __align__(16) uint8_t sA[];  // [MR][K]

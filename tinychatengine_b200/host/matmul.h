@@ -90,7 +90,7 @@ class MatmulOperator {  // stateless, constructed per call by the reference's wr
     TCE_MATMUL_OPS_ELSEWHERE(TCE_DECLARE_OP, TCE_DECLARE_OP_MUT)
 #undef TCE_DECLARE_OP
 #undef TCE_DECLARE_OP_MUT
-    // the prefill GEMM slot (kernels/matmul.h:142-145: declared, never defined by the reference): tcgen05 GEMM for M >= 16
+    // the prefill GEMM slot (kernels/matmul.h:142-145: declared, never defined by the reference): wgmma GEMM for M >= 16
     void gemm_forward_cuda(const struct matmul_params *params, int split_k_iters);
     void gemm_forward_cuda_8splits(const struct matmul_params *params, float16_t *split_8_buffer);
     void gemm_forward_cuda_half(const struct matmul_params *params, int split_k_iters);

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Micro-benchmark of the tcgen05 GEMMs at the prefill shapes of BASELINE.json configs 3 and 4.
+"""Micro-benchmark of the wgmma GEMMs at the prefill shapes of BASELINE.json configs 3 and 4.
 W4A16: Llama-2-13B prefill (M = 2048 tokens): expansion kernel + GEMM timed together (what tce_w4a16_gemm costs), and against
 torch.matmul (cuBLAS fp16) on pre-expanded weights as the library yardstick.  W8A8: Llama-2-7B shapes, M = 2048.
     python tools/gemm_bench.py [--reps 10] [--m 2048]

@@ -24,8 +24,8 @@ def main():
         for i in range(5):
             ctx.w4a16_gemv(x, *bufs[i % len(bufs)], out=y)
         torch.cuda.synchronize()
-        out = np.zeros((148, 8), np.uint64)
-        n = ctx.L.tce_ctx_read_gemv_timing(ctx.h, out.ctypes.data_as(C.c_void_p), 148)
+        out = np.zeros((ctx.num_sms, 8), np.uint64)
+        n = ctx.L.tce_ctx_read_gemv_timing(ctx.h, out.ctypes.data_as(C.c_void_p), ctx.num_sms)
         t = out[:n].astype(np.int64)
         t0 = t[:, 0].min()
         rel = (t - t0) / 1e3

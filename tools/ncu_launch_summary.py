@@ -2,9 +2,9 @@
 """Condense an `ncu --csv` launch list (gpu__time_duration.sum, dram__bytes_read.sum, dram__bytes_write.sum per launch) of decode
 steps into a per-kernel table and the per-launch DRAM traffic of the dominant kernel (roofline.traffic of bench.py).
     ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum --clock-control none \\
-        -k regex:'gemv|attn|embedding|argmax' -c 400 --csv --log-file gpurun_out/step_kernels.csv \\
+        -k regex:'gemv|attn|embedding|argmax' -c 400 --csv --log-file step_kernels.csv \\
         python bench.py --steps 1 --warmup 1 --no-cpu-baseline --ctx 2048
-    python tools/ncu_launch_summary.py gpurun_out/step_kernels.csv profiles/r01_decode_step_kernels.csv profiles/roofline_traffic.json
+    python tools/ncu_launch_summary.py step_kernels.csv profiles/decode_step_kernels.csv profiles/roofline_traffic.json
 """
 import collections
 import csv

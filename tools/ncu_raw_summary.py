@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Condense `ncu -i X.ncu-rep --page raw --csv` (one captured launch of `ncu --set full`) into the handful of counters the docs quote.
-    ncu -i gpurun_out/r02_gemm_pair.ncu-rep --page raw --csv > gpurun_out/r02_gemm_pair_raw.csv
-    python tools/ncu_raw_summary.py gpurun_out/r02_gemm_pair_raw.csv "command line of the capture" > profiles/r02_ncu_gemm_pair.txt
+    ncu -i gemm_pair.ncu-rep --page raw --csv > gemm_pair_raw.csv
+    python tools/ncu_raw_summary.py gemm_pair_raw.csv "command line of the capture" > profiles/ncu_gemm_pair.txt
 """
 import csv
 import sys

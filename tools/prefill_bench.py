@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""BASELINE.json config 4: Llama-2-13B AWQ-INT4 prompt processing (2048 tokens) on one B200 through tce_llama_prefill.
+"""BASELINE.json config 4: Llama-2-13B AWQ-INT4 prompt processing (2048 tokens) on one H100 through tce_llama_prefill.
 Reports ms, tokens/s and linear-layer TFLOP/s (SURVEY.md 8(d): 2*n*12.688 G + attention 4*T^2*E*L un-masked count).
     python tools/prefill_bench.py [--model llama2-13b] [--n 2048] [--reps 3]
 """
@@ -16,11 +16,11 @@ from tinychatengine_b200.llama import GEOMETRIES, LlamaModel  # noqa: E402
 from tinychatengine_b200.runtime import Context  # noqa: E402
 
 
-def prefill_once(ctx, dev, stream, model_name="llama2-13b", n=2048, peaks=None, reps=3):
+def prefill_once(ctx, dev, stream, model_name="llama2-13b", n=2048, peaks=None, reps=3, logits_out=None):
     """One prompt pass through tce_llama_prefill (host tokens in, greedy token out), best of `reps`, timed with CUDA events on `stream`."""
     g = GEOMETRIES[model_name]
     model = LlamaModel(ctx, g, max_ctx=n, seed=1)
-    toks = [int(t) for t in torch.randint(0, g.vocab_size, (n,))]
+    toks = [int(t) for t in torch.randint(0, g.vocab_size, (n,), generator=torch.Generator().manual_seed(7))]
     model.prefill(toks, 0, None)  # warm-up: allocations, module load
     torch.cuda.synchronize(dev)
     ts = []
@@ -31,6 +31,9 @@ def prefill_once(ctx, dev, stream, model_name="llama2-13b", n=2048, peaks=None, 
         e1.record(stream)
         torch.cuda.synchronize(dev)
         ts.append(e0.elapsed_time(e1) * 1e-3)
+    if logits_out is not None:  # the same pass once more, untimed: the last position's logits row
+        logits_out.append(torch.empty(g.vocab_size, dtype=torch.float32))
+        model.prefill(toks, 0, logits_out[0])
     model.close()
     t = min(ts)
     hd = g.head_dim

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Per-kernel counts of the Blackwell-specific SASS mnemonics in the shipped library (cuobjdump -sass, no GPU needed):
-    python tools/sass_mnemonics.py > profiles/r02_sass_mnemonics.txt
-UTCHMMA/UTCIMMA = tcgen05.mma (f16 / i8), LDTM = tcgen05.ld, UTMALDG = TMA tensor load, UBLKCP = TMA bulk copy, UTMAPF = TMA prefetch,
-IMMA/HMMA = mma.sync, LDSM = ldmatrix, SYNCS = mbarrier ops, UTCBAR = tcgen05.commit, USETMAXREG = setmaxnreg, UCGABAR = cluster barrier."""
+"""Per-kernel counts of the Hopper-specific SASS mnemonics in the shipped library (cuobjdump -sass, no GPU needed):
+    python tools/sass_mnemonics.py
+HGMMA/IGMMA = wgmma (f16 / s8), UTMALDG = TMA tensor load, UBLKCP = TMA bulk copy, UTMAPF = TMA prefetch,
+IMMA/HMMA = mma.sync, LDSM = ldmatrix, SYNCS = mbarrier ops, USETMAXREG = setmaxnreg, UCGABAR = cluster barrier."""
 import collections
 import re
 import subprocess
@@ -11,7 +11,7 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parents[1]
 LIB = ROOT / "tinychatengine_b200" / "lib" / "libtce_b200.so"
-COLS = ["UTCHMMA", "UTCIMMA", "LDTM", "UTMALDG", "UBLKCP", "UTMAPF", "IMMA", "HMMA", "LDSM", "SYNCS", "UTCBAR", "USETMAXREG", "REDUX", "UCGABAR"]
+COLS = ["HGMMA", "IGMMA", "UTMALDG", "UBLKCP", "UTMAPF", "IMMA", "HMMA", "LDSM", "SYNCS", "USETMAXREG", "REDUX", "UCGABAR"]
 
 
 def short_name(demangled: str) -> str:
@@ -44,10 +44,10 @@ def main():
         if m and cur:
             op = m.group(1)
             for c in COLS:
-                if op == c or op.startswith(c + "_") or (c in ("IMMA", "HMMA", "LDSM", "SYNCS", "LDTM", "REDUX", "UTCBAR", "UCGABAR") and op.startswith(c)):
+                if op == c or op.startswith(c + "_") or (c in ("IMMA", "HMMA", "HGMMA", "IGMMA", "LDSM", "SYNCS", "REDUX", "UCGABAR") and op.startswith(c)):
                     counts[cur][c] += 1
-    print(f"SASS mnemonic counts per kernel of {lib.relative_to(ROOT) if lib.is_relative_to(ROOT) else lib} (cuobjdump -sass; sm_100a), kernels that use any of them.")
-    print(__doc__.split("profiles/r02_sass_mnemonics.txt\n", 1)[1].strip())
+    print(f"SASS mnemonic counts per kernel of {lib.relative_to(ROOT) if lib.is_relative_to(ROOT) else lib} (cuobjdump -sass; sm_90a), kernels that use any of them.")
+    print(__doc__.split("tools/sass_mnemonics.py\n", 1)[1].strip())
     print()
     print(f"{'kernel':<78}" + "".join(f"{c[:7]:>8}" for c in COLS))
     for k in sorted(set(order), key=lambda k: (-sum(counts[k].values()), k)):

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """BASELINE.json config 3: one Int8OPTDecoderLayer-shaped W8A8 layer at Llama-2-7B shapes (E 4096, F 11008, 32 heads x 128) on one
-B200, end to end through the C ABI in the order of Int8OPTDecoderLayer::forward (llm/src/nn_modules/Int8OPTDecoderLayer.cc:24-59):
+H100, end to end through the C ABI in the order of Int8OPTDecoderLayer::forward (llm/src/nn_modules/Int8OPTDecoderLayer.cc:24-59):
 LayerNormQ -> q/k/v (W8A8B8O8Linear) -> tce_opt_int8_attention (int8 KV cache in place) -> out_proj (W8A8BFP32OFP32Linear) -> residual
 add -> LayerNormQ -> fc1 (W8A8B8O8LinearReLU) -> fc2 (W8A8BFP32OFP32Linear) -> residual add.  M = 1 (decode at ctx 1024: HBM-bound, GB/s
 of int8 weights) and M = 2048 (prompt: tensor-bound, TOP/s).  Layers rotate over > 2x L2 of distinct weights.
@@ -98,7 +98,7 @@ def w8a8_layer(ctx, dev, stream, peaks, nlayers=3, reps=4):
                                         "tok_s_at_32_layers": 1e3 / (32 * ms)}
         else:
             tops = Layer.ops(M) / (ms * 1e-3) / 1e12
-            out["prefill_m2048"] = {"ms_per_layer": ms, "linear_TOP_per_s": tops, "note": "int8 tcgen05 (kind::i8) GEMMs + bit-exact int8 attention + serial-order LayerNormQ"}
+            out["prefill_m2048"] = {"ms_per_layer": ms, "linear_TOP_per_s": tops, "note": "int8 wgmma (s8 x s8) GEMMs + bit-exact int8 attention + serial-order LayerNormQ"}
     out["shapes"] = "Llama-2-7B widths in the OPT W8A8 layer structure (q/k/v/o 4096x4096, fc1 11008x4096 ReLU, fc2 4096x11008, 32 heads x 128), eager launches"
     return out
 
