@@ -8,11 +8,17 @@ from helpers import oracle_decode_step, rel_err
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("mega", ["1", "0"])
+@pytest.mark.parametrize("mega,pair", [("1", None), ("0", None), ("1", "0")], ids=["1", "0", "1-pair0"])
 @pytest.mark.parametrize("geom", ["tiny-gqa", "tiny-mha"])
-def test_decode_steps_match_oracle(geom, mega, monkeypatch):
-    """mega=1: one persistent cooperative kernel per token (the default); mega=0: one kernel per op inside a CUDA graph."""
+def test_decode_steps_match_oracle(geom, mega, pair, monkeypatch):
+    """mega=1: one persistent cooperative kernel per token (the default), with pair staging (clusters of two CTAs) where the device
+    allows it, or with TCE_PK_PAIR=0 single-CTA staging (what a refused cluster launch falls back to); mega=0: one kernel per op
+    inside a CUDA graph."""
     monkeypatch.setenv("TCE_PERSISTENT", mega)
+    if pair is None:
+        monkeypatch.delenv("TCE_PK_PAIR", raising=False)
+    else:
+        monkeypatch.setenv("TCE_PK_PAIR", pair)
     from tinychatengine_b200.llama import GEOMETRIES, LlamaModel
     from tinychatengine_b200.runtime import Context
 
@@ -117,17 +123,22 @@ def test_persistent_kernel_is_deterministic_when_asked(monkeypatch):
     assert torch.equal(outs[0], outs[1])
 
 
-@pytest.mark.parametrize("mega", ["1", "0"])
-@pytest.mark.parametrize("pos", [0, 2048, 4095])
-def test_benchmarked_geometry_step_matches_oracle(pos, mega, monkeypatch):
+@pytest.mark.parametrize(
+    "widths,pos,mega",
+    [pytest.param(w, pos, mega, id=f"{pos}-{mega}" if w == "llama3-8b" else f"{pos}-{mega}-{w}")
+     for w in ("llama3-8b", "llama2-7b") for mega in ("1", "0") for pos in (0, 2048, 4095)],
+)
+def test_benchmarked_geometry_step_matches_oracle(widths, pos, mega, monkeypatch):
     """The configuration bench.py times -- Llama-3-8B widths (E 4096, F 14336, 32:8 heads, vocab 128256), max_ctx 4096 -- with two
-    layers, at the start, the middle and the end of the context window, against the oracle-composed step on a random-filled cache."""
+    layers, at the start, the middle and the end of the context window, against the oracle-composed step on a random-filled cache.
+    Llama-2-7B widths (F 11008: 86 groups per down_proj row) add weight stages that are only partly filled (22 of 32 groups)."""
     monkeypatch.setenv("TCE_PERSISTENT", mega)
-    from tinychatengine_b200.llama import GEOMETRIES, LlamaGeometry, LlamaModel
+    import dataclasses
+
+    from tinychatengine_b200.llama import GEOMETRIES, LlamaModel
     from tinychatengine_b200.runtime import Context
 
-    g8 = GEOMETRIES["llama3-8b"]
-    g = LlamaGeometry("llama3-8b-2l", 2, g8.num_heads, g8.num_kv_heads, g8.embed_dim, g8.hidden_dim, g8.vocab_size, g8.rms_eps, g8.rope_theta)
+    g = dataclasses.replace(GEOMETRIES[widths], name=f"{widths}-2l", num_layers=2)
     ctx = Context(0)
     model = LlamaModel(ctx, g, max_ctx=4096, seed=21, random_zeros=True)
     gen = torch.Generator(device="cuda")

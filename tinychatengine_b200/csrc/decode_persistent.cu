@@ -6,9 +6,10 @@
 // token is ONE kernel of one CTA per SM whose warp roles persist across all phases (5 per layer + lm_head):
 //
 //   producer (1 warp, 1 elected lane)  walks the phases in order and keeps a ring of `nst` TMA stages full.  A stage is either
-//        [16 rows x <=32 groups] of packed int4 weights (two 2-D UTMALDG boxes of 16 KiB) + the stage's repacked scales|zeros record (one
-//        1280 B UBLKCP), or 64 cached K rows + 64 cached V rows of the attention phase (four 128B-swizzled 2-D boxes).  It depends on
-//        nothing but static data and the token position, so it runs ahead across every phase boundary.
+//        [16 rows x <=32 groups] of packed int4 weights (one or two 3-D UTMALDG boxes of 16 groups through the [group][row][64 B] view,
+//        16 KiB each; see GemvOp) + the stage's repacked scales|zeros record (one 1536 B UBLKCP), or 64 cached K rows + 64 cached V rows
+//        of the attention phase (four 128B-swizzled 2-D boxes).  It depends on nothing but static data and the token position, so it
+//        runs ahead across every phase boundary.
 //   consumers (16 warps)  per phase: spin on the flag-carrying words of their input vector, quantise it (fused RMSNorm, four int8 planes
 //        per 128-group), run the integer-MMA GEMV over this CTA's tiles (two 128-k groups per warp and stage), or run flash-decoding
 //        attention straight out of the ring stages (mma.sync m16n8k16, ldmatrix on the swizzled K/V rows).
@@ -23,7 +24,6 @@
 // 8-byte words, flag included) and every reader sums the P slots in rank order.
 // All waits are bounded: a protocol bug surfaces as a launch failure within seconds, not as a hung GPU.
 #include <stdio.h>
-#include <stdlib.h>
 
 #include "attention_impl.cuh"
 #include "persistent.h"
@@ -67,8 +67,7 @@ TCE_DEVINL uint2 ld_ll1(const uint2 *p, bool sys) {
 }
 // A failed poll waits this long before it asks L2 again: thousands of threads spinning without a pause fill the L2 request queues and
 // stretch every round trip (their own and the producers' stores).
-__constant__ unsigned g_poll_ns = 100;  // TCE_PK_POLL_NS (set_poll_backoff)
-#define kPollBackoffNs g_poll_ns
+constexpr unsigned kPollBackoffNs = 100;
 constexpr long long kSpinLimit = 20000000000LL;  // ~10 s: a peer rank may legitimately start its kernel later
 // spin until both words of the pair carry `tag`
 TCE_DEVINL uint4 wait_ll2(const uint2 *p, uint32_t tag, bool sys) {
@@ -148,26 +147,11 @@ TCE_DEVINL void mbar_wait_u32(uint32_t bar, uint32_t parity) {
 }
 TCE_DEVINL void mbar_arrive_u32(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
 
-// L2 prefetch of a TMA box / of a byte range: HBM -> L2 only, no shared-memory slot, no barrier
-TCE_DEVINL void tma_prefetch_2d_pred(const void *tmap, int x, int y, uint32_t pred) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %3, 0;\n\t@p cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];\n\t}" ::"l"(tmap), "r"(x), "r"(y),
-                 "r"(pred)
-                 : "memory");
-}
-TCE_DEVINL void tma_prefetch_3d_pred(const void *tmap, int x, int y, int z, uint32_t pred) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t@p cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];\n\t}" ::"l"(tmap), "r"(x),
-                 "r"(y), "r"(z), "r"(pred)
-                 : "memory");
-}
-TCE_DEVINL void bulk_prefetch_pred(const void *src, uint32_t bytes, uint32_t pred) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p cp.async.bulk.prefetch.L2.global [%0], %1;\n\t}" ::"l"(src), "r"(bytes), "r"(pred) : "memory");
-}
 TCE_DEVINL int lds_volatile_i32(const int *p) {
     int v;
     asm volatile("ld.volatile.shared.s32 %0, [%1];" : "=r"(v) : "r"(smem_u32(p)) : "memory");
     return v;
 }
-TCE_DEVINL void sts_volatile_i32(int *p, int v) { asm volatile("st.volatile.shared.s32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory"); }
 
 TCE_DEVINL void stamp(const Args &a, int cta, int nphase, int p, int k) {  // one thread
     if (a.dbg) {
@@ -193,7 +177,6 @@ struct PSmem {
     float *rms;         // [kCW]
     float *rope;        // cos[128] | sin[128] of the token position
     uint64_t *full, *empty, *red_full, *red_empty;
-    int *issued;        // stages the loader has issued so far (read by the L2 prefetch warp)
     uint64_t *rx;       // pair staging: counts the bytes the partner has mirrored into this CTA for the current staging
     int *free_gen;      // pair staging: written by the partner: the number of phases it has finished (its buffers may be overwritten)
     uint32_t ring_u32, xs_u32, gx_u32, gsum_u32, full_u32, empty_u32, redfull_u32, redempty_u32;
@@ -225,8 +208,7 @@ TCE_DEVINL PSmem carve(uint8_t *raw, const Args &a) {
     s.red_full = s.empty + a.nst;
     s.red_empty = s.red_full + kRedBufs;
     s.rx = s.red_empty + kRedBufs;
-    s.issued = reinterpret_cast<int *>(s.rx + 1);
-    s.free_gen = s.issued + 1;
+    s.free_gen = reinterpret_cast<int *>(s.rx + 1);
     s.ring_u32 = smem_u32(s.ring);
     s.xs_u32 = smem_u32(s.xs);
     s.gx_u32 = smem_u32(s.gx);
@@ -267,7 +249,8 @@ TCE_DEVINL void partition(const GemvOp &op, int cta, int ncta, int &t0, int &t1)
 }
 
 // attention work split: the visible positions [0, T) in chunks of kKvChunk; every KV head gets NS = #CTAs / KVH consecutive CTAs,
-// each takes `cps` consecutive chunks (the fewest that cover the context: see kAttnCps)
+// each takes `cps` consecutive chunks, the fewest that cover the context: as many CTAs as the context has chunks take part, so that a
+// CTA's K/V stages fit the ring slots left free by the tail of the q|k|v GEMV (a 4-chunk CTA waited ~3 us for its last stage)
 struct AttnSplit {
     int kvh, split, ch0, ch1, nsplit;  // ch0 >= ch1: nothing to do
 };
@@ -278,8 +261,6 @@ TCE_DEVINL AttnSplit attn_split(int cta, int ncta, int KVH, int pos) {
     int NS = ncta / KVH;
     if (NS < 1) NS = 1;
     int cps = (nch + NS - 1) / NS;
-    const int want = nch < kAttnCps ? nch : kAttnCps;
-    if (cps < want) cps = want;
     if (cps * 32 < nch) cps = (nch + 31) / 32;  // the split merge keeps one split per lane
     s.nsplit = (nch + cps - 1) / cps;
     s.kvh = cta / NS;
@@ -295,144 +276,79 @@ TCE_DEVINL AttnSplit attn_split(int cta, int ncta, int KVH, int pos) {
 }
 
 // ------------------------------------------------------------------------------------------------------------ producer
-// The same walk over (tile, stage, box) serves two warps: the loader (PF = false) moves stages into the ring as slots free up; the
-// prefetcher (PF = true) runs `kPrefetchAhead` stages ahead of it and only asks L2 for the same boxes, so that the bytes in flight
-// towards HBM are not bounded by the ring (4 x 32 KiB per SM per loaded HBM round trip) and a ring slot waits one L2 round trip instead of one DRAM round trip.
-constexpr int kPrefetchAhead = 10;
-struct ProdState {
-    Ring rs;
-    int count = 0;  // stages issued (loader) / prefetched (prefetcher) so far
-};
-template <bool PF>
-TCE_DEVINL void prod_throttle_or_slot(const PSmem &sm, ProdState &ps) {
-    if (PF) {
-        if (ps.count >= lds_volatile_i32(sm.issued) + kPrefetchAhead) {
-            const long long t0 = clock64();
-            while (ps.count >= lds_volatile_i32(sm.issued) + kPrefetchAhead) {
-                __nanosleep(64);
-                if (clock64() - t0 > kSpinLimit) __trap();
-            }
-        }
-    } else {
-        mbar_wait(&sm.empty[ps.rs.stage], ps.rs.phase ^ 1);
-    }
-}
-template <bool PF>
-TCE_DEVINL void prod_done(const PSmem &sm, ProdState &ps, uint32_t leader) {
-    ps.count++;
-    if (!PF) {
-        if (leader) sts_volatile_i32(sm.issued, ps.count);
-        __syncwarp();
-        ps.rs.advance(sm.nst);
-    }
-}
-
-template <bool PF>
-TCE_DEVINL void produce_gemv(const GemvOp &op, const CUtensorMap *m0, const uint8_t *meta, const PSmem &sm, ProdState &ps, int cta, int ncta, uint32_t leader,
+// one weight stage: the box of groups 32s + 16b lands at b * 16 KiB (gate | up: the up rows 8 KiB into it); see GemvOp
+TCE_DEVINL void produce_gemv(const GemvOp &op, const CUtensorMap *m0, const uint8_t *meta, const PSmem &sm, Ring &rs, int cta, int ncta, uint32_t leader,
                              uint64_t policy) {
     int t0, t1;
     partition(op, cta, ncta, t0, t1);
-    const bool ragged = (op.NG % kStageGroups) != 0;
+    const uint32_t box_bytes = 16u * (uint32_t)op.bw * 64u;  // 16 rows (gate | up: 8 of each matrix) x bw groups x 64 B
     for (int tile = t0; tile < t1; tile++) {
-        for (int s = 0; s < op.S; s++) {
-            const BoxPlan &pl = op.plan[(ragged && s == op.S - 1) ? 1 : 0];
-            prod_throttle_or_slot<PF>(sm, ps);
-            uint64_t *bar = &sm.full[ps.rs.stage];
-            uint8_t *dst = sm.ring + (size_t)ps.rs.stage * kStageBytes;
-            if (!PF) mbar_arrive_expect_tx_pred(bar, (uint32_t)pl.bytes + kMetaBytes, leader);
-#pragma unroll 1
-            for (int b = 0; b < pl.nbox; b++) {
-                const int xw = (kStageGroups * s + pl.b0[b]) * 16;  // first 32-bit word of the box within the row
-                uint8_t *d = dst + pl.off[b];
-                if (op.pair) {  // matrices of an op are kMapsPerMat maps apart
-                    if (PF && op.unit) {
-                        tma_prefetch_3d_pred(m0 + pl.map[b], 0, tile * 8, xw >> 4, leader);
-                        tma_prefetch_3d_pred(m0 + kMapsPerMat + pl.map[b], 0, tile * 8, xw >> 4, leader);
-                    } else if (PF) {
-                        tma_prefetch_2d_pred(m0 + pl.map[b], xw, tile * 8, leader);
-                        tma_prefetch_2d_pred(m0 + kMapsPerMat + pl.map[b], xw, tile * 8, leader);
-                    } else if (op.unit) {
-                        tma_load_3d_pred(d, m0 + pl.map[b], 0, tile * 8, xw >> 4, bar, policy, leader);
-                        tma_load_3d_pred(d + 8 * pl.bw[b] * 64, m0 + kMapsPerMat + pl.map[b], 0, tile * 8, xw >> 4, bar, policy, leader);
-                    } else {
-                        tma_load_2d_pred(d, m0 + pl.map[b], xw, tile * 8, bar, policy, leader);
-                        tma_load_2d_pred(d + 8 * pl.bw[b] * 64, m0 + kMapsPerMat + pl.map[b], xw, tile * 8, bar, policy, leader);
-                    }
-                } else {
-                    int row = tile * 16;
-                    const CUtensorMap *m = m0;
-                    if (op.nseg > 1 && row >= op.rows0) {
-                        row -= op.rows0;
-                        m = m0 + kMapsPerMat;
-                        if (op.nseg > 2 && row >= op.rows1) {
-                            row -= op.rows1;
-                            m = m0 + 2 * kMapsPerMat;
-                        }
-                    }
-                    if (PF && op.unit)
-                        tma_prefetch_3d_pred(m + pl.map[b], 0, row, xw >> 4, leader);
-                    else if (PF)
-                        tma_prefetch_2d_pred(m + pl.map[b], xw, row, leader);
-                    else if (op.unit)
-                        tma_load_3d_pred(d, m + pl.map[b], 0, row, xw >> 4, bar, policy, leader);
-                    else
-                        tma_load_2d_pred(d, m + pl.map[b], xw, row, bar, policy, leader);
-                }
+        // the tile's matrix (q|k|v: tiles never straddle two segments; gate | up: the gate map, the up map follows it) and first row
+        int row = op.pair ? tile * 8 : tile * 16;
+        const CUtensorMap *m = m0;
+        if (!op.pair && op.nseg > 1 && row >= op.rows0) {
+            row -= op.rows0;
+            m = m0 + 1;
+            if (op.nseg > 2 && row >= op.rows1) {
+                row -= op.rows1;
+                m = m0 + 2;
             }
-            const uint8_t *mrec = meta + ((size_t)tile * op.S + s) * kMetaBytes;
-            if (PF)
-                bulk_prefetch_pred(mrec, kMetaBytes, leader);
-            else
-                bulk_g2s_pred(dst + kMetaOff, mrec, kMetaBytes, bar, policy, leader);
-            prod_done<PF>(sm, ps, leader);
+        }
+        for (int s = 0; s < op.S; s++) {
+            const int nbox = (min(kStageGroups, op.NG - kStageGroups * s) + 15) >> 4;
+            mbar_wait(&sm.empty[rs.stage], rs.phase ^ 1);
+            uint64_t *bar = &sm.full[rs.stage];
+            uint8_t *dst = sm.ring + (size_t)rs.stage * kStageBytes;
+            mbar_arrive_expect_tx_pred(bar, (uint32_t)nbox * box_bytes + kMetaBytes, leader);
+#pragma unroll 1
+            for (int b = 0; b < nbox; b++) {
+                const int grp = kStageGroups * s + 16 * b;
+                tma_load_3d_pred(dst + b * 16384, m, 0, row, grp, bar, policy, leader);
+                if (op.pair) tma_load_3d_pred(dst + b * 16384 + 8192, m + 1, 0, row, grp, bar, policy, leader);
+            }
+            bulk_g2s_pred(dst + kMetaOff, meta + ((size_t)tile * op.S + s) * kMetaBytes, kMetaBytes, bar, policy, leader);
+            __syncwarp();
+            rs.advance(sm.nst);
         }
     }
 }
 
-template <bool PF>
-TCE_DEVINL void produce_attn(const Args &a, const LayerDesc &L, const CUtensorMap *kvmap, const PSmem &sm, ProdState &ps, int cta, int ncta, int pos,
+TCE_DEVINL void produce_attn(const Args &a, const LayerDesc &L, const CUtensorMap *kvmap, const PSmem &sm, Ring &rs, int cta, int ncta, int pos,
                              uint32_t leader, uint64_t policy) {
     const AttnSplit sp = attn_split(cta, ncta, a.KVH, pos);
     for (int c = sp.ch0; c < sp.ch1; c++) {
-        prod_throttle_or_slot<PF>(sm, ps);
-        uint64_t *bar = &sm.full[ps.rs.stage];
-        uint8_t *dst = sm.ring + (size_t)ps.rs.stage * kStageBytes;
+        mbar_wait(&sm.empty[rs.stage], rs.phase ^ 1);
+        uint64_t *bar = &sm.full[rs.stage];
+        uint8_t *dst = sm.ring + (size_t)rs.stage * kStageBytes;
         const int krow = L.k_row0 + sp.kvh * a.max_ctx + c * kKvChunk, vrow = L.v_row0 + sp.kvh * a.max_ctx + c * kKvChunk;
-        if (PF) {
-            tma_prefetch_2d_pred(kvmap, 0, krow, leader);
-            tma_prefetch_2d_pred(kvmap, 64, krow, leader);
-            tma_prefetch_2d_pred(kvmap, 0, vrow, leader);
-            tma_prefetch_2d_pred(kvmap, 64, vrow, leader);
-        } else {
-            mbar_arrive_expect_tx_pred(bar, 2u * kHalfBytes, leader);
-            tma_load_2d_pred(dst, kvmap, 0, krow, bar, policy, leader);
-            tma_load_2d_pred(dst + 8192, kvmap, 64, krow, bar, policy, leader);
-            tma_load_2d_pred(dst + kHalfBytes, kvmap, 0, vrow, bar, policy, leader);
-            tma_load_2d_pred(dst + kHalfBytes + 8192, kvmap, 64, vrow, bar, policy, leader);
-        }
-        prod_done<PF>(sm, ps, leader);
+        mbar_arrive_expect_tx_pred(bar, 2u * kHalfBytes, leader);
+        tma_load_2d_pred(dst, kvmap, 0, krow, bar, policy, leader);
+        tma_load_2d_pred(dst + 8192, kvmap, 64, krow, bar, policy, leader);
+        tma_load_2d_pred(dst + kHalfBytes, kvmap, 0, vrow, bar, policy, leader);
+        tma_load_2d_pred(dst + kHalfBytes + 8192, kvmap, 64, vrow, bar, policy, leader);
+        __syncwarp();
+        rs.advance(sm.nst);
     }
 }
 
-// the producer role: PF = false on warp 0 (loader), PF = true on warp 2 (L2 prefetcher)
-template <bool PF>
+// the loader warp: every byte this CTA needs from HBM, in consumption order, as ring slots free up
 TCE_DEVINL void producer_walk(const Args &a, const PSmem &sm, int cta, int ncta, int pos, int lane) {
-    ProdState ps;
+    Ring rs;
     const uint64_t policy = l2_policy_evict_first();
     const uint32_t leader = (lane == 0) ? 1u : 0u;
     const int Lyr = a.num_layers, nphase = 5 * Lyr + 1;
-    const CUtensorMap *kvmap = a.maps + ((size_t)Lyr * 7 + 1) * kMapsPerMat;
+    const CUtensorMap *kvmap = a.maps + (size_t)Lyr * 7 + 1;
 #pragma unroll 1
     for (int p = 0; p < nphase; p++) {
         const int l = p / 5, k = p - 5 * l;
         if (l == Lyr) {
-            produce_gemv<PF>(a.op[OPI_LMHEAD], a.maps + (size_t)Lyr * 7 * kMapsPerMat, a.lm_meta, sm, ps, cta, ncta, leader, policy);
+            produce_gemv(a.op[OPI_LMHEAD], a.maps + (size_t)Lyr * 7, a.lm_meta, sm, rs, cta, ncta, leader, policy);
         } else if (k == 1) {
-            produce_attn<PF>(a, a.layers[l], kvmap, sm, ps, cta, ncta, pos, leader, policy);
+            produce_attn(a, a.layers[l], kvmap, sm, rs, cta, ncta, pos, leader, policy);
         } else {
             const int oi = (k == 0) ? OPI_QKV : (k - 1);       // k = 2,3,4 -> OPI_O, OPI_GATEUP, OPI_DOWN
             const int mi = (k == 0) ? 0 : (k == 2 ? 3 : (k == 3 ? 4 : 6));  // first tensor map of the op within the layer's seven
-            produce_gemv<PF>(a.op[oi], a.maps + ((size_t)l * 7 + mi) * kMapsPerMat, a.layers[l].meta[oi], sm, ps, cta, ncta, leader, policy);
+            produce_gemv(a.op[oi], a.maps + (size_t)l * 7 + mi, a.layers[l].meta[oi], sm, rs, cta, ncta, leader, policy);
         }
     }
 }
@@ -680,20 +596,6 @@ struct UnitRegs {
     int sxv;
     float st;
 };
-TCE_DEVINL void unit_load(UnitRegs &u, uint32_t w_addr, uint32_t rp8, uint32_t x_addr, uint32_t meta_addr, int gi, int g, int G, uint32_t gx_u32,
-                          uint32_t gsum_u32, int gsel) {
-    u.wa = lds_u4(w_addr);
-    u.wb = lds_u4(w_addr + rp8);
-    u.xe = u.xo = make_uint4(0u, 0u, 0u, 0u);
-    if (g < 4) {  // MMA columns 4..7 are don't-cares: half of the warp skips the activation loads (half the shared-memory wavefronts)
-        u.xe = lds_u4(x_addr + (uint32_t)G * 256u);
-        u.xo = lds_u4(x_addr + (uint32_t)G * 256u + 128u);
-    }
-    u.sc = lds_u32(meta_addr + (uint32_t)(gi * 8 + g) * 4u);
-    u.z = lds_u16(meta_addr + 1024u + (uint32_t)(gi * 8 + g) * 2u);
-    u.sxv = (int)lds_u32(gsum_u32 + (uint32_t)(2 * G + gsel) * 4u);
-    u.st = lds_f32(gx_u32 + (uint32_t)G * 4u);
-}
 TCE_DEVINL void unit_compute(const UnitRegs &u, float lscale, float &totA, float &totB) {
     constexpr uint32_t ML = 0x0f0f0f0fu, MH = 0xf0f0f0f0u;
     int accL[4], accH[4];
@@ -711,29 +613,17 @@ TCE_DEVINL void unit_compute(const UnitRegs &u, float lscale, float &totA, float
     totB += (sc.y * st) * (float)vB;
 }
 
-// where group `gi` of a stage lives: byte offset of (row g, this lane's 16-byte chunk) and the distance to row g + 8
-TCE_DEVINL void locate(const BoxPlan &pl, int gi, int g, int t, uint32_t &off, uint32_t &rp8) {
-    int b = 0;
-#pragma unroll
-    for (int i = 1; i < kMaxBoxes; i++)
-        if (i < pl.nbox && gi >= pl.b0[i]) b = i;
-    const uint32_t rp = (uint32_t)pl.bw[b] * 64u;
-    off = (uint32_t)pl.off[b] + (uint32_t)g * rp + (uint32_t)(gi - pl.b0[b]) * 64u + (uint32_t)t * 16u;
-    rp8 = 8u * rp;
-}
-
-// Fast path for dense boxes of 16 groups (NG >= 16: every Llama width): within a stage every operand address is a per-lane constant
-// plus the slot base, and the second unit of a warp sits at fixed distances (+16 KiB weights, +4 KiB planes, +512 B scales ...), so the
-// inner loop carries almost no address arithmetic (the ALU pipe is what bounds this loop).
-TCE_DEVINL void consume_gemv_dense(const GemvOp &op, const PSmem &sm, Ring &rs, Red &cs, float inv, int cta, int ncta, int cw, int lane) {
+// Warp cw consumes groups cw and cw + 16 of every stage.  Group gi of a stage sits at a fixed place whatever the shape (see GemvOp), so
+// every operand address is a per-lane constant plus the slot base, and the second unit of a warp sits at fixed distances (+16 KiB weights,
+// +4 KiB planes, +512 B scales ...): the inner loop carries almost no address arithmetic (the ALU pipe is what bounds this loop).
+TCE_DEVINL void consume_gemv(const GemvOp &op, const PSmem &sm, Ring &rs, Red &cs, float inv, int cta, int ncta, int cw, int lane) {
     const int g = lane >> 2, t = lane & 3;
     int t0, t1;
     partition(op, cta, ncta, t0, t1);
     const int NG = op.NG, S = op.S;
-    // row g of group cw, this lane's 16-byte chunk.  Row-major boxes: rows 1 KiB apart (2-way bank conflict between rows g, g + 1 of a quarter-warp);
-    // unit boxes: the 16 rows of a group 64 B apart (conflict free), gate | up pairs as two 8-row regions
-    const uint32_t w_lane = op.unit ? (uint32_t)cw * (op.pair ? 512u : 1024u) + (uint32_t)g * 64u + (uint32_t)t * 16u : (uint32_t)g * 1024u + (uint32_t)t * 16u + (uint32_t)cw * 64u;
-    const uint32_t wb_off = op.unit ? (op.pair ? 8192u : 512u) : 8192u;  // row g + 8
+    // row g of group cw, this lane's 16-byte chunk: the 16 rows of a group 64 B apart (conflict-free LDS.128), gate | up as two 8-row regions
+    const uint32_t w_lane = (uint32_t)cw * (op.pair ? 512u : 1024u) + (uint32_t)g * 64u + (uint32_t)t * 16u;
+    const uint32_t wb_off = op.pair ? 8192u : 512u;  // row g + 8
     const uint32_t m_lane = (uint32_t)kMetaOff + (uint32_t)(cw * 8 + g) * 4u;                            // scales of rows g, g + 8 of group cw
     const uint32_t z_lane = (uint32_t)kMetaOff + 1024u + (uint32_t)(cw * 8 + g) * 2u;
     const uint32_t x_lane = sm.xs_u32 + (uint32_t)((g >> 1) & 1) * (uint32_t)op.IC * 2u + (uint32_t)(t * 2 + (g & 1)) * 16u + (uint32_t)cw * 256u;
@@ -744,24 +634,27 @@ TCE_DEVINL void consume_gemv_dense(const GemvOp &op, const PSmem &sm, Ring &rs, 
     for (int tile = t0; tile < t1; tile++) {
         float totA = 0.f, totB = 0.f;
         for (int s = 0; s < S; s++) {
-            const bool two = kStageGroups * s + 16 < NG;  // the stage carries groups 16..31 as well (warp-uniform)
+            // the stage carries this warp's groups (warp-uniform; a partly filled last stage has fewer than 32)
+            const bool has0 = kStageGroups * s + cw < NG, has1 = kStageGroups * s + cw + 16 < NG;
             mbar_wait_u32(sm.full_u32 + (uint32_t)rs.stage * 8u, rs.phase);
             const uint32_t base = sm.ring_u32 + (uint32_t)rs.stage * (uint32_t)kStageBytes;
             const uint32_t wb_ = base + w_lane, mb_ = base + m_lane, zb_ = base + z_lane;
             const uint32_t xb_ = x_lane + (uint32_t)s * (kStageGroups * 256u), sb_ = s_lane + (uint32_t)s * (kStageGroups * 8u), qb_ = q_lane + (uint32_t)s * (kStageGroups * 4u);
             UnitRegs u0, u1;
-            u0.wa = lds_u4(wb_);
-            u0.wb = lds_u4(wb_ + wb_off);
             u0.xe = u0.xo = u1.xe = u1.xo = make_uint4(0u, 0u, 0u, 0u);
-            if (xl) {
-                u0.xe = lds_u4(xb_);
-                u0.xo = lds_u4(xb_ + 128u);
+            if (has0) {
+                u0.wa = lds_u4(wb_);
+                u0.wb = lds_u4(wb_ + wb_off);
+                if (xl) {
+                    u0.xe = lds_u4(xb_);
+                    u0.xo = lds_u4(xb_ + 128u);
+                }
+                u0.sc = lds_u32(mb_);
+                u0.z = lds_u16(zb_);
+                u0.sxv = (int)lds_u32(sb_);
+                u0.st = lds_f32(qb_);
             }
-            u0.sc = lds_u32(mb_);
-            u0.z = lds_u16(zb_);
-            u0.sxv = (int)lds_u32(sb_);
-            u0.st = lds_f32(qb_);
-            if (two) {
+            if (has1) {
                 u1.wa = lds_u4(wb_ + 16384u);
                 u1.wb = lds_u4(wb_ + 16384u + wb_off);
                 if (xl) {
@@ -773,57 +666,6 @@ TCE_DEVINL void consume_gemv_dense(const GemvOp &op, const PSmem &sm, Ring &rs, 
                 u1.sxv = (int)lds_u32(sb_ + 128u);
                 u1.st = lds_f32(qb_ + 64u);
             }
-            unit_compute(u0, lscale, totA, totB);
-            if (two) unit_compute(u1, lscale, totA, totB);
-            __syncwarp();
-            if (lane == 0) mbar_arrive_u32(sm.empty_u32 + (uint32_t)rs.stage * 8u);
-            rs.advance(sm.nst);
-        }
-        // ---- hand the tile sums to the epilogue warp ----
-        totA += __shfl_xor_sync(0xffffffffu, totA, 1);  // (p3, p2) share of t = 0 + (p1, p0) share of t = 1
-        totB += __shfl_xor_sync(0xffffffffu, totB, 1);
-        mbar_wait_u32(sm.redempty_u32 + (uint32_t)cs.rb * 8u, cs.rphase ^ 1);
-        float *rbuf = sm.red + ((size_t)cs.rb * kCW + cw) * 16;
-        if (t == 0) {
-            rbuf[g] = totA * inv;
-            rbuf[g + 8] = totB * inv;
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive_u32(sm.redfull_u32 + (uint32_t)cs.rb * 8u);
-        cs.advance();
-    }
-}
-
-TCE_DEVINL void consume_gemv(const GemvOp &op, const PSmem &sm, Ring &rs, Red &cs, float inv, int cta, int ncta, int cw, int lane) {
-    const int g = lane >> 2, t = lane & 3;
-    int t0, t1;
-    partition(op, cta, ncta, t0, t1);
-    const int NG = op.NG, S = op.S;
-    const bool ragged = (NG % kStageGroups) != 0;
-    // lane-constant weight operands of this warp's two groups (cw, cw + 16), for a full stage and for the ragged last stage of a tile
-    uint32_t wf0, rf0, wf1, rf1, wl0 = 0, rl0 = 0, wl1 = 0, rl1 = 0;
-    locate(op.plan[0], cw, g, t, wf0, rf0);
-    locate(op.plan[0], cw + 16, g, t, wf1, rf1);
-    if (ragged) {
-        locate(op.plan[1], cw, g, t, wl0, rl0);
-        locate(op.plan[1], cw + 16, g, t, wl1, rl1);
-    }
-    // lane-constant activation operands: MMA column g & 3 supplies plane 3 - (g & 3)
-    const uint32_t x_lane = sm.xs_u32 + (uint32_t)((g >> 1) & 1) * (uint32_t)op.IC * 2u + (uint32_t)(t * 2 + (g & 1)) * 16u;
-    const float lscale = (t == 0) ? 65536.f : (t == 1 ? 1.f : 0.f);
-    const int gsel = t & 1;
-    const uint32_t gx_u32 = sm.gx_u32, gsum_u32 = sm.gsum_u32;
-    for (int tile = t0; tile < t1; tile++) {
-        float totA = 0.f, totB = 0.f;
-        for (int s = 0; s < S; s++) {
-            const int n = min(kStageGroups, NG - kStageGroups * s);  // groups this stage carries
-            const bool last = ragged && s == S - 1;
-            mbar_wait_u32(sm.full_u32 + (uint32_t)rs.stage * 8u, rs.phase);
-            const uint32_t base = sm.ring_u32 + (uint32_t)rs.stage * (uint32_t)kStageBytes;
-            UnitRegs u0, u1;
-            const bool has0 = cw < n, has1 = cw + 16 < n;
-            if (has0) unit_load(u0, base + (last ? wl0 : wf0), last ? rl0 : rf0, x_lane, base + kMetaOff, cw, g, kStageGroups * s + cw, gx_u32, gsum_u32, gsel);
-            if (has1) unit_load(u1, base + (last ? wl1 : wf1), last ? rl1 : rf1, x_lane, base + kMetaOff, cw + 16, g, kStageGroups * s + cw + 16, gx_u32, gsum_u32, gsel);
             if (has0) unit_compute(u0, lscale, totA, totB);
             if (has1) unit_compute(u1, lscale, totA, totB);
             __syncwarp();
@@ -1162,7 +1004,6 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
             mbar_init(&sm.red_full[lane - 16], kCW);
             mbar_init(&sm.red_empty[lane - 16], 1);
         }
-        if (lane == 31) *sm.issued = 0;
         if (lane == 30) {
             mbar_init(sm.rx, 1);
             *sm.free_gen = 0;
@@ -1194,18 +1035,12 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
     // and the 16 consumer warps grow to 112 (per scheduler: 32 + 4 x 112 <= 5 x 96 registers per lane)
     if (warp < kAuxWarps) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 32;" ::: "memory");
-        if (warp == 3) return;
+        if (warp >= 2) return;  // warps 2 and 3 only donate their registers
         if (warp == 0) {
             // ================= loader: every byte this CTA needs from HBM, in consumption order =================
-            producer_walk<false>(a, sm, cta, ncta, pos, lane);
+            producer_walk(a, sm, cta, ncta, pos, lane);
             return;
         }
-        if (warp == 2) {
-            // ================= L2 prefetcher: the same walk, kPrefetchAhead stages ahead =================
-            if (a.l2_prefetch) producer_walk<true>(a, sm, cta, ncta, pos, lane);
-            return;
-        }
-    if (warp == 1) {
         // ================= epilogue warp =================
         Red es;
         EpiState st;
@@ -1231,8 +1066,6 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
         __syncwarp();
         if (lane == 0) red_release_gpu(a.done);
         return;
-    }
-        return;  // (not reached: every warp of warpgroup 0 has returned above)
     }
     asm volatile("setmaxnreg.inc.sync.aligned.u32 112;" ::: "memory");
 
@@ -1278,12 +1111,7 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
             inv = stage_rms(a, op, sm, pc, delta, tag_in, gamma, token, p == 0, stage, cta, ctid, cw, lane, p, nphase);
         }
         if (ctid == 0) stamp(a, cta, nphase, p, 1);
-        if (work) {
-            if (op.plan[0].bw[0] == 16 && (op.NG & 15) == 0)
-                consume_gemv_dense(op, sm, rs, cs, inv, cta, ncta, cw, lane);
-            else
-                consume_gemv(op, sm, rs, cs, inv, cta, ncta, cw, lane);
-        }
+        if (work) consume_gemv(op, sm, rs, cs, inv, cta, ncta, cw, lane);
         if (ctid == 0) stamp(a, cta, nphase, p, 2);
         named_bar_sync(1, kConsumerThreads);  // every warp is done with the planes before the next phase overwrites them
         if (pc.on && ctid == 0 && p + 1 < nphase) st_cluster_u32(pc.r_free, (uint32_t)(p + 1));  // (not after the last phase: the partner may be gone)
@@ -1358,52 +1186,6 @@ __global__ void repack_meta_kernel(W4Seg s0, W4Seg s1, W4Seg s2, int nseg, int p
 
 }  // namespace
 
-BoxPlan make_box_plan(int n, int *widths, int *nwidths) {
-    BoxPlan pl{};
-    int w[kMaxBoxes], nb = 0;
-    // Dense boxes of up to 16 groups.  (Odd widths -- 9+9+7+7 -- make the weight LDS.128 conflict free, but rows of 576 / 448 bytes are
-    // not multiples of the 128-byte L2 line: slower end to end when last measured; kept selectable.)
-    const bool odd = getenv("TCE_PK_ODD_BOXES") != nullptr;
-    if (!odd) {
-        w[nb++] = n < 16 ? n : 16;
-        if (n > 16) w[nb++] = n - 16;
-    } else if (n <= 15 && (n & 1)) {
-        w[nb++] = n;
-    } else if (n <= 30) {
-        const int a = ((n / 2) & 1) ? n / 2 : n / 2 + 1;  // two odd parts
-        w[nb++] = a;
-        w[nb++] = n - a;
-    } else if (n == 31) {
-        w[nb++] = 15;
-        w[nb++] = 15;
-        w[nb++] = 1;
-    } else {  // 32
-        w[nb++] = 9;
-        w[nb++] = 9;
-        w[nb++] = 7;
-        w[nb++] = 7;
-    }
-    int g0 = 0, off = 0;
-    for (int i = 0; i < nb; i++) {
-        pl.b0[i] = g0;
-        pl.bw[i] = w[i];
-        pl.off[i] = off;
-        int m = -1;
-        for (int k = 0; k < *nwidths; k++)
-            if (widths[k] == w[i]) m = k;
-        if (m < 0 && *nwidths < kMapsPerMat) {
-            m = (*nwidths)++;
-            widths[m] = w[i];
-        }
-        pl.map[i] = m;  // -1: more distinct widths than maps (caller rejects)
-        g0 += w[i];
-        off += 16 * w[i] * 64;
-        pl.bytes += 16 * w[i] * 64;
-    }
-    pl.nbox = nb;
-    return pl;
-}
-
 int attn_scratch_bytes(int nrep) { return 8 * 136 * 2 + kCW * nrep * 128 * 4 + kCW * nrep * 2 * 4; }
 
 int attn_nsplit_max(int ncta, int KVH, int max_ctx) {
@@ -1477,8 +1259,6 @@ bool pair_supported(Ctx *ctx, const Args &a) {
     }
     return nclusters * 2 >= ctx->num_sms;
 }
-
-cudaError_t set_poll_backoff(unsigned ns) { return cudaMemcpyToSymbol(g_poll_ns, &ns, sizeof(ns)); }
 
 cudaError_t launch(Ctx *ctx, const Args &a, cudaStream_t stream) {
     const size_t smem = smem_bytes(a);

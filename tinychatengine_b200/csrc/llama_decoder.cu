@@ -416,9 +416,10 @@ void LlamaDecoder::build_ops() {
     }
 }
 
-// Everything the persistent decode kernel (decode_persistent.cu) needs beyond the caller's weights: one 2-D tensor map per packed
-// matrix, the per-stage scales|zeros records (a one-off repack of the QM_CUDA scales / zeros arrays into the order the TMA ring
-// consumes them: SURVEY.md 8(f)2 "repack once into the TMA-friendly interleave"), the layer table and the tagged hand-off buffers.
+// Everything the persistent decode kernel (decode_persistent.cu) needs beyond the caller's weights: one 3-D tensor map per packed
+// matrix (the [group][row][64 B] view, see pk::GemvOp), the per-stage scales|zeros records (a one-off repack of the QM_CUDA scales /
+// zeros arrays into the order the TMA ring consumes them: SURVEY.md 8(f)2 "repack once into the TMA-friendly interleave"), the layer
+// table and the tagged hand-off buffers.
 cudaError_t LlamaDecoder::build_persistent(std::string *err) {
     const int E = cfg_.embed_dim, F = cfg_.hidden_dim, H = cfg_.num_heads, KVH = cfg_.num_kv_heads, hd = cfg_.head_dim, V = cfg_.vocab_size;
     const int Lyr = cfg_.num_layers, ncta = ctx_->num_sms;
@@ -446,8 +447,6 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         o.epi = epi;
         return o;
     };
-    // TMA box plans (odd box widths, see persistent.h) and the distinct widths each op needs a tensor map for
-    int widths[pk::OPI_COUNT][pk::kMapsPerMat] = {}, nwidths[pk::OPI_COUNT] = {};
     const bool tp = tp_ > 1;
     a.op[pk::OPI_QKV] = mk(E, (H + 2 * KVH) * hd, 3, 0, H * hd, KVH * hd, pk::PX_RMS_F32, pk::PE_HALF_LL);
     a.op[pk::OPI_O] = mk(H * hd, E, 1, 0, E, 0, pk::PX_HALF, pk::PE_DELTA_LL);
@@ -456,14 +455,7 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
     a.op[pk::OPI_LMHEAD] = mk(E, V, 1, 0, V, 0, pk::PX_RMS_F32, pk::PE_LOGITS);
     int max_ic = 0, max_ng = 0;
     for (int i = 0; i < pk::OPI_COUNT; i++) {
-        const int NG = a.op[i].NG, full = NG < pk::kStageGroups ? NG : pk::kStageGroups, rem = NG % pk::kStageGroups;
-        a.op[i].plan[0] = pk::make_box_plan(full, widths[i], &nwidths[i]);
-        a.op[i].plan[1] = (NG > pk::kStageGroups && rem) ? pk::make_box_plan(rem, widths[i], &nwidths[i]) : a.op[i].plan[0];
-        for (int k = 0; k < pk::kMaxBoxes; k++)
-            if ((k < a.op[i].plan[0].nbox && a.op[i].plan[0].map[k] < 0) || (k < a.op[i].plan[1].nbox && a.op[i].plan[1].map[k] < 0)) return no("too many box widths");
-        // unit boxes ([group][row][64 B], conflict-free LDS.128) where the dense consumer applies (every stage made of 16-group boxes)
-        static const bool want_units = !getenv("TCE_PK_UNIT_BOXES") || atoi(getenv("TCE_PK_UNIT_BOXES")) != 0;  // default on
-        a.op[i].unit = (want_units && a.op[i].plan[0].bw[0] == 16 && (NG & 15) == 0) ? 1 : 0;
+        a.op[i].bw = a.op[i].NG < 16 ? a.op[i].NG : 16;
         if (a.op[i].IC > max_ic) max_ic = a.op[i].IC;
         if (a.op[i].NG > max_ng) max_ng = a.op[i].NG;
         if (a.op[i].IC % kW4Group || a.op[i].num_tiles < 1) return no("bad GEMV shape");
@@ -476,14 +468,8 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
     a.max_ng = max_ng;
     a.E = E;
     a.nst = pk::pick_stages(ctx_->smem_optin, xs, max_ng, E);
-    if (getenv("TCE_PK_STAGES")) {
-        const int want = atoi(getenv("TCE_PK_STAGES"));
-        if (want >= 2 && want < a.nst) a.nst = want;
-    }
     if (a.nst < 2) return no("shared memory too small for the persistent kernel");
-    a.l2_prefetch = getenv("TCE_PK_L2_PREFETCH") ? atoi(getenv("TCE_PK_L2_PREFETCH")) : 0;
     a.pair = 0;  // decided below, once the shared-memory footprint is known
-    if (getenv("TCE_PK_POLL_NS")) DCK(pk::set_poll_backoff((unsigned)atoi(getenv("TCE_PK_POLL_NS"))));
 
     auto dalloc = [&](size_t bytes) -> void * {
         void *p = nullptr;
@@ -493,7 +479,7 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
     };
     cudaStream_t s = ctx_->stream;
     // ---- tensor maps: [Lyr][7] + lm_head + KV cache ----
-    std::vector<CUtensorMap> maps(((size_t)Lyr * 7 + 1) * pk::kMapsPerMat + 1);
+    std::vector<CUtensorMap> maps((size_t)Lyr * 7 + 2);
     memset(maps.data(), 0, maps.size() * sizeof(CUtensorMap));
     std::vector<pk::LayerDesc> descs(Lyr);
     const size_t per_kv = (size_t)KVH * cfg_.max_ctx;  // rows per (layer, K|V) slab
@@ -503,9 +489,7 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         const int opi[7] = {pk::OPI_QKV, pk::OPI_QKV, pk::OPI_QKV, pk::OPI_O, pk::OPI_GATEUP, pk::OPI_GATEUP, pk::OPI_DOWN};
         for (int i = 0; i < 7; i++) {
             const pk::GemvOp &o = a.op[opi[i]];
-            for (int k = 0; k < nwidths[opi[i]]; k++)
-                DCK((o.unit ? encode_w4_tmap_units : encode_w4_tmap)(&maps[((size_t)l * 7 + i) * pk::kMapsPerMat + k], t7[i]->w, t7[i]->oc, t7[i]->ic, widths[opi[i]][k],
-                                                                   o.pair ? 8 : 16));
+            DCK(encode_w4_tmap_units(&maps[(size_t)l * 7 + i], t7[i]->w, t7[i]->oc, t7[i]->ic, o.bw, o.pair ? 8 : 16));
         }
         pk::LayerDesc &D = descs[l];
         memset(&D, 0, sizeof(D));
@@ -529,15 +513,13 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
     }
     {
         const pk::GemvOp &o = a.op[pk::OPI_LMHEAD];
-        for (int k = 0; k < nwidths[pk::OPI_LMHEAD]; k++)
-            DCK((o.unit ? encode_w4_tmap_units : encode_w4_tmap)(&maps[(size_t)Lyr * 7 * pk::kMapsPerMat + k], w_.lm_head.w, w_.lm_head.oc, w_.lm_head.ic,
-                                                               widths[pk::OPI_LMHEAD][k], 16));
+        DCK(encode_w4_tmap_units(&maps[(size_t)Lyr * 7], w_.lm_head.w, w_.lm_head.oc, w_.lm_head.ic, o.bw, 16));
         uint8_t *m = (uint8_t *)dalloc((size_t)o.num_tiles * o.S * pk::kMetaBytes);
         if (!m) return cudaErrorMemoryAllocation;
         const W4Seg lm[1] = {seg_of(w_.lm_head)};
         DCK(pk::repack_meta(ctx_, lm, 1, 0, o.IC, m, s));
         a.lm_meta = m;
-        DCK(pk::encode_kv_tmap(&maps[((size_t)Lyr * 7 + 1) * pk::kMapsPerMat], d_kv_, (long long)Lyr * 2 * per_kv));
+        DCK(pk::encode_kv_tmap(&maps[(size_t)Lyr * 7 + 1], d_kv_, (long long)Lyr * 2 * per_kv));
     }
     CUtensorMap *dmaps = (CUtensorMap *)dalloc(maps.size() * sizeof(CUtensorMap));
     pk::LayerDesc *ddesc = (pk::LayerDesc *)dalloc(descs.size() * sizeof(pk::LayerDesc));

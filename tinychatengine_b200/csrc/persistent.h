@@ -12,45 +12,35 @@ namespace tce {
 namespace pk {
 
 constexpr int kCW = 16;                          // consumer warps
-constexpr int kAuxWarps = 4;                     // warpgroup 0: loader warp, epilogue warp, L2-prefetch warp, one spare warp that only donates its registers
+constexpr int kAuxWarps = 4;                     // warpgroup 0: loader warp, epilogue warp, two spare warps that only donate their registers
 constexpr int kThreads = 32 * (kAuxWarps + kCW); // 640
 constexpr int kConsumerThreads = 32 * kCW;       // 512
 constexpr int kStageGroups = 32;                 // 128-k groups per ring stage: every consumer warp owns two of them
 constexpr int kHalfBytes = 16384;                // 64 K rows or 64 V rows (one half of an attention stage)
-constexpr int kMaxBoxes = 4;                     // TMA boxes per weight stage
-constexpr int kMapsPerMat = 4;                   // tensor maps per weight matrix (one per distinct box width)
 constexpr int kMetaOff = 2 * kHalfBytes;         // scales half[32 groups][8][2] (rows g, g+8 adjacent; 1 KiB) then zero points u8[32 groups][8][2] (512 B)
 constexpr int kMetaBytes = 1536;
 constexpr int kStageBytes = 34816;               // 32 KiB + 1.5 KiB meta (+ pad), 1 KiB multiple (128B-swizzle atoms of the K/V boxes)
 constexpr int kMaxStages = 6;
 constexpr int kRedBufs = 3;
 constexpr int kKvChunk = 64;                     // cached positions per ring stage (K rows in the first half, V rows in the second)
-constexpr int kAttnCps = 1;                      // least chunks per attention CTA: as many CTAs as the context has chunks take part, so that a CTA's K/V stages
-                                                 // fit the ring slots left free by the tail of the q|k|v GEMV (a 4-chunk CTA waited ~3 us for its last stage)
 
 enum XMode : int { PX_HALF = 0, PX_RMS_F32 = 1 };
 enum Epi : int { PE_HALF_LL = 0, PE_DELTA_LL = 1, PE_SILU_LL = 2, PE_LOGITS = 3 };
 enum OpIdx : int { OPI_QKV = 0, OPI_O = 1, OPI_GATEUP = 2, OPI_DOWN = 3, OPI_LMHEAD = 4, OPI_COUNT = 5 };
 
-// shape of one GEMV op; identical for every layer, so it lives in the kernel parameter block
-// A stage's <= 32 groups arrive as up to four 2-D TMA boxes (by default two dense boxes of 16 groups; see make_box_plan).
-struct BoxPlan {
-    int nbox;
-    int b0[kMaxBoxes];   // first group of the box within the stage
-    int bw[kMaxBoxes];   // width in groups (<= 16)
-    int off[kMaxBoxes];  // byte offset of the box inside the stage (1 KiB multiple)
-    int map[kMaxBoxes];  // which of the matrix's tensor maps has this box width
-    int bytes;           // sum over boxes of 16 * bw * 64
-};
+// shape of one GEMV op; identical for every layer, so it lives in the kernel parameter block.
+// Weights arrive through one 3-D tensor map per matrix, the view [group][row][64 B] (encode_w4_tmap_units), in boxes of `bw` groups:
+// stage s of a tile carries groups 32s .. min(32s + 32, NG) - 1 as one box per 16 groups, box b at stage offset b * 16 KiB.  So group gi of
+// a stage always sits at gi KiB (gate | up: the 8 gate rows at gi * 512 B, the 8 up rows 8 KiB further), whatever the shape; a box that
+// runs past NG is zero-filled by TMA and still counts its full bytes.
 struct GemvOp {
     int IC, NG;          // input channels, 128-groups per row
-    BoxPlan plan[2];     // [0] a full stage (min(32, NG) groups), [1] the last stage of a tile when NG % 32 != 0
+    int bw;              // TMA box width in groups: min(16, NG)
     int S;               // stages per 16-row tile = ceil(NG / 32)
     int num_tiles;       // 16-row tiles (pair mode: 8 gate rows + 8 up rows)
     int nseg, pair;      // row segments (q|k|v = 3); pair = gate/up interleave
     int rows0, rows1;    // rows of segments 0 and 1 (tile -> segment)
     int x_mode, epi;
-    int unit;            // 1: the op's tensor maps are the 3-D [group][row][64 B] views: a (tile, group) unit is 1 KiB contiguous in the stage
 };
 
 struct LayerDesc {       // per layer, global memory
@@ -65,7 +55,7 @@ struct Args {
     GemvOp op[OPI_COUNT];
     const LayerDesc *layers;
     int num_layers;
-    const CUtensorMap *maps;     // [num_layers][7 (q k v o gate up down)][kMapsPerMat], then lm_head [kMapsPerMat], then the KV cache map
+    const CUtensorMap *maps;     // [num_layers][7 (q k v o gate up down)], then lm_head, then the KV cache map
     const uint8_t *lm_meta;
     const float *final_norm;
     const __half *embed;         // [rows][E]
@@ -88,7 +78,6 @@ struct Args {
     int H, KVH, nrep, max_ctx, E, V, F;
     int nsplit_max;
     int nst;                     // ring depth
-    int l2_prefetch;             // 1: a second producer warp prefetches the stages into L2 ahead of the loader
     int pair;                    // 1: launched as clusters of two CTAs that share the activation staging: each polls and quantises every other
                                  // 128-group and mirrors the result into its partner's shared memory (st.async over DSMEM)
     int xs_bytes;                // activation-plane buffer (also the attention scratch)
@@ -107,13 +96,10 @@ int pick_stages(int smem_optin, int xs_bytes, int max_ng, int E);
 int attn_scratch_bytes(int nrep);
 int attn_nsplit_max(int ncta, int KVH, int max_ctx);
 cudaError_t launch(Ctx *ctx, const Args &a, cudaStream_t stream);
-bool pair_supported(Ctx *ctx, const Args &a);
-cudaError_t set_poll_backoff(unsigned ns);  // pause of a failed hand-off poll before it asks L2 again (default 100 ns)  // the grid fits as co-resident clusters of two CTAs
+bool pair_supported(Ctx *ctx, const Args &a);  // the grid fits as co-resident clusters of two CTAs
 // one-off repack of a (possibly multi-segment / gate-up paired) matrix's scales and zeros into per-stage records
 cudaError_t repack_meta(Ctx *ctx, const W4Seg *segs, int nseg, int pair, int IC, uint8_t *out, cudaStream_t stream);
 cudaError_t encode_kv_tmap(CUtensorMap *out, const void *kv, long long rows);
-// split n <= 32 groups into odd-width boxes; `widths` collects the distinct widths (<= kMapsPerMat) of the op
-BoxPlan make_box_plan(int n, int *widths, int *nwidths);
 
 }  // namespace pk
 }  // namespace tce
