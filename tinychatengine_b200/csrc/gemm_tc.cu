@@ -1,8 +1,8 @@
-// gemm_tc.cu -- instantiations of the wgmma GEMM for the two large-M slots of the path:
+// gemm_tc.cu -- the large-M slots of the path that are not the CTA-pair GEMM (gemm_tc2.cu):
 //   * W4A16 prefill (MatmulOperator::gemm_forward_cuda, declared-but-undefined in the reference, kernels/matmul.h:142-145): the
 //     QM_CUDA int4 weights are expanded once per call to fp16 ((q - z) * s, one rounding) into an L2-resident scratch by a
-//     bandwidth-bound kernel, then C = X * W16^T runs on the tensor cores with fp32 accumulation.  Expanding once per call
-//     instead of once per M tile keeps the CUDA-core dequant work at OC*IC instead of OC*IC*ceil(M/128).
+//     bandwidth-bound kernel (here), then C = X * W16^T runs on the tensor cores with fp32 accumulation (gemm_tc2.cu).  Expanding
+//     once per call instead of once per M tile keeps the CUDA-core dequant work at OC*IC instead of OC*IC*ceil(M/128).
 //   * W8A8 (mat_mul_accelerator_int8_fast_2x2_32unroll* at M >= 16, kernels/ref/matmul_ref_int8.cc:11-159): wgmma s8 x s8 with
 //     int32 accumulation is exact, the float epilogue keeps the reference's evaluation order -> bit-identical int8 / fp32 outputs.
 #include "gemm_tc.cuh"
@@ -12,8 +12,6 @@
 namespace tce {
 namespace {
 
-using tc::EpiAddF32;
-using tc::EpiHalf;
 using tc::GemmArgs;
 
 // ------------------------------------------------------------------------------------------------ epilogues
@@ -66,39 +64,20 @@ __global__ void w4_expand_kernel(const uint32_t *__restrict__ w, const uint32_t 
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-template <int BLOCK_N, int STAGES, bool I8, class Epi>
-cudaError_t launch(Ctx *ctx, GemmArgs &a, const void *A, long long lda, const void *B, long long ldb, long long K) {
-    cudaError_t e = tc::encode_kmajor(&a.tmA, A, I8, a.M, K, lda, tc::kBlockM);
+template <int BLOCK_N, int STAGES, class Epi>
+cudaError_t launch(Ctx *ctx, GemmArgs &a, const int8_t *A, const int8_t *B, long long K) {
+    cudaError_t e = tc::encode_kmajor(&a.tmA, A, true, a.M, K, K, tc::kBlockM);
     if (e != cudaSuccess) return e;
-    e = tc::encode_kmajor(&a.tmB, B, I8, a.N, K, ldb, BLOCK_N / 2);
+    e = tc::encode_kmajor(&a.tmB, B, true, a.N, K, K, BLOCK_N / 2);
     if (e != cudaSuccess) return e;
-    a.k_blocks = (int)(K * (I8 ? 1 : 2) / tc::kAtomBytes);
-    return tc::launch_wg<BLOCK_N, STAGES, I8, false, 1, Epi>(ctx, a);
+    a.k_blocks = (int)(K / tc::kAtomBytes);
+    return tc::launch_wg<BLOCK_N, STAGES, true, 1, Epi>(ctx, a);
 }
 
-// Tile width by wave quantisation: a persistent grid of `sms` CTAs needs ceil(tiles / sms) rounds, each costing ~BLOCK_N (the MMA
-// time of one tile) times a penalty for the narrower tile (the 128-row A tile is re-read once per N block); the 1.12 is a guess, not measured on H100.
-int pick_block_n(int M, int N, int sms) {
-    const long long mb = (M + 127) / 128;
-    const int bn[2] = {256, 128};
-    const double pen[2] = {1.00, 1.12};
-    int best = 256;
-    double best_cost = 1e30;
-    for (int i = 0; i < 2; i++) {
-        const long long tiles = mb * ((N + bn[i] - 1) / bn[i]);
-        const double cost = (double)((tiles + sms - 1) / sms) * bn[i] * pen[i];
-        if (cost < best_cost) {
-            best_cost = cost;
-            best = bn[i];
-        }
-    }
-    return best;
-}
-
-template <class Epi, bool I8>
-cudaError_t dispatch(Ctx *ctx, GemmArgs &a, const void *A, long long lda, const void *B, long long ldb, long long K) {
-    if (pick_block_n(a.M, a.N, ctx->num_sms) == 256) return launch<256, 4, I8, Epi>(ctx, a, A, lda, B, ldb, K);
-    return launch<128, 6, I8, Epi>(ctx, a, A, lda, B, ldb, K);
+template <class Epi>
+cudaError_t dispatch(Ctx *ctx, GemmArgs &a, const int8_t *A, const int8_t *B, long long K) {
+    if (tc::pick_block_n((a.M + tc::kBlockM - 1) / tc::kBlockM, a.N, ctx->num_sms) == 256) return launch<256, 4, Epi>(ctx, a, A, B, K);
+    return launch<128, 6, Epi>(ctx, a, A, B, K);
 }
 
 }  // namespace
@@ -123,19 +102,6 @@ cudaError_t launch_w4_expand(Ctx *ctx, const uint32_t *w, const uint32_t *zeros,
     return cudaGetLastError();
 }
 
-// C[M][N] = A[M][K] fp16 * B[N][K]^T fp16, fp32 accumulation; C is fp16 (stored) or, with add_f32, fp32 (accumulated into).  K % 64 == 0, pointers 16-byte aligned, lda/ldb % 8 == 0.
-cudaError_t launch_gemm_f16_tc(Ctx *ctx, const __half *A, long long lda, const __half *B, long long ldb, void *C, long long ldc, int M, int N, int K,
-                               int add_f32) {
-    if (M < 1 || N < 1 || K < 64 || (K % 64) || (lda % 8) || (ldb % 8)) return cudaErrorInvalidValue;
-    GemmArgs a = {};
-    a.M = M;
-    a.N = N;
-    a.C = C;
-    a.ldc = ldc;
-    if (add_f32) return dispatch<EpiAddF32, false>(ctx, a, A, lda, B, ldb, K);
-    return dispatch<EpiHalf, false>(ctx, a, A, lda, B, ldb, K);
-}
-
 // the four non-batched W8A8 variants on the int8 tensor cores.  K % 128 == 0 (one swizzle atom), pointers 16-byte aligned.
 cudaError_t launch_w8a8_tc(Ctx *ctx, const W8A8Args &w) {
     if (w.batch || w.M < 1 || w.N < 1 || w.K < 128 || (w.K % 128)) return cudaErrorInvalidValue;
@@ -150,10 +116,10 @@ cudaError_t launch_w8a8_tc(Ctx *ctx, const W8A8Args &w) {
     a.q_min = w.q_min;
     a.q_max = w.q_max;
     switch (w.variant) {
-        case W8_BIAS8_O8: a.C = w.C8; return dispatch<EpiW8<W8_BIAS8_O8>, true>(ctx, a, w.A, w.K, w.B, w.K, w.K);
-        case W8_NOBIAS_O8: a.C = w.C8; return dispatch<EpiW8<W8_NOBIAS_O8>, true>(ctx, a, w.A, w.K, w.B, w.K, w.K);
-        case W8_BIASF_OF32: a.C = w.Cf; return dispatch<EpiW8<W8_BIASF_OF32>, true>(ctx, a, w.A, w.K, w.B, w.K, w.K);
-        case W8_NOBIAS_OF32: a.C = w.Cf; return dispatch<EpiW8<W8_NOBIAS_OF32>, true>(ctx, a, w.A, w.K, w.B, w.K, w.K);
+        case W8_BIAS8_O8: a.C = w.C8; return dispatch<EpiW8<W8_BIAS8_O8>>(ctx, a, w.A, w.B, w.K);
+        case W8_NOBIAS_O8: a.C = w.C8; return dispatch<EpiW8<W8_NOBIAS_O8>>(ctx, a, w.A, w.B, w.K);
+        case W8_BIASF_OF32: a.C = w.Cf; return dispatch<EpiW8<W8_BIASF_OF32>>(ctx, a, w.A, w.B, w.K);
+        case W8_NOBIAS_OF32: a.C = w.Cf; return dispatch<EpiW8<W8_NOBIAS_OF32>>(ctx, a, w.A, w.B, w.K);
     }
     return cudaErrorInvalidValue;
 }

@@ -11,10 +11,7 @@
 // CL = 2 (CTA pairs): the two CTAs of a cluster own two vertically adjacent 128-row tiles of the same N block.  Each CTA fetches half
 // of the B tile and multicasts it into both CTAs' shared memory, so every weight byte leaves L2 once per 256 output rows.
 //
-// FUSED: B is the packed QM_CUDA int4 matrix.  TMA brings BLOCK_N rows x 32 bytes of nibbles per k-block; dequant warps (one thread per
-// weight row) turn them into the fp16 SWIZZLE_128B operand tile ((q - z) * s, one rounding), fence.proxy.async, arrive on the operand ring.
-//
-// Roles: warps 0-7 = consumers (warpgroup w owns tile rows 64w..64w+63), warp 8 = TMA producer, FUSED: warps 9.. = dequant.
+// Roles: warps 0-7 = consumers (warpgroup w owns tile rows 64w..64w+63), warp 8 = TMA producer, warps 9-11 idle.
 #pragma once
 #include <cuda.h>
 
@@ -30,19 +27,15 @@ constexpr int kBlockM = 128;
 constexpr int kAtomBytes = 128;  // bytes of K per row per stage = one SWIZZLE_128B atom
 constexpr int kABytes = kBlockM * kAtomBytes;  // 16 KiB
 constexpr int kConsumerThreads = 256;
-constexpr int kOpStages = 3;     // FUSED: ring of dequantised fp16 weight tiles
+constexpr int kThreads = kConsumerThreads + 128;
 
 struct GemmArgs {
     alignas(64) CUtensorMap tmA;  // [M][K] box {128 B, 128 rows}, SWIZZLE_128B
-    alignas(64) CUtensorMap tmB;  // [N][K] box {128 B, BLOCK_N / 2 rows}, SWIZZLE_128B; FUSED: uint32 [N][K/8], box {8, BLOCK_N / 2}, no swizzle
+    alignas(64) CUtensorMap tmB;  // [N][K] box {128 B, BLOCK_N / 2 rows}, SWIZZLE_128B
     int M, N;
     int k_blocks;                 // K * sizeof(element) / 128
     int m_blocks, n_blocks;       // m_blocks counts rows of 128 * CL
     int silu_F;                   // > 0: B = [gate (F rows); up (F rows)]; tile columns 0..127 = gate, 128..255 = up of the SAME 128 channels
-    // FUSED
-    const __half *scales;
-    const uint32_t *zeros;
-    int sf_w, zeros_w;
     // epilogue
     void *C;
     long long ldc;                // elements between output rows
@@ -125,58 +118,37 @@ TCE_DEVINL uint64_t make_sw128_desc(uint32_t smem_addr) {
     return ((uint64_t)hi << 32) | lo;
 }
 
-template <int BLOCK_N, bool FUSED>
-constexpr int b_stage_bytes() {
-    return BLOCK_N * (FUSED ? 32 : kAtomBytes);
-}
-template <int BLOCK_N, int STAGES, bool FUSED>
+template <int BLOCK_N, int STAGES>
 constexpr size_t smem_bytes() {
-    return 1024 + (size_t)STAGES * (kABytes + b_stage_bytes<BLOCK_N, FUSED>()) + (FUSED ? (size_t)kOpStages * BLOCK_N * kAtomBytes : 0);
-}
-template <int BLOCK_N, bool FUSED>
-constexpr int num_threads() {
-    return FUSED ? kConsumerThreads + 32 + BLOCK_N : kConsumerThreads + 128;
+    return 1024 + (size_t)STAGES * (kABytes + BLOCK_N * kAtomBytes);
 }
 
-// 8 nibbles -> 8 fp16 (q - z) * s in k order
-TCE_DEVINL uint4 dequant_word(uint32_t w, uint32_t zmagic, __half2 s2) {
-    constexpr uint32_t Mk = 0x000F000Fu, MG = 0x64006400u;
-    const __half2 zm = *reinterpret_cast<const __half2 *>(&zmagic);
-    // (1024 + e0, 1024 + e4), (e1, e5), (e2, e6), (e3, e7)
-    uint32_t q[4] = {lop3_and_or(w, Mk, MG), lop3_and_or(w >> 4, Mk, MG), lop3_and_or(w >> 8, Mk, MG), lop3_and_or(w >> 12, Mk, MG)};
-    uint32_t p[4];
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        const __half2 v = __hmul2(__hsub2(*reinterpret_cast<const __half2 *>(&q[i]), zm), s2);  // exact difference, one rounding
-        p[i] = *reinterpret_cast<const uint32_t *>(&v);
-    }
-    return make_uint4(__byte_perm(p[0], p[1], 0x5410), __byte_perm(p[2], p[3], 0x5410), __byte_perm(p[0], p[1], 0x7632), __byte_perm(p[2], p[3], 0x7632));
+// Tile width by wave quantisation: a persistent grid of `ctas` CTAs (or clusters) over row_blocks x ceil(N / BLOCK_N) tiles needs
+// ceil(tiles / ctas) rounds, each costing ~BLOCK_N (the MMA time of one tile), times a penalty for the narrower tile (the A tile is
+// re-read once per N block); the 1.12 is a guess, not measured on H100.  Ties go to 256.
+inline int pick_block_n(long long row_blocks, int N, int ctas) {
+    auto rounds = [&](int bn) { return (row_blocks * ((N + bn - 1) / bn) + ctas - 1) / ctas; };
+    return (double)rounds(128) * 128 * 1.12 < (double)rounds(256) * 256 ? 128 : 256;
 }
 
 // Epilogues see the wgmma fragment two columns at a time: Epi::apply(args, row, col, v0, v1) owns C[row][col], C[row][col + 1] (col even,
 // col < N).  Epi::kSilu: apply(args, row, col, g0, g1, u0, u1) with the gate / up accumulators of channels col, col + 1.
-template <int BLOCK_N, int STAGES, bool I8, bool FUSED, int CL, class Epi>
-__global__ void __launch_bounds__(num_threads<BLOCK_N, FUSED>(), 1) gemm_wg_kernel(const __grid_constant__ GemmArgs a) {
+template <int BLOCK_N, int STAGES, bool I8, int CL, class Epi>
+__global__ void __launch_bounds__(kThreads, 1) gemm_wg_kernel(const __grid_constant__ GemmArgs a) {
     static_assert(BLOCK_N == 128 || BLOCK_N == 256, "BLOCK_N");
-    static_assert(!FUSED || (BLOCK_N == 128 && !I8), "the fused unpack is built for 128-row fp16 operand tiles");
     static_assert(!Epi::kSilu || BLOCK_N == 256, "gate and up share a 256-column tile");
     static_assert(CL == 1 || CL == 2, "CL");
     using Acc = typename std::conditional<I8, int, float>::type;
     constexpr int NH = BLOCK_N / 128;                      // 128-column halves of the tile, one wgmma each
     constexpr int kHalfRows = BLOCK_N / 2;                 // rows per B load (one per CTA of a pair)
-    constexpr int kBBytes = b_stage_bytes<BLOCK_N, FUSED>();
+    constexpr int kBBytes = BLOCK_N * kAtomBytes;
     constexpr int kLdBytes = kABytes + kBBytes;
-    constexpr int kOpBytes = BLOCK_N * kAtomBytes;
-    constexpr int kDqWarps = FUSED ? BLOCK_N / 32 : 0;
-    constexpr int OS = FUSED ? kOpStages : 1;
     extern __shared__ uint8_t smem_raw[];
     // barriers live at identical offsets in both CTAs of a pair (multicast loads and remote arrives address "the same barrier in the other CTA")
-    __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES], op_full[OS], op_empty[OS];
+    __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
 
     const uint32_t raw = smem_u32(smem_raw);
-    uint8_t *tiles = smem_raw + (((raw + 1023u) & ~1023u) - raw);  // SWIZZLE_128B tiles need 1024-byte alignment
-    uint8_t *sLd = tiles;                                           // [STAGES][A 16 KiB | B]
-    uint8_t *sOp = tiles + (size_t)STAGES * kLdBytes;               // FUSED: [OS][dequantised B]
+    uint8_t *sLd = smem_raw + (((raw + 1023u) & ~1023u) - raw);  // [STAGES][A 16 KiB | B]; SWIZZLE_128B tiles need 1024-byte alignment
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t rank = CL == 1 ? 0u : blockIdx.x % CL;
     const int cl = blockIdx.x / CL, ncl = gridDim.x / CL;
@@ -185,11 +157,7 @@ __global__ void __launch_bounds__(num_threads<BLOCK_N, FUSED>(), 1) gemm_wg_kern
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; s++) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], CL * (8 + kDqWarps));  // every warp that reads the slot, in every CTA that is written with it
-        }
-        for (int s = 0; s < OS; s++) {
-            mbar_init(&op_full[s], kDqWarps);
-            mbar_init(&op_empty[s], 8);
+            mbar_init(&empty_bar[s], CL * 8);  // every consumer warp, in every CTA that is written with the slot
         }
         mbar_fence_init();
     }
@@ -199,16 +167,15 @@ __global__ void __launch_bounds__(num_threads<BLOCK_N, FUSED>(), 1) gemm_wg_kern
     if (warp < 8) {
         // ------------------------------------------------------------------------------- consumers: MMA + epilogue
         const int wg = warp >> 2;
-        int s = 0, os = 0;
-        uint32_t ph = 0, oph = 0;
+        int s = 0;
+        uint32_t ph = 0;
         Acc acc[NH][64];
         for (int t = cl; t < tiles_total; t += ncl) {
             const int mb = (t % a.m_blocks) * CL + (int)rank, nb = t / a.m_blocks;
             for (int kb = 0; kb < a.k_blocks; kb++) {
                 mbar_wait(&full_bar[s], ph);
-                if (FUSED) mbar_wait(&op_full[os], oph);
                 const uint32_t aaddr = smem_u32(sLd + (size_t)s * kLdBytes) + (uint32_t)wg * 64u * kAtomBytes;
-                const uint32_t baddr = FUSED ? smem_u32(sOp + (size_t)os * kOpBytes) : smem_u32(sLd + (size_t)s * kLdBytes + kABytes);
+                const uint32_t baddr = smem_u32(sLd + (size_t)s * kLdBytes + kABytes);
                 wg_fence();
 #pragma unroll
                 for (int h = 0; h < NH; h++) {
@@ -219,17 +186,10 @@ __global__ void __launch_bounds__(num_threads<BLOCK_N, FUSED>(), 1) gemm_wg_kern
                 }
                 wg_commit();
                 wg_wait0();  // the other warpgroup's MMAs fill the tensor pipe meanwhile
-                if (lane == 0) {
-                    mbar_release<CL>(&empty_bar[s]);
-                    if (FUSED) mbar_arrive(&op_empty[os]);
-                }
+                if (lane == 0) mbar_release<CL>(&empty_bar[s]);
                 if (++s == STAGES) {
                     s = 0;
                     ph ^= 1u;
-                }
-                if (FUSED && ++os == OS) {
-                    os = 0;
-                    oph ^= 1u;
                 }
             }
 #pragma unroll
@@ -274,7 +234,7 @@ __global__ void __launch_bounds__(num_threads<BLOCK_N, FUSED>(), 1) gemm_wg_kern
                     mbar_arrive_expect_tx(&full_bar[s], kLdBytes);
                     uint8_t *dst = sLd + (size_t)s * kLdBytes;
                     tma_load_2d(dst, &a.tmA, kb * (I8 ? kAtomBytes : kAtomBytes / 2), mb * kBlockM, &full_bar[s]);
-                    const int bx = FUSED ? kb * 8 : kb * (I8 ? kAtomBytes : kAtomBytes / 2);  // element coordinate along K
+                    const int bx = kb * (I8 ? kAtomBytes : kAtomBytes / 2);  // element coordinate along K
 #pragma unroll
                     for (int h = 0; h < 2; h++) {
                         if (CL == 2 && h != (int)rank) continue;  // a pair splits the B tile and multicasts the halves
@@ -291,63 +251,6 @@ __global__ void __launch_bounds__(num_threads<BLOCK_N, FUSED>(), 1) gemm_wg_kern
             }
         }
         __syncwarp();
-    } else if (FUSED) {
-        // ------------------------------------------------------------------------------- dequant warps: thread r owns weight row r of the tile
-        const int r = threadIdx.x - 32 * 9;
-        int ls = 0, os = 0;
-        uint32_t lph = 0, oph = 0;
-        // destination of chunk c (8 fp16) of row r inside a 128B-swizzled K-major tile: 8-row groups of 1024 B, chunk index XOR (row & 7)
-        const uint32_t row_off = (uint32_t)(r >> 3) * 1024u + (uint32_t)(r & 7) * 128u;
-        const uint32_t sw = (uint32_t)(r & 7);
-        for (int t = cl; t < tiles_total; t += ncl) {
-            const int nb = t / a.m_blocks;
-            const int grow = nb * BLOCK_N + r;
-            const bool live = grow < a.N;
-            const __half *srow = a.scales + (size_t)(live ? grow : 0) * a.sf_w;
-            const uint32_t *zrow = a.zeros + (size_t)(live ? grow : 0) * a.zeros_w;
-            // scale / zero point of a 128-k group are requested one group (two k-blocks) before they are used, off the critical path of the ring
-            const int ngroups = a.k_blocks >> 1;
-            uint32_t zword = 0u, zword_nxt = live ? zrow[0] : 0u, zmagic = 0x64006400u;
-            __half s_nxt = live ? srow[0] : __float2half(0.f);
-            __half2 s2 = __float2half2_rn(0.f);
-            for (int kb = 0; kb < a.k_blocks; kb++) {
-                if ((kb & 1) == 0) {  // a new group (rows past N: scale 0 -> zero weights)
-                    const int g = kb >> 1;
-                    if ((g & 7) == 0) {
-                        zword = zword_nxt;
-                        if (live && g + 8 < ngroups) zword_nxt = zrow[(g >> 3) + 1];
-                    }
-                    const uint32_t z = (zword >> (4 * (g & 7))) & 0xFu;
-                    zmagic = 0x64006400u | z | (z << 16);
-                    s2 = __half2half2(s_nxt);
-                    if (live && g + 1 < ngroups) s_nxt = srow[g + 1];
-                }
-                mbar_wait(&full_bar[ls], lph);
-                const uint8_t *src = sLd + (size_t)ls * kLdBytes + kABytes + (size_t)r * 32;
-                const uint4 w0 = *reinterpret_cast<const uint4 *>(src), w1 = *reinterpret_cast<const uint4 *>(src + 16);
-                __syncwarp();
-                if (lane == 0) mbar_release<CL>(&empty_bar[ls]);  // the packed tile is in registers
-                if (++ls == STAGES) {
-                    ls = 0;
-                    lph ^= 1u;
-                }
-                const uint32_t ww[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
-                uint4 o[8];
-#pragma unroll
-                for (int c = 0; c < 8; c++) o[c] = dequant_word(ww[c], zmagic, s2);
-                mbar_wait(&op_empty[os], oph ^ 1u);
-                uint8_t *dst = sOp + (size_t)os * kOpBytes + row_off;
-#pragma unroll
-                for (int c = 0; c < 8; c++) *reinterpret_cast<uint4 *>(dst + (((uint32_t)c ^ sw) << 4)) = o[c];
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes, read by the tensor core (async proxy)
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&op_full[os]);
-                if (++os == OS) {
-                    os = 0;
-                    oph ^= 1u;
-                }
-            }
-        }
     }
     if constexpr (CL == 2) cluster_sync_all();  // the peer may still write this CTA's shared memory and barriers until it is done too
 }
@@ -380,26 +283,13 @@ inline cudaError_t encode_kmajor(CUtensorMap *out, const void *base, bool i8, lo
     return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
-// packed QM_CUDA int4 weights: uint32 [N][K/8], box {8 words = 64 k, box_rows}, no swizzle
-inline cudaError_t encode_w4_packed(CUtensorMap *out, const uint32_t *w, long long N, long long K, int box_rows) {
-    EncodeFn fn = encoder();
-    if (!fn) return cudaErrorNotSupported;
-    const cuuint64_t gdim[2] = {(cuuint64_t)(K / 8), (cuuint64_t)N};
-    const cuuint64_t gstride[1] = {(cuuint64_t)(K / 8) * 4};
-    const cuuint32_t box[2] = {8u, (cuuint32_t)box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, const_cast<uint32_t *>(w), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
-}
-
 // a.tmA / a.tmB, M, N, k_blocks and the epilogue fields are set by the caller; fills the block counts and launches the persistent grid
-template <int BLOCK_N, int STAGES, bool I8, bool FUSED, int CL, class Epi>
+template <int BLOCK_N, int STAGES, bool I8, int CL, class Epi>
 cudaError_t launch_wg(Ctx *ctx, GemmArgs &a) {
     a.m_blocks = (a.M + kBlockM * CL - 1) / (kBlockM * CL);
     a.n_blocks = a.silu_F > 0 ? a.silu_F / 128 : (a.N + BLOCK_N - 1) / BLOCK_N;
-    auto kern = gemm_wg_kernel<BLOCK_N, STAGES, I8, FUSED, CL, Epi>;
-    constexpr size_t smem = smem_bytes<BLOCK_N, STAGES, FUSED>();
+    auto kern = gemm_wg_kernel<BLOCK_N, STAGES, I8, CL, Epi>;
+    constexpr size_t smem = smem_bytes<BLOCK_N, STAGES>();
     static DeviceOnce attr_once;  // per instantiation
     if (attr_once.pending(ctx->device)) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -410,7 +300,7 @@ cudaError_t launch_wg(Ctx *ctx, GemmArgs &a) {
     const int clusters = tiles < ctx->num_sms / CL ? tiles : ctx->num_sms / CL;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)(clusters * CL));
-    cfg.blockDim = dim3((unsigned)num_threads<BLOCK_N, FUSED>());
+    cfg.blockDim = dim3((unsigned)kThreads);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = ctx->stream;
     cudaLaunchAttribute attr[1];
@@ -423,7 +313,7 @@ cudaError_t launch_wg(Ctx *ctx, GemmArgs &a) {
     return cudaLaunchKernelEx(&cfg, kern, a);
 }
 
-// ------------------------------------------------------------------------------------------------ epilogues shared by the fp16 GEMMs
+// ------------------------------------------------------------------------------------------------ epilogues of the fp16 GEMM (gemm_tc2.cu)
 struct EpiHalf {  // fp32 accumulator -> fp16 C
     static constexpr bool kSilu = false;
     TCE_DEVINL static void apply(const GemmArgs &a, int row, int col, float v0, float v1) {

@@ -34,7 +34,6 @@ struct AttnPrefillArgs {
 cudaError_t launch_attn_prefill(Ctx *ctx, const AttnPrefillArgs &a);
 cudaError_t launch_embedding_rows(Ctx *ctx, const __half *table, const int *tokens, float *resid, int n, int E);
 cudaError_t launch_rmsnorm_rows_f32(Ctx *ctx, const float *x, const float *gamma, __half *y, int rows, int dim, float eps);
-cudaError_t launch_silu_mul_rows(Ctx *ctx, const __half *gu, __half *act, int rows, int F);
 
 // resid_f32[E] = (float) table[token][:]   (reference: CPU Embedding + float2half, cuda/Int4llamaDecoder.cu:62-69)
 cudaError_t launch_embedding(Ctx *ctx, const __half *table, const int *token, float *resid, int E, bool pdl, int rows = 0, int max_ctx = 0, int *safe = nullptr);

@@ -160,7 +160,6 @@ LlamaDecoder::~LlamaDecoder() {
     cudaFree(pf_xn_);
     cudaFree(pf_qkv_);
     cudaFree(pf_att_);
-    cudaFree(pf_gu_);
     cudaFree(pf_act_);
     cudaFree(pf_tok_);
     for (void *p : pk_allocs_) cudaFree(p);
@@ -829,10 +828,9 @@ cudaError_t LlamaDecoder::prefill_reserve(int n) {
     cudaFree(pf_xn_);
     cudaFree(pf_qkv_);
     cudaFree(pf_att_);
-    cudaFree(pf_gu_);
     cudaFree(pf_act_);
     cudaFree(pf_tok_);
-    pf_x_ = nullptr; pf_xn_ = nullptr; pf_qkv_ = nullptr; pf_att_ = nullptr; pf_gu_ = nullptr; pf_act_ = nullptr; pf_tok_ = nullptr;
+    pf_x_ = nullptr; pf_xn_ = nullptr; pf_qkv_ = nullptr; pf_att_ = nullptr; pf_act_ = nullptr; pf_tok_ = nullptr;
     pf_cap_ = 0;
     const size_t E = cfg_.embed_dim, F = cfg_.hidden_dim, Q = (size_t)(cfg_.num_heads + 2 * cfg_.num_kv_heads) * cfg_.head_dim,
                  A = (size_t)cfg_.num_heads * cfg_.head_dim;
@@ -840,56 +838,28 @@ cudaError_t LlamaDecoder::prefill_reserve(int n) {
     DCK(cudaMalloc(&pf_xn_, n * E * sizeof(__half)));
     DCK(cudaMalloc(&pf_qkv_, n * Q * sizeof(__half)));
     DCK(cudaMalloc(&pf_att_, n * A * sizeof(__half)));
-    DCK(cudaMalloc(&pf_gu_, n * 2 * F * sizeof(__half)));
     DCK(cudaMalloc(&pf_act_, n * F * sizeof(__half)));
     DCK(cudaMalloc(&pf_tok_, n * sizeof(int)));
     pf_cap_ = n;
     return cudaSuccess;
 }
 
-// C[n][sum oc] (row-major, leading dimension ldc) = X[n][ic] * [deq(t0); deq(t1); ...]^T : the `count` weight matrices (same ic) are
-// expanded into consecutive row ranges of the fp16 scratch and multiplied by ONE GEMM (q|k|v and gate|up share their input)
-cudaError_t LlamaDecoder::prefill_linear(const tce_w4_tensor *const *ts, int count, const __half *x, void *C, long long ldc, int n, bool add_f32, bool silu) {
-    const int ic = ts[0]->ic;
-    const int mode = w4_gemm_mode();
-    if (mode == W4G_FUSED || mode == W4G_PAIR_FUSED) {
-        // one launch per tensor, each writing its column range of C: the packed weights are unpacked inside the GEMM's tile pipeline
-        size_t c0 = 0;
-        for (int i = 0; i < count; i++) {
-            const tce_w4_tensor &t = *ts[i];
-            void *Ci = add_f32 ? static_cast<void *>(static_cast<float *>(C) + c0) : static_cast<void *>(static_cast<__half *>(C) + c0);
-            if (mode == W4G_PAIR_FUSED)
-                DCK(launch_gemm_w4_pair(ctx_, x, ic, (const uint32_t *)t.w, (const uint32_t *)t.zeros, (const __half *)t.scales, Ci, ldc, n, t.oc, ic, add_f32 ? 1 : 0));
-            else
-                DCK(launch_gemm_w4_tc(ctx_, x, ic, (const uint32_t *)t.w, (const uint32_t *)t.zeros, (const __half *)t.scales, Ci, ldc, n, t.oc, ic, add_f32 ? 1 : 0));
-            c0 += (size_t)t.oc;
-        }
-        return cudaSuccess;
-    }
+// C[n][rows] (row-major, leading dimension ldc) = X[n][ic] * W^T, W = the weights of job j stacked (q|k|v and gate|up share their input),
+// expanded to fp16 on the side stream while the previous GEMM ran.  epi: EPI_STORE_HALF, EPI_ADD_F32 (residual add) or EPI_SILU_MUL_HALF
+// (job = gate|up, C = SiLU(gate) * up)
+cudaError_t LlamaDecoder::prefill_linear(int j, const __half *x, void *C, long long ldc, int n, EpiMode epi) {
+    const PfJob &job = pf_jobs_[j];
+    const int ic = job.ts[0]->ic, b = j & 1;
     size_t rows = 0;
-    for (int i = 0; i < count; i++) rows += (size_t)ts[i]->oc;
-    if (mode == W4G_PAIR_OVERLAP && !pf_jobs_.empty()) {
-        // this job's weights were expanded on the side stream while the previous GEMM ran; queue the next job's expansion, then run
-        const int j = pf_next_job_++;
-        const int b = j & 1;
-        if (j + 1 < (int)pf_jobs_.size()) DCK(pf_expand_job(j + 1));
-        DCK(cudaStreamWaitEvent(ctx_->stream, pf_expanded_[b], 0));
-        if (silu)
-            DCK(launch_gemm_f16_pair_silu(ctx_, x, ic, pf_w16_[b], ic, (__half *)C, ldc, n, (int)(rows / 2), ic));
-        else
-            DCK(launch_gemm_f16_pair(ctx_, x, ic, pf_w16_[b], ic, C, ldc, n, (int)rows, ic, add_f32 ? 1 : 0));
-        return cudaEventRecord(pf_consumed_[b], ctx_->stream);
-    }
-    DCK(w4_scratch_reserve(ctx_, rows * ic));
-    size_t r0 = 0;
-    for (int i = 0; i < count; i++) {
-        const tce_w4_tensor &t = *ts[i];
-        DCK(launch_w4_expand(ctx_, (const uint32_t *)t.w, (const uint32_t *)t.zeros, (const __half *)t.scales, ctx_->w16_scratch + r0 * ic, t.oc, ic));
-        r0 += (size_t)t.oc;
-    }
-    if (silu) return launch_gemm_f16_pair_silu(ctx_, x, ic, ctx_->w16_scratch, ic, (__half *)C, ldc, n, (int)(rows / 2), ic);
-    if (mode == W4G_PAIR || mode == W4G_PAIR_OVERLAP) return launch_gemm_f16_pair(ctx_, x, ic, ctx_->w16_scratch, ic, C, ldc, n, (int)rows, ic, add_f32 ? 1 : 0);
-    return launch_gemm_f16_tc(ctx_, x, ic, ctx_->w16_scratch, ic, C, ldc, n, (int)rows, ic, add_f32 ? 1 : 0);
+    for (int i = 0; i < job.count; i++) rows += (size_t)job.ts[i]->oc;
+    // queue the next job's expansion, then run this one
+    if (j + 1 < (int)pf_jobs_.size()) DCK(pf_expand_job(j + 1));
+    DCK(cudaStreamWaitEvent(ctx_->stream, pf_expanded_[b], 0));
+    if (epi == EPI_SILU_MUL_HALF)
+        DCK(launch_gemm_f16_pair_silu(ctx_, x, ic, pf_w16_[b], ic, (__half *)C, ldc, n, (int)(rows / 2), ic));
+    else
+        DCK(launch_gemm_f16_pair(ctx_, x, ic, pf_w16_[b], ic, C, ldc, n, (int)rows, ic, epi == EPI_ADD_F32 ? 1 : 0));
+    return cudaEventRecord(pf_consumed_[b], ctx_->stream);
 }
 
 // expansion of job j into scratch half (j & 1) on the side stream, after the GEMM that last read that half
@@ -918,35 +888,32 @@ cudaError_t LlamaDecoder::prefill(const int *tokens_host, int n, int pos0, float
     for (int i = 0; i < n; i++)
         if (tokens_host[i] < 0 || tokens_host[i] >= cfg_.vocab_size) return cudaErrorInvalidValue;
     DCK(prefill_reserve(n));
-    if (w4_gemm_mode() == W4G_PAIR_OVERLAP) {
-        if (pf_jobs_.empty()) {
-            size_t need = 0;
-            for (int l = 0; l < cfg_.num_layers; l++) {
-                const tce_llama_layer &L = layers_[l];
-                pf_jobs_.push_back(PfJob{{&L.q, &L.k, &L.v}, 3});
-                pf_jobs_.push_back(PfJob{{&L.o, nullptr, nullptr}, 1});
-                pf_jobs_.push_back(PfJob{{&L.gate, &L.up, nullptr}, 2});
-                pf_jobs_.push_back(PfJob{{&L.down, nullptr, nullptr}, 1});
-            }
-            for (const PfJob &jb : pf_jobs_) {
-                size_t e = 0;
-                for (int i = 0; i < jb.count; i++) e += (size_t)jb.ts[i]->oc * jb.ts[i]->ic;
-                need = e > need ? e : need;
-            }
-            for (int b = 0; b < 2; b++) {
-                DCK(cudaMalloc((void **)&pf_w16_[b], need * sizeof(__half)));
-                DCK(cudaEventCreateWithFlags(&pf_expanded_[b], cudaEventDisableTiming));
-                DCK(cudaEventCreateWithFlags(&pf_consumed_[b], cudaEventDisableTiming));
-            }
-            pf_w16_elems_ = need;
-            DCK(cudaStreamCreateWithFlags(&pf_side_, cudaStreamNonBlocking));
+    if (pf_jobs_.empty()) {
+        size_t need = 0;
+        for (int l = 0; l < cfg_.num_layers; l++) {
+            const tce_llama_layer &L = layers_[l];
+            pf_jobs_.push_back(PfJob{{&L.q, &L.k, &L.v}, 3});
+            pf_jobs_.push_back(PfJob{{&L.o, nullptr, nullptr}, 1});
+            pf_jobs_.push_back(PfJob{{&L.gate, &L.up, nullptr}, 2});
+            pf_jobs_.push_back(PfJob{{&L.down, nullptr, nullptr}, 1});
         }
-        pf_next_job_ = 0;
-        // the side stream starts after everything already queued on the main stream (a previous prompt's GEMMs read the scratch)
-        DCK(cudaEventRecord(pf_consumed_[0], ctx_->stream));
-        DCK(cudaStreamWaitEvent(pf_side_, pf_consumed_[0], 0));
-        DCK(pf_expand_job(0));
+        for (const PfJob &jb : pf_jobs_) {
+            size_t e = 0;
+            for (int i = 0; i < jb.count; i++) e += (size_t)jb.ts[i]->oc * jb.ts[i]->ic;
+            need = e > need ? e : need;
+        }
+        for (int b = 0; b < 2; b++) {
+            DCK(cudaMalloc((void **)&pf_w16_[b], need * sizeof(__half)));
+            DCK(cudaEventCreateWithFlags(&pf_expanded_[b], cudaEventDisableTiming));
+            DCK(cudaEventCreateWithFlags(&pf_consumed_[b], cudaEventDisableTiming));
+        }
+        pf_w16_elems_ = need;
+        DCK(cudaStreamCreateWithFlags(&pf_side_, cudaStreamNonBlocking));
     }
+    // the side stream starts after everything already queued on the main stream (a previous prompt's GEMMs read the scratch)
+    DCK(cudaEventRecord(pf_consumed_[0], ctx_->stream));
+    DCK(cudaStreamWaitEvent(pf_side_, pf_consumed_[0], 0));
+    DCK(pf_expand_job(0));
     cudaStream_t s = ctx_->stream;
     const int E = cfg_.embed_dim, F = cfg_.hidden_dim, H = cfg_.num_heads, KVH = cfg_.num_kv_heads, hd = cfg_.head_dim;
     const long long Q = (long long)(H + 2 * KVH) * hd;
@@ -955,8 +922,7 @@ cudaError_t LlamaDecoder::prefill(const int *tokens_host, int n, int pos0, float
     for (int l = 0; l < cfg_.num_layers; l++) {
         const tce_llama_layer &L = layers_[l];
         DCK(launch_rmsnorm_rows_f32(ctx_, pf_x_, L.input_norm, pf_xn_, n, E, cfg_.rms_eps));
-        const tce_w4_tensor *qkv[3] = {&L.q, &L.k, &L.v}, *gu[2] = {&L.gate, &L.up}, *o1[1] = {&L.o}, *d1[1] = {&L.down};
-        DCK(prefill_linear(qkv, 3, pf_xn_, pf_qkv_, Q, n, false));
+        DCK(prefill_linear(4 * l, pf_xn_, pf_qkv_, Q, n, EPI_STORE_HALF));
         AttnPrefillArgs a{};
         a.qkv = pf_qkv_;
         a.k_cache = (__half *)kv_cache(l, 0);
@@ -972,16 +938,10 @@ cudaError_t LlamaDecoder::prefill(const int *tokens_host, int n, int pos0, float
         a.head_dim = hd;
         a.max_ctx = cfg_.max_ctx;
         DCK(launch_attn_prefill(ctx_, a));
-        DCK(prefill_linear(o1, 1, pf_att_, pf_x_, E, n, true));  // residual add in the GEMM epilogue
+        DCK(prefill_linear(4 * l + 1, pf_att_, pf_x_, E, n, EPI_ADD_F32));  // residual add in the GEMM epilogue
         DCK(launch_rmsnorm_rows_f32(ctx_, pf_x_, L.post_norm, pf_xn_, n, E, cfg_.rms_eps));
-        const int gm = w4_gemm_mode();
-        if ((gm == W4G_PAIR || gm == W4G_PAIR_OVERLAP) && (F % 128) == 0) {
-            DCK(prefill_linear(gu, 2, pf_xn_, pf_act_, F, n, false, true));  // SiLU(gate) * up in the GEMM epilogue: gate|up never reach HBM
-        } else {
-            DCK(prefill_linear(gu, 2, pf_xn_, pf_gu_, 2LL * F, n, false));
-            DCK(launch_silu_mul_rows(ctx_, pf_gu_, pf_act_, n, F));
-        }
-        DCK(prefill_linear(d1, 1, pf_act_, pf_x_, E, n, true));
+        DCK(prefill_linear(4 * l + 2, pf_xn_, pf_act_, F, n, EPI_SILU_MUL_HALF));  // SiLU(gate) * up in the GEMM epilogue: gate|up never reach HBM
+        DCK(prefill_linear(4 * l + 3, pf_act_, pf_x_, E, n, EPI_ADD_F32));
     }
     // only the last position feeds the sampler: final RMSNorm + lm_head as the decode step's last GEMV, then arg-max
     DCK(cudaMemcpyAsync(d_resid_, pf_x_ + (size_t)(n - 1) * E, (size_t)E * sizeof(float), cudaMemcpyDeviceToDevice, s));

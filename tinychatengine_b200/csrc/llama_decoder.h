@@ -42,7 +42,7 @@ class LlamaDecoder {
    private:
     LlamaDecoder() = default;
     cudaError_t prefill_reserve(int n);
-    cudaError_t prefill_linear(const tce_w4_tensor *const *ts, int count, const __half *x, void *C, long long ldc, int n, bool add_f32, bool silu = false);
+    cudaError_t prefill_linear(int j, const __half *x, void *C, long long ldc, int n, EpiMode epi);
     cudaError_t enqueue_step(const int *tokpos, cudaStream_t s, bool pdl, bool gemv_only = false);  // raw kernel sequence
     cudaError_t build_graphs(std::string *err);
     void build_ops();
@@ -93,18 +93,17 @@ class LlamaDecoder {
     __half *pf_xn_ = nullptr;       // RMSNorm output [n][E]
     __half *pf_qkv_ = nullptr;      // [n][(H+2KVH)*hd]
     __half *pf_att_ = nullptr;      // [n][H*hd]
-    __half *pf_gu_ = nullptr;       // [n][2F] gate | up
-    __half *pf_act_ = nullptr;      // [n][F]
+    __half *pf_act_ = nullptr;      // [n][F] SiLU(gate) * up
     int *pf_tok_ = nullptr;
-    // W4G_PAIR_OVERLAP: the int4 -> fp16 expansion of the NEXT linear runs on a side stream into the other half of a double-buffered scratch
-    // while the tensor cores work on the current one (the expansion is HBM-bound, the GEMM tensor-bound)
+    // the int4 -> fp16 expansion of the NEXT linear runs on a side stream into the other half of a double-buffered scratch while the
+    // tensor cores work on the current one (the expansion is HBM-bound, the GEMM tensor-bound)
     __half *pf_w16_[2] = {nullptr, nullptr};
     size_t pf_w16_elems_ = 0;
     cudaStream_t pf_side_ = nullptr;
     cudaEvent_t pf_expanded_[2] = {nullptr, nullptr}, pf_consumed_[2] = {nullptr, nullptr};
+    // one job per linear of the prompt pass, in launch order: job 4 * layer + {0: q|k|v, 1: o, 2: gate|up, 3: down}
     struct PfJob { const tce_w4_tensor *ts[3]; int count; };
     std::vector<PfJob> pf_jobs_;
-    int pf_next_job_ = 0;
     cudaError_t pf_expand_job(int j);
     // pinned host staging for the end-to-end entry point
     int *h_tokpos_ = nullptr;
