@@ -65,9 +65,10 @@ TCE_DEVINL uint2 ld_ll1(const uint2 *p, bool sys) {
         asm volatile("ld.relaxed.gpu.global.v2.b32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p) : "memory");
     return r;
 }
-// A failed poll waits this long before it asks L2 again: thousands of threads spinning without a pause fill the L2 request queues and
-// stretch every round trip (their own and the producers' stores).
-constexpr unsigned kPollBackoffNs = 100;
+// Polls of this GPU's L2 spin without a pause: on H100 (700 W) a 100 ns back-off per failed poll cost 5 % of the Llama-3-8B step (no
+// pause: 471 tok/s, 100 ns: 460, 250 ns: 457).  Polls of a peer's memory over NVLink (tensor parallel) keep the back-off: that case has
+// not been measured without it.
+constexpr unsigned kPeerPollBackoffNs = 100;
 constexpr long long kSpinLimit = 20000000000LL;  // ~10 s: a peer rank may legitimately start its kernel later
 // spin until both words of the pair carry `tag`
 TCE_DEVINL uint4 wait_ll2(const uint2 *p, uint32_t tag, bool sys) {
@@ -75,7 +76,7 @@ TCE_DEVINL uint4 wait_ll2(const uint2 *p, uint32_t tag, bool sys) {
     if (r.y == tag && r.w == tag) return r;
     const long long t0 = clock64();
     while (true) {
-        __nanosleep(kPollBackoffNs);
+        if (sys) __nanosleep(kPeerPollBackoffNs);
         r = ld_ll2(p, sys);
         if (r.y == tag && r.w == tag) return r;
         if (clock64() - t0 > kSpinLimit) __trap();
@@ -86,7 +87,7 @@ TCE_DEVINL uint32_t wait_ll1(const uint2 *p, uint32_t tag, bool sys) {
     if (r.y == tag) return r.x;
     const long long t0 = clock64();
     while (true) {
-        __nanosleep(kPollBackoffNs);
+        if (sys) __nanosleep(kPeerPollBackoffNs);
         r = ld_ll1(p, sys);
         if (r.y == tag) return r.x;
         if (clock64() - t0 > kSpinLimit) __trap();
@@ -105,7 +106,7 @@ TCE_DEVINL void wait_ll2xN(const uint2 *p, uint32_t tag, bool sys, uint4 (&r)[N]
         if (ok) return;
         if (t0 == 0) t0 = clock64();
         if (clock64() - t0 > kSpinLimit) __trap();
-        __nanosleep(kPollBackoffNs);
+        if (sys) __nanosleep(kPeerPollBackoffNs);
     }
 }
 
@@ -437,7 +438,6 @@ TCE_DEVINL void stage_half(const Args &a, const GemvOp &op, const PSmem &sm, Pai
                 if (ok) break;
                 if (t0 == 0) t0 = clock64();
                 if (clock64() - t0 > kSpinLimit) __trap();
-                __nanosleep(kPollBackoffNs);
 #pragma unroll
                 for (int k = 0; k < PRE; k++) {
                     if (ui[k] >= 0 && !(w[k][0].y == tag && w[k][0].w == tag && w[k][1].y == tag && w[k][1].w == tag)) {
@@ -488,7 +488,7 @@ TCE_DEVINL void tp_accumulate(float (&x)[8], const uint2 *slot0, int tp_size, in
             if (ok) break;
             if (t0 == 0) t0 = clock64();
             if (clock64() - t0 > kSpinLimit) __trap();
-            __nanosleep(kPollBackoffNs);
+            __nanosleep(kPeerPollBackoffNs);
         }
         x[0] += __uint_as_float(wa[0].x); x[1] += __uint_as_float(wa[0].z); x[2] += __uint_as_float(wa[1].x); x[3] += __uint_as_float(wa[1].z);
         x[4] += __uint_as_float(wa[2].x); x[5] += __uint_as_float(wa[2].z); x[6] += __uint_as_float(wa[3].x); x[7] += __uint_as_float(wa[3].z);
@@ -776,15 +776,26 @@ TCE_DEVINL void attention_phase(const Args &a, const LayerDesc &L, const PSmem &
         __half *sQ = reinterpret_cast<__half *>(sm.xs);                        // [8][136] q * alpha after RoPE, rows >= nrep zero
         float *sO = reinterpret_cast<float *>(sm.xs + 8 * 136 * 2);            // [kCW][nrep][128] per-warp unnormalised outputs
         float *sML = sO + (size_t)kCW * nrep * 128;                            // [kCW][nrep][2] per-warp (max, sum)
+        uint32_t *sKV = reinterpret_cast<uint32_t *>(sML + (size_t)kCW * nrep * 2);  // [2][64] the token's RoPE(k) and v as half2 words
         const float *cosr = sm.rope, *sinr = sm.rope + 128;  // the position's table rows, staged once per kernel
-        // ---- RoPE on the nrep query heads of this KV head (fp32), one {half2} word per thread and pass ----
-        for (int i = ctid; i < 8 * 64; i += kConsumerThreads) {
-            const int r = i >> 6, j = i & 63;
+        // the split whose chunks hold the token appends its key and value.  They are fetched here, in the same L2 round trip as the
+        // queries: fetched inside the chunk loop, they put two dependent round trips on this split, the last one the merge waits for.
+        const bool owns_new = sp.ch1 * kKvChunk > pos;
+        // ---- RoPE on the nrep query heads of this KV head (fp32), one {half2} word per thread and pass; rows 6 and 7 (>= nrep) fetch v and k ----
+        static_assert(8 * 64 == kConsumerThreads, "one pass");
+        {
+            const int r = ctid >> 6, j = ctid & 63;
             float2 v = make_float2(0.f, 0.f);
             if (r < nrep) {
                 v = rope_pair(a.qkv_ll + (size_t)(sp.kvh * nrep + r) * 64, j, tag_qkv, cosr, sinr);
                 v.x *= a.alpha;
                 v.y *= a.alpha;
+            } else if (owns_new && r == 7) {
+                const float2 kr = rope_pair(a.qkv_ll + (size_t)a.H * 64 + (size_t)sp.kvh * 64, j, tag_qkv, cosr, sinr);
+                const __half2 kh = __floats2half2_rn(kr.x, kr.y);
+                sKV[j] = *reinterpret_cast<const uint32_t *>(&kh);
+            } else if (owns_new && r == 6) {
+                sKV[64 + j] = wait_ll1(a.qkv_ll + (size_t)(a.H + a.KVH) * 64 + (size_t)sp.kvh * 64 + j, tag_qkv, false);
             }
             *reinterpret_cast<__half2 *>(sQ + r * 136 + 2 * j) = __floats2half2_rn(v.x, v.y);
         }
@@ -809,18 +820,15 @@ TCE_DEVINL void attention_phase(const Args &a, const LayerDesc &L, const PSmem &
             if (mine) {
                 uint8_t *kst = sm.ring + (size_t)rs.stage * kStageBytes, *vst = kst + kHalfBytes;
                 if (has_new) {
-                    // the token's own key / value: RoPE(k), round to fp16, append to the cache and patch the (stale) rows of the stage
-                    const uint2 *kw = a.qkv_ll + (size_t)a.H * 64 + (size_t)sp.kvh * 64, *vw = a.qkv_ll + (size_t)(a.H + a.KVH) * 64 + (size_t)sp.kvh * 64;
+                    // the token's own key / value (RoPE'd and rounded to fp16 above): append to the cache and patch the (stale) rows of the stage
                     const int r = pos - c * kKvChunk;
 #pragma unroll
                     for (int i = 0; i < 2; i++) {
                         const int j = lane * 2 + i;  // word j = dims 2j, 2j+1
-                        const float2 kr = rope_pair(kw, j, tag_qkv, cosr, sinr);
-                        const __half2 kh = __floats2half2_rn(kr.x, kr.y);
-                        const uint32_t vv = wait_ll1(vw + j, tag_qkv, false);
-                        *reinterpret_cast<__half2 *>(kst + kv_off(r, j >> 2) + (j & 3) * 4) = kh;
+                        const uint32_t kh = sKV[j], vv = sKV[64 + j];
+                        *reinterpret_cast<uint32_t *>(kst + kv_off(r, j >> 2) + (j & 3) * 4) = kh;
                         *reinterpret_cast<uint32_t *>(vst + kv_off(r, j >> 2) + (j & 3) * 4) = vv;
-                        *reinterpret_cast<__half2 *>(L.k_cache + ((size_t)sp.kvh * a.max_ctx + pos) * 128 + 2 * j) = kh;
+                        *reinterpret_cast<uint32_t *>(L.k_cache + ((size_t)sp.kvh * a.max_ctx + pos) * 128 + 2 * j) = kh;
                         *reinterpret_cast<uint32_t *>(L.v_cache + ((size_t)sp.kvh * a.max_ctx + pos) * 128 + 2 * j) = vv;
                     }
                     // V rows of the block beyond the token were never written for this sequence: finite zeros (0 * garbage must not be NaN)
@@ -962,7 +970,6 @@ TCE_DEVINL void attention_phase(const Args &a, const LayerDesc &L, const PSmem &
                 if (ok) break;
                 if (t0 == 0) t0 = clock64();
                 if (clock64() - t0 > kSpinLimit) __trap();
-                __nanosleep(kPollBackoffNs);
             }
             __syncwarp();
         }
@@ -1186,7 +1193,7 @@ __global__ void repack_meta_kernel(W4Seg s0, W4Seg s1, W4Seg s2, int nseg, int p
 
 }  // namespace
 
-int attn_scratch_bytes(int nrep) { return 8 * 136 * 2 + kCW * nrep * 128 * 4 + kCW * nrep * 2 * 4; }
+int attn_scratch_bytes(int nrep) { return 8 * 136 * 2 + kCW * nrep * 128 * 4 + kCW * nrep * 2 * 4 + 2 * 64 * 4; }
 
 int attn_nsplit_max(int ncta, int KVH, int max_ctx) {
     int NS = ncta / KVH;

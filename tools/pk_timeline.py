@@ -51,6 +51,9 @@ def main():
     bytes_of = {0: (H + 2 * KVH) * hd * E * 0.5 * 1.0390625, 1: 2 * KVH * hd * 2 * (args.ctx + 1), 2: E * H * hd * 0.5 * 1.0390625, 3: 2 * F * E * 0.5 * 1.0390625,
                 4: E * F * 0.5 * 1.0390625}
     names = {0: "qkv", 1: "attn", 2: "o_proj", 3: "gate_up", 4: "down"}
+    # the attention phase publishes its results from the consumer warps (no epilogue stamp): its "results written" is "phase left"
+    for p in range(1, nphase - 1, 5):
+        T[:, p, 3] = T[:, p, 2]
     total = np.nanmax(T[:, -1, 3]) if not np.all(np.isnan(T[:, -1, 3])) else np.nanmax(T)
     print(f"kernel span (first barrier-pass stamp -> last arrival): {total:.1f} us over {nphase} phases, ctx {args.ctx}")
     # attention sub-steps (medians over the CTAs that own chunks and over layers): time since the CTA entered the phase
@@ -63,6 +66,20 @@ def main():
                     att[k].append(np.nanmedian(d))
     print("attention, since phase entry (median): q roped+bar %.2f  first stage landed %.2f  chunks done %.2f  partial written %.2f  phase left %.2f us" %
           tuple(float(np.median(att[k])) if att[k] else float("nan") for k in (4, 7, 5, 6, 2)))
+    # the same sub-steps against the hand-off they wait for: the last q|k|v result of the layer (median over layers of the median / the
+    # latest CTA).  The split merge ends with "phase left"; o_proj staging waits for the latest one.
+    chain = {}
+    for p in range(1, nphase - 1, 5):
+        qkv_done = np.nanmax(T[:, p - 1, 3])
+        for k, nm in ((4, "q_roped"), (7, "first_stage"), (5, "chunks_done"), (6, "partial_written"), (2, "merged")):
+            d = T[:, p, k] - qkv_done
+            if not np.all(np.isnan(d)):
+                chain.setdefault(nm + "_med_us", []).append(np.nanmedian(d))
+                chain.setdefault(nm + "_max_us", []).append(np.nanmax(d))
+    chain = {k: float(np.median(v)) for k, v in chain.items()}
+    print("attention, since the last q|k|v result (median / latest CTA): " +
+          "  ".join(f"{nm} {chain[nm + '_med_us']:.2f}/{chain[nm + '_max_us']:.2f}" for nm in ("q_roped", "first_stage", "chunks_done", "partial_written", "merged")
+                    if nm + "_med_us" in chain) + " us")
     acc = {}
     for p in range(1, nphase - 1):
         k = p % 5
@@ -80,7 +97,7 @@ def main():
     for k, lst in sorted(acc.items()):
         m = {key: float(np.median([d[key] for d in lst])) for key in lst[0]}
         m["GBps"] = bytes_of[k] / m["phase_us"] / 1e3
-        m["hbm_floor_us"] = bytes_of[k] / 6.5696e6
+        m["hbm_floor_us"] = bytes_of[k] / 3.35e6  # H100 SXM data-sheet HBM3 rate, 3.35 TB/s
         summ[names[k]] = m
         print(f"{names[k]:8s} phase {m['phase_us']:6.2f} us (HBM floor {m['hbm_floor_us']:5.2f})  barrier {m['barrier_us']:5.2f}  stage {m['stage_us']:5.2f}  "
               f"consume {m['consume_us']:6.2f}  tail {m['tail_us']:5.2f}  skew {m['skew_us']:5.2f}  hop {m['hop_us']:5.2f}  etail {m['etail_us']:5.2f}  -> {m['GBps']:7.0f} GB/s")
@@ -89,6 +106,7 @@ def main():
     print(f"lm_head  phase {np.nanmax(T[:, lm, 3]) - prev_done:6.2f} us")
     summ["lm_head_us"] = float(np.nanmax(T[:, lm, 3]) - prev_done)
     summ["kernel_us"] = float(total)
+    summ["attention_chain"] = chain
     if args.out:
         Path(args.out).write_text(json.dumps(summ, indent=1))
     model.close()
