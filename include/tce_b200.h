@@ -205,6 +205,29 @@ TCE_API int tce_sample(tce_ctx *ctx, float *logits_dev, int n_vocab, const int *
  * ids (4 bytes each) cross PCIe.  Single GPU (tp_size == 1).                                                                       */
 TCE_API int tce_llama_generate(tce_llama *m, int first_token, int pos0, int n_predict, const tce_sampling *cfg, const int *history_host,
                                int n_history, int eos_id, int *out_tokens_host, int *n_out);
+/* ---- batched decode: up to TCE_LLAMA_MAX_BATCH sequences per step, each in its own KV-cache slot -------------------------------------
+ * One step streams the weights once for the whole batch (a batch-1 step's bytes are almost all weights).  A slot is one sequence's cache,
+ * half[L][2][KVH][max_ctx][hd]; slot 0 is the cache of the single-sequence entry points above.  Single GPU: with tp_size > 1 every entry
+ * point of this block returns TCE_ERR_UNSUPPORTED.  The batched step is one kernel per op (4 W4A16 GEMVs per layer + lm_head, each reading
+ * its weights once for all rows), not the persistent kernel.                                                                          */
+#define TCE_LLAMA_MAX_BATCH 8
+/* grow the number of slots to n_slots (never shrinks; new slots are zeroed).  Slot 0 always exists.  Invalidates captured batch graphs. */
+TCE_API int tce_llama_reserve_slots(tce_llama *m, int n_slots);
+/* half[KVH][max_ctx][hd] of (slot, layer, which: 0 K, 1 V), or NULL */
+TCE_API void *tce_llama_kv_cache_slot(tce_llama *m, int slot, int layer, int which);
+/* tce_llama_prefill into the cache of `slot`; slot 0 is exactly tce_llama_prefill */
+TCE_API int tce_llama_prefill_slot(tce_llama *m, int slot, const int *tokens_host, int n, int pos0, float *logits_host, int *next_token);
+/* inputs resident: req_dev = device int[batch][3] {token, position, slot}, 1 <= batch <= TCE_LLAMA_MAX_BATCH.  The logits land in
+ * tce_llama_batch_logits(m).  Entries are range-checked on the device: an entry with a token, position or slot out of range writes no KV row
+ * in any slot (its logits row is meaningless) and the other entries proceed.  Two entries naming the same slot are the caller's error:
+ * both append to that slot in an unspecified order.                                                                                       */
+TCE_API int tce_llama_decode_batch(tce_llama *m, int batch, const int *req_dev);
+/* end to end: batch host entries; logits_host float[batch][vocab] and next_tokens int[batch] (greedy) may be NULL.  TCE_ERR_INVALID, before
+ * anything is enqueued, for a batch outside [1, TCE_LLAMA_MAX_BATCH], a slot >= the reserved count or named twice, a position outside
+ * [0, max_ctx) or a token outside [0, vocab).  Returns after the copies have completed.                                                  */
+TCE_API int tce_llama_decode_batch_host(tce_llama *m, int batch, const int *tokens, const int *positions, const int *slots, float *logits_host,
+                                        int *next_tokens);
+TCE_API const float *tce_llama_batch_logits(tce_llama *m);    /* device float[TCE_LLAMA_MAX_BATCH][vocab] */
 TCE_API const float *tce_llama_logits(tce_llama *m);          /* device float[vocab] */
 TCE_API void *tce_llama_kv_cache(tce_llama *m, int layer, int which); /* which: 0 K, 1 V; half[KVH][max_ctx][hd] */
 TCE_API int tce_llama_kernels_per_step(tce_llama *m);

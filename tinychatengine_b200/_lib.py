@@ -73,6 +73,12 @@ SIGNATURES = {
     "tce_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(Sampling), C.c_ulonglong, C.POINTER(C.c_int), C.c_void_p, C.c_void_p,
                              C.POINTER(C.c_int)]),
     "tce_llama_generate": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int)]),
+    "tce_llama_reserve_slots": (C.c_int, [C.c_void_p, C.c_int]),
+    "tce_llama_kv_cache_slot": (C.c_void_p, [C.c_void_p, C.c_int, C.c_int, C.c_int]),
+    "tce_llama_prefill_slot": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "tce_llama_decode_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
+    "tce_llama_decode_batch_host": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tce_llama_batch_logits": (C.c_void_p, [C.c_void_p]),
     "tce_llama_logits": (C.c_void_p, [C.c_void_p]),
     "tce_llama_kv_cache": (C.c_void_p, [C.c_void_p, C.c_int, C.c_int]),
     "tce_llama_kernels_per_step": (C.c_int, [C.c_void_p]),

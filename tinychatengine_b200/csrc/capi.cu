@@ -86,7 +86,8 @@ int tce_ctx_create(int device, tce_ctx **out) {
     c.gemv_max_ctas = c.num_sms * 4;
     c.gemv_max_tiles = 32768;
     c.attn_ws_bytes = (size_t)128 * 1024 * 130 * sizeof(float);  // heads * splits * (128 + 2): 128 heads x 1024 splits
-    cudaError_t ie = cudaMalloc(&c.gemv_partials, (size_t)c.gemv_max_ctas * 2 * 16 * 8 * sizeof(float));
+    c.gemv_partial_records = c.gemv_max_ctas * 2 > 16384 ? c.gemv_max_ctas * 2 : 16384;  // 8 MB: e.g. 256 row tiles x 32 K-slices
+    cudaError_t ie = cudaMalloc(&c.gemv_partials, (size_t)c.gemv_partial_records * 16 * 8 * sizeof(float));
     if (ie == cudaSuccess) ie = cudaMalloc(&c.gemv_counters, (size_t)c.gemv_max_tiles * sizeof(unsigned));
     if (ie == cudaSuccess) ie = cudaMemset(c.gemv_counters, 0, (size_t)c.gemv_max_tiles * sizeof(unsigned));
     if (ie == cudaSuccess) ie = cudaMalloc(&c.attn_ws, c.attn_ws_bytes);
@@ -512,6 +513,44 @@ int tce_sample(tce_ctx *ctx, float *logits_dev, int n_vocab, const int *window_h
     if (want_cand) *cand_count_host = out[2];
     return TCE_OK;
 }
+// ---- batched decode
+static int batch_fail(cudaError_t e, const char *what, const std::string &err) {
+    if (e == cudaErrorNotSupported) return fail(TCE_ERR_UNSUPPORTED, "%s: %s", what, err.empty() ? "not supported for this model" : err.c_str());
+    if (e == cudaErrorInvalidValue) return fail(TCE_ERR_INVALID, "%s: bad argument%s%s", what, err.empty() ? "" : ": ", err.c_str());
+    return fail(TCE_ERR_CUDA, "%s: %s (%s)", what, cudaGetErrorString(e), err.c_str());
+}
+int tce_llama_reserve_slots(tce_llama *m, int n_slots) {
+    if (!m) return fail(TCE_ERR_INVALID, "tce_llama_reserve_slots: null argument");
+    std::string err;
+    cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->reserve_slots(n_slots, &err);
+    if (e == cudaErrorInvalidValue) return fail(TCE_ERR_INVALID, "tce_llama_reserve_slots: n_slots = %d outside [1, 1024]", n_slots);
+    return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_reserve_slots", err);
+}
+void *tce_llama_kv_cache_slot(tce_llama *m, int slot, int layer, int which) {
+    return m ? reinterpret_cast<LlamaDecoder *>(m)->kv_cache_slot(slot, layer, which) : nullptr;
+}
+int tce_llama_prefill_slot(tce_llama *m, int slot, const int *tokens_host, int n, int pos0, float *logits_host, int *next_token) {
+    if (!m || !tokens_host) return fail(TCE_ERR_INVALID, "tce_llama_prefill_slot: null argument");
+    LlamaDecoder *d = reinterpret_cast<LlamaDecoder *>(m);
+    if (d->tensor_parallel()) return fail(TCE_ERR_UNSUPPORTED, "tce_llama_prefill_slot: single GPU only (tp_size > 1)");
+    std::string err;
+    cudaError_t e = d->prefill(tokens_host, n, pos0, logits_host, next_token, &err, slot);
+    if (e == cudaErrorInvalidValue) return fail(TCE_ERR_INVALID, "tce_llama_prefill_slot: bad slot %d / tokens / n=%d pos0=%d", slot, n, pos0);
+    return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_prefill_slot", err);
+}
+int tce_llama_decode_batch(tce_llama *m, int batch, const int *req_dev) {
+    if (!m || !req_dev) return fail(TCE_ERR_INVALID, "tce_llama_decode_batch: null argument");
+    std::string err;
+    cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->decode_batch_device(batch, req_dev, &err);
+    return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_decode_batch", err);
+}
+int tce_llama_decode_batch_host(tce_llama *m, int batch, const int *tokens, const int *positions, const int *slots, float *logits_host, int *next_tokens) {
+    if (!m || !tokens || !positions || !slots) return fail(TCE_ERR_INVALID, "tce_llama_decode_batch_host: null argument");
+    std::string err;
+    cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->decode_batch_host(batch, tokens, positions, slots, logits_host, next_tokens, &err);
+    return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_decode_batch_host", err);
+}
+const float *tce_llama_batch_logits(tce_llama *m) { return m ? reinterpret_cast<LlamaDecoder *>(m)->batch_logits() : nullptr; }
 const float *tce_llama_logits(tce_llama *m) { return m ? reinterpret_cast<LlamaDecoder *>(m)->logits() : nullptr; }
 void *tce_llama_kv_cache(tce_llama *m, int layer, int which) { return m ? reinterpret_cast<LlamaDecoder *>(m)->kv_cache(layer, which) : nullptr; }
 int tce_llama_enqueue_gemvs(tce_llama *m) {

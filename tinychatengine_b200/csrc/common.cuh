@@ -49,6 +49,11 @@ TCE_DEVINL uint64_t l2_policy_evict_first() {
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
     return pol;
 }
+TCE_DEVINL uint64_t l2_policy_evict_normal() {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
 TCE_DEVINL uint64_t l2_policy_evict_last() {
     uint64_t pol;
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));

@@ -31,6 +31,64 @@ __global__ void embedding_kernel(const __half *__restrict__ table, const int *__
     }
 }
 
+// grid (blocks per row, batch): entry b of req = {token, position, slot}
+__global__ void embedding_batch_kernel(const __half *__restrict__ table, const int *__restrict__ req, float *__restrict__ resid, int E, int rows,
+                                       int max_ctx, int n_slots, int *__restrict__ safe) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const int b = blockIdx.y;
+    const int tok = req[3 * b], pos = req[3 * b + 1], slot = req[3 * b + 2];
+    const bool ok = tok >= 0 && tok < rows && pos >= 0 && pos < max_ctx && slot >= 0 && slot < n_slots;
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        safe[4 * b] = ok ? tok : 0;
+        safe[4 * b + 1] = ok ? pos : 0;
+        safe[4 * b + 2] = ok ? slot : 0;
+        safe[4 * b + 3] = ok ? 1 : 0;
+    }
+    const __half2 *row = reinterpret_cast<const __half2 *>(table + (size_t)(ok ? tok : 0) * E);
+    float2 *dst = reinterpret_cast<float2 *>(resid + (size_t)b * E);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < E / 2; i += gridDim.x * blockDim.x) dst[i] = __half22float2(row[i]);
+}
+
+// one CTA per row; ties resolve to the lowest index
+__global__ void __launch_bounds__(1024) argmax_rows_kernel(const float *__restrict__ logits, int n, int *__restrict__ out) {
+    __shared__ float sval[32];
+    __shared__ int sidx[32];
+    pdl_launch_dependents();
+    pdl_wait();
+    const float *x = logits + (size_t)blockIdx.x * n;
+    float best = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const float v = x[i];
+        if (v > best) {  // indices rise within a thread: the first maximum stays
+            best = v;
+            bi = i;
+        }
+    }
+    auto combine = [](float &bv, int &bidx, float ov, int oidx) {
+        if (ov > bv || (ov == bv && oidx < bidx)) {
+            bv = ov;
+            bidx = oidx;
+        }
+    };
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) combine(best, bi, __shfl_xor_sync(0xffffffffu, best, o), __shfl_xor_sync(0xffffffffu, bi, o));
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (lane == 0) {
+        sval[warp] = best;
+        sidx[warp] = bi;
+    }
+    __syncthreads();
+    if (warp == 0) {
+        best = (lane < (int)(blockDim.x >> 5)) ? sval[lane] : -INFINITY;
+        bi = (lane < (int)(blockDim.x >> 5)) ? sidx[lane] : 0x7fffffff;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) combine(best, bi, __shfl_xor_sync(0xffffffffu, best, o), __shfl_xor_sync(0xffffffffu, bi, o));
+        if (lane == 0) out[blockIdx.x] = bi == 0x7fffffff ? 0 : bi;
+    }
+}
+
 // two-phase argmax with a last-block finish; ties resolve to the lowest index
 struct ArgmaxWs {
     float val[256];
@@ -258,6 +316,21 @@ cudaError_t launch_argmax(Ctx *ctx, const float *logits, int n, int *out, bool p
     if (blocks < 1) blocks = 1;
     launch_cfg(cfg, attr, dim3(blocks), dim3(256), ctx->stream, pdl);
     return cudaLaunchKernelEx(&cfg, argmax_kernel, logits, n, out);
+}
+
+cudaError_t launch_embedding_batch(Ctx *ctx, const __half *table, const int *req, float *resid, int E, int batch, int rows, int max_ctx, int n_slots,
+                                   int *safe, bool pdl) {
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute attr[1];
+    launch_cfg(cfg, attr, dim3(4, batch), dim3(256), ctx->stream, pdl);
+    return cudaLaunchKernelEx(&cfg, embedding_batch_kernel, table, req, resid, E, rows, max_ctx, n_slots, safe);
+}
+
+cudaError_t launch_argmax_rows(Ctx *ctx, const float *logits, int rows, int n, int *out, bool pdl) {
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute attr[1];
+    launch_cfg(cfg, attr, dim3(rows), dim3(1024), ctx->stream, pdl);
+    return cudaLaunchKernelEx(&cfg, argmax_rows_kernel, logits, n, out);
 }
 
 cudaError_t launch_embedding_rows(Ctx *ctx, const __half *table, const int *tokens, float *resid, int n, int E) {

@@ -15,8 +15,10 @@ struct Ctx {
     cudaStream_t stream = nullptr;
     int num_sms = 0;
     int smem_optin = 0;
-    // stream-K fix-up workspace of the W4A16 GEMV: 2 partial records per CTA + one arrival counter per row tile
+    // stream-K fix-up workspace of the W4A16 GEMV: partial records of 16 x 8 floats (2 per CTA, or 1 per (K-slice, row tile) in the
+    // multi-column kernel, grown on demand by gemv_partials_reserve) + one arrival counter per row tile
     float *gemv_partials = nullptr;
+    int gemv_partial_records = 0;
     unsigned *gemv_counters = nullptr;
     int gemv_max_ctas = 0;
     int gemv_max_tiles = 0;
@@ -101,10 +103,13 @@ struct W4GemvParams {
     int tp_sig_k = 0;
 };
 
+// M = 2..8 at long rows needs one stream-K fix-up record per (K-slice, row tile); the launch grows ctx->gemv_partials when it has too few
+// (outside of stream capture only; the context's option generation moves, so captured graphs are rebuilt)
 cudaError_t launch_w4a16_gemv(Ctx *ctx, const W4GemvParams &p);
+long long w4a16_gemv_fixup_records(const Ctx *ctx, const W4GemvParams &p);  // records a launch of p needs beyond the per-CTA ones
+cudaError_t gemv_partials_reserve(Ctx *ctx, long long records);
 cudaError_t launch_w4a16_gemv_simple(Ctx *ctx, const W4GemvParams &p);
 cudaError_t launch_w4a16_gemv_g64(Ctx *ctx, const __half *x, const uint32_t *w, const uint32_t *zeros, const __half *scales, __half *y, int M, int IC, int OC);
-size_t w4a16_gemv_smem_bytes(int ncols, int consumer_warps, int IC);
 cudaError_t encode_w4_tmap(CUtensorMap *out, const void *w, int rows, int IC, int sg, int box_rows);
 cudaError_t encode_w4_tmap_units(CUtensorMap *out, const void *w, int rows, int IC, int sg, int box_rows);  // [group][row][64 B] boxes
 

@@ -21,6 +21,22 @@ struct AttnDecodeArgs {
 };
 cudaError_t launch_attn_decode(Ctx *ctx, AttnDecodeArgs a, bool pdl);
 
+// batched decode: sequence b of the batch is grid.z = b, with its own q|k|v / output rows, KV-cache slot and position
+struct AttnBatchArgs {
+    AttnDecodeArgs base;     // qkv / out of sequence 0, RoPE tables, shapes, and the split workspace base.ws / base.counters (k_cache, v_cache and
+                             // pos unused)
+    size_t ws_floats;        // capacity of base.ws: batch * num_heads * nsplit * (head_dim + 2) floats are used
+    size_t n_counters;       // capacity of base.counters (zero-initialised): batch * num_kv_heads are used
+    const int *req;          // device int[batch][4] {token, position, slot, valid} (launch_embedding_batch); valid = 0: the CTA writes nothing
+    __half *const *slots;    // device table of slot bases, each [L][2][KVH][max_ctx][head_dim]
+    long long k_off, v_off;  // elements from a slot's base to this layer's K / V slab
+    int qkv_stride, out_stride;  // elements between the rows of consecutive sequences
+};
+// returns cudaErrorNotSupported for a head_dim or a query-heads-per-KV-head ratio the kernel does not cover
+cudaError_t launch_attn_decode_batch(Ctx *ctx, AttnBatchArgs b, int batch, bool pdl);
+// floats of split workspace the batched kernel needs per sequence
+size_t attn_batch_ws_floats(int num_heads, int max_ctx, int chunk);
+
 // prompt processing (sqlen = n > 1): RoPE + KV append for rows pos0..pos0+n-1, causal attention over the cache
 struct AttnPrefillArgs {
     __half *qkv;         // [n][(H + 2*KVH) * head_dim]; q is rotated in place
@@ -39,6 +55,13 @@ cudaError_t launch_rmsnorm_rows_f32(Ctx *ctx, const float *x, const float *gamma
 cudaError_t launch_embedding(Ctx *ctx, const __half *table, const int *token, float *resid, int E, bool pdl, int rows = 0, int max_ctx = 0, int *safe = nullptr);
 // argmax over fp32 logits -> int (first index of the maximum, like arg_max.cc)
 cudaError_t launch_argmax(Ctx *ctx, const float *logits, int n, int *out, bool pdl);
+// batched decode step prologue: resid[b][E] = table[token_b] for req = device int[batch][3] {token, position, slot}.  Every entry is
+// range-checked (token < rows, position < max_ctx, slot < n_slots) and published as safe[b] = {token, position, slot, valid}; a refused
+// entry (valid = 0) embeds row 0 and the attention kernels skip it, so it writes no KV row in any slot
+cudaError_t launch_embedding_batch(Ctx *ctx, const __half *table, const int *req, float *resid, int E, int batch, int rows, int max_ctx, int n_slots,
+                                   int *safe, bool pdl);
+// out[b] = argmax over logits[b][0..n) for b < rows (first index of the maximum)
+cudaError_t launch_argmax_rows(Ctx *ctx, const float *logits, int rows, int n, int *out, bool pdl);
 
 // device sampler (sampling.cu): llm/src/Generate.cc:14-136, 304-327 in the order of LLaMAGenerate.cu:112-166
 struct SampleArgs {

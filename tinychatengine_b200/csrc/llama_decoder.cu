@@ -173,12 +173,28 @@ LlamaDecoder::~LlamaDecoder() {
     if (h_tokpos_) cudaFreeHost(h_tokpos_);
     if (h_logits_) cudaFreeHost(h_logits_);
     if (h_next_) cudaFreeHost(h_next_);
+    drop_batch_graphs();
+    for (__half *p : slot_kv_) cudaFree(p);
+    cudaFree(d_slot_table_);
+    cudaFree(d_bresid_);
+    cudaFree(d_bqkv_);
+    cudaFree(d_battn_);
+    cudaFree(d_bact_);
+    cudaFree(d_blogits_);
+    cudaFree(d_breq_);
+    cudaFree(d_bsafe_);
+    cudaFree(d_bnext_);
+    cudaFree(d_battn_ws_);
+    cudaFree(d_battn_counters_);
+    if (h_breq_) cudaFreeHost(h_breq_);
+    if (h_bnext_) cudaFreeHost(h_bnext_);
+    if (h_blogits_) cudaFreeHost(h_blogits_);
 }
 
-void *LlamaDecoder::kv_cache(int layer, int which) const {
-    if (layer < 0 || layer >= cfg_.num_layers || which < 0 || which > 1) return nullptr;
+void *LlamaDecoder::kv_cache_slot(int slot, int layer, int which) const {
+    if (slot < 0 || slot >= n_slots() || layer < 0 || layer >= cfg_.num_layers || which < 0 || which > 1) return nullptr;
     const size_t per = (size_t)cfg_.num_kv_heads * cfg_.max_ctx * cfg_.head_dim;
-    return d_kv_ + ((size_t)layer * 2 + which) * per;
+    return (slot == 0 ? d_kv_ : slot_kv_[slot - 1]) + ((size_t)layer * 2 + which) * per;
 }
 
 static W4Seg seg_of(const tce_w4_tensor &t) { return W4Seg{(const uint32_t *)t.w, (const uint32_t *)t.zeros, (const __half *)t.scales, t.oc}; }
@@ -879,12 +895,12 @@ cudaError_t LlamaDecoder::pf_expand_job(int j) {
     return cudaEventRecord(pf_expanded_[b], pf_side_);
 }
 
-cudaError_t LlamaDecoder::prefill(const int *tokens_host, int n, int pos0, float *logits_host, int *next_token, std::string *err) {
+cudaError_t LlamaDecoder::prefill(const int *tokens_host, int n, int pos0, float *logits_host, int *next_token, std::string *err, int slot) {
     if (tp_ > 1) {
         if (err) *err = "prefill is single-GPU in this build (tensor-parallel ranks process the prompt with decode steps)";
         return cudaErrorNotSupported;
     }
-    if (!tokens_host || n < 1 || pos0 < 0 || pos0 + n > cfg_.max_ctx) return cudaErrorInvalidValue;
+    if (!tokens_host || n < 1 || pos0 < 0 || pos0 + n > cfg_.max_ctx || slot < 0 || slot >= n_slots()) return cudaErrorInvalidValue;
     for (int i = 0; i < n; i++)
         if (tokens_host[i] < 0 || tokens_host[i] >= cfg_.vocab_size) return cudaErrorInvalidValue;
     DCK(prefill_reserve(n));
@@ -925,8 +941,8 @@ cudaError_t LlamaDecoder::prefill(const int *tokens_host, int n, int pos0, float
         DCK(prefill_linear(4 * l, pf_xn_, pf_qkv_, Q, n, EPI_STORE_HALF));
         AttnPrefillArgs a{};
         a.qkv = pf_qkv_;
-        a.k_cache = (__half *)kv_cache(l, 0);
-        a.v_cache = (__half *)kv_cache(l, 1);
+        a.k_cache = (__half *)kv_cache_slot(slot, l, 0);
+        a.v_cache = (__half *)kv_cache_slot(slot, l, 1);
         a.cos = d_cos_;
         a.sin = d_sin_;
         a.out = pf_att_;
@@ -956,6 +972,317 @@ cudaError_t LlamaDecoder::prefill(const int *tokens_host, int n, int pos0, float
     DCK(cudaStreamSynchronize(s));
     if (logits_host) memcpy(logits_host, h_logits_, (size_t)cfg_.vocab_size * sizeof(float));
     if (next_token) *next_token = *h_next_;
+    return cudaSuccess;
+}
+
+}  // namespace tce
+
+// ------------------------------------------------------------------------------------------------ batched decode
+// Up to TCE_LLAMA_MAX_BATCH sequences per step, each in its own KV-cache slot.  The step is the op list of the single-sequence graph path
+// (build_ops) with every activation buffer widened to [8][.]: the GEMVs run with M = batch rows (one pass over each weight matrix), the
+// attention kernel takes one grid layer per sequence, and a batched embedding kernel range-checks every request first.
+namespace tce {
+
+void LlamaDecoder::drop_batch_graphs() {
+    for (int b = 0; b <= TCE_LLAMA_MAX_BATCH; b++) {
+        for (int h = 0; h < 2; h++)
+            if (g_bhost_[h][b]) {
+                cudaGraphExecDestroy(g_bhost_[h][b]);
+                g_bhost_[h][b] = nullptr;
+            }
+        if (g_bdev_[b]) {
+            cudaGraphExecDestroy(g_bdev_[b]);
+            g_bdev_[b] = nullptr;
+        }
+    }
+}
+
+cudaError_t LlamaDecoder::batch_alloc(std::string *err) {
+    auto no = [&](const char *m) {
+        if (err) *err = m;
+        return cudaErrorNotSupported;
+    };
+    if (tp_ > 1) return no("the batched step is single-GPU (tp_size > 1)");
+    if (d_slot_table_) return cudaSuccess;
+    const int nrep = cfg_.num_heads / cfg_.num_kv_heads;
+    if (nrep != 1 && nrep != 2 && nrep != 4 && nrep != 8) return no("the batched attention kernel takes 1, 2, 4 or 8 query heads per KV head");
+    const int chunk = attn_chunk_ > 0 ? attn_chunk_ : 128;
+    const size_t B = TCE_LLAMA_MAX_BATCH, E = cfg_.embed_dim, F = cfg_.hidden_dim, V = cfg_.vocab_size,
+                 Q = (size_t)(cfg_.num_heads + 2 * cfg_.num_kv_heads) * cfg_.head_dim, A = (size_t)cfg_.num_heads * cfg_.head_dim;
+    const size_t ws_floats = B * attn_batch_ws_floats(cfg_.num_heads, cfg_.max_ctx, chunk), n_counters = B * cfg_.num_kv_heads;
+    // all or nothing: a failed allocation releases what this call took, so a later call starts from scratch without leaking
+    std::vector<void *> dev, host;
+    cudaError_t e = cudaSuccess;
+    auto D = [&](void **p, size_t bytes) {
+        *p = nullptr;
+        if (e == cudaSuccess) e = cudaMalloc(p, bytes);
+        if (e == cudaSuccess) dev.push_back(*p);
+    };
+    auto Hst = [&](void **p, size_t bytes) {
+        *p = nullptr;
+        if (e == cudaSuccess) e = cudaMallocHost(p, bytes);
+        if (e == cudaSuccess) host.push_back(*p);
+    };
+    float *resid, *logits, *ws;
+    __half *qkv, *attn, *act, **table;
+    int *req, *safe, *next, *hreq, *hnext;
+    unsigned *counters;
+    float *hlogits;
+    D((void **)&resid, B * E * sizeof(float));
+    D((void **)&qkv, B * Q * sizeof(__half));
+    D((void **)&attn, B * A * sizeof(__half));
+    D((void **)&act, B * F * sizeof(__half));
+    D((void **)&logits, B * V * sizeof(float));
+    D((void **)&req, B * 3 * sizeof(int));
+    D((void **)&safe, B * 4 * sizeof(int));
+    D((void **)&next, B * sizeof(int));
+    D((void **)&ws, ws_floats * sizeof(float));
+    D((void **)&counters, n_counters * sizeof(unsigned));
+    D((void **)&table, sizeof(__half *));
+    Hst((void **)&hreq, B * 3 * sizeof(int));
+    Hst((void **)&hnext, B * sizeof(int));
+    Hst((void **)&hlogits, B * V * sizeof(float));
+    if (e == cudaSuccess) e = cudaMemset(logits, 0, B * V * sizeof(float));
+    if (e == cudaSuccess) e = cudaMemset(counters, 0, n_counters * sizeof(unsigned));  // the split merge re-arms them after every use
+    if (e == cudaSuccess) e = cudaMemcpy(table, &d_kv_, sizeof(__half *), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        for (void *p : dev) cudaFree(p);
+        for (void *p : host) cudaFreeHost(p);
+        if (err) *err = std::string("batched-step buffers: ") + cudaGetErrorString(e);
+        return e;
+    }
+    d_bresid_ = resid;
+    d_bqkv_ = qkv;
+    d_battn_ = attn;
+    d_bact_ = act;
+    d_blogits_ = logits;
+    d_breq_ = req;
+    d_bsafe_ = safe;
+    d_bnext_ = next;
+    d_battn_ws_ = ws;
+    battn_ws_floats_ = ws_floats;
+    d_battn_counters_ = counters;
+    battn_counters_ = n_counters;
+    h_breq_ = hreq;
+    h_bnext_ = hnext;
+    h_blogits_ = hlogits;
+    d_slot_table_ = table;  // last: a non-null table means every buffer above exists
+    return cudaSuccess;
+}
+
+const float *LlamaDecoder::batch_logits() { return batch_alloc(nullptr) == cudaSuccess ? d_blogits_ : nullptr; }
+
+cudaError_t LlamaDecoder::reserve_slots(int n, std::string *err) {
+    if (tp_ > 1) return batch_alloc(err);  // not supported, with its message
+    if (n < 1 || n > 1024) return cudaErrorInvalidValue;
+    DCK(batch_alloc(err));
+    if (n <= n_slots()) return cudaSuccess;
+    // queued work may still read the old table: drain it before the table (and the graphs holding it) go away
+    DCK(cudaStreamSynchronize(ctx_->stream));
+    DCK(cudaStreamSynchronize(cap_stream_));
+    // all or nothing: the new slots and the table that lists them are built aside and only then published, so the slot count and the
+    // device table always agree (a failed call leaves both as they were)
+    const size_t kv_bytes = (size_t)cfg_.num_layers * 2 * cfg_.num_kv_heads * cfg_.max_ctx * cfg_.head_dim * sizeof(__half);
+    std::vector<__half *> added;
+    __half **table = nullptr;
+    cudaError_t e = cudaSuccess;
+    while (e == cudaSuccess && n_slots() + (int)added.size() < n) {
+        __half *p = nullptr;
+        e = cudaMalloc((void **)&p, kv_bytes);
+        if (e == cudaSuccess) {
+            added.push_back(p);
+            e = cudaMemset(p, 0, kv_bytes);
+        }
+    }
+    std::vector<__half *> h;
+    h.push_back(d_kv_);
+    h.insert(h.end(), slot_kv_.begin(), slot_kv_.end());
+    h.insert(h.end(), added.begin(), added.end());
+    if (e == cudaSuccess) e = cudaMalloc((void **)&table, h.size() * sizeof(__half *));
+    if (e == cudaSuccess) e = cudaMemcpy(table, h.data(), h.size() * sizeof(__half *), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        for (__half *p : added) cudaFree(p);
+        cudaFree(table);
+        if (err) *err = std::string("slot allocation: ") + cudaGetErrorString(e);
+        return e;
+    }
+    drop_batch_graphs();  // they hold the old table and slot count
+    cudaFree(d_slot_table_);
+    d_slot_table_ = table;
+    slot_kv_.insert(slot_kv_.end(), added.begin(), added.end());
+    return cudaSuccess;
+}
+
+cudaError_t LlamaDecoder::enqueue_batch(int batch, const int *req, cudaStream_t s, bool pdl) {
+    const int E = cfg_.embed_dim, F = cfg_.hidden_dim, V = cfg_.vocab_size, A = cfg_.num_heads * cfg_.head_dim,
+              Q = (cfg_.num_heads + 2 * cfg_.num_kv_heads) * cfg_.head_dim;
+    // the K-sliced GEMVs' fix-up records are grown on the context itself (the launches below see a copy of it); a no-op after the first step
+    long long records = 0;
+    for (const StepOp &op : ops_) {
+        if (op.type != OP_GEMV) continue;
+        W4GemvParams p = op.g;
+        p.M = batch;
+        const long long r = w4a16_gemv_fixup_records(ctx_, p);
+        records = r > records ? r : records;
+    }
+    DCK(gemv_partials_reserve(ctx_, records));
+    Ctx local = *ctx_;
+    local.stream = s;
+    Ctx *c = &local;
+    // single-sequence buffer -> its [8][.] batched counterpart and row pitch
+    auto widen = [&](const void *p, int *ld) -> void * {
+        if (p == d_resid_) return *ld = E, d_bresid_;
+        if (p == d_qkv_) return *ld = Q, d_bqkv_;
+        if (p == d_attn_) return *ld = A, d_battn_;
+        if (p == d_act_) return *ld = F, d_bact_;
+        if (p == d_logits_) return *ld = V, d_blogits_;
+        return nullptr;
+    };
+    bool first = true;
+    for (const StepOp &op : ops_) {
+        const bool use_pdl = pdl && !first;
+        switch (op.type) {
+            case OP_EMBED:
+                DCK(launch_embedding_batch(c, (const __half *)w_.embed_f16, req, d_bresid_, E, batch, V, cfg_.max_ctx, n_slots(), d_bsafe_, use_pdl));
+                break;
+            case OP_GEMV: {
+                W4GemvParams p = op.g;
+                p.M = batch;
+                p.x = widen(p.x, &p.ldx);
+                p.y = widen(p.y, &p.ldy);
+                if (!p.x || !p.y) return cudaErrorUnknown;
+                p.pdl = use_pdl;
+                DCK(launch_w4a16_gemv(c, p));
+                break;
+            }
+            case OP_ATTN: {
+                AttnBatchArgs b{};
+                b.base = op.at;
+                b.base.qkv = d_bqkv_;
+                b.base.out = d_battn_;
+                b.base.ws = d_battn_ws_;
+                b.base.counters = d_battn_counters_;
+                b.ws_floats = battn_ws_floats_;
+                b.n_counters = battn_counters_;
+                b.req = d_bsafe_;
+                b.slots = d_slot_table_;
+                b.k_off = op.at.k_cache - d_kv_;  // this layer's slabs within a slot
+                b.v_off = op.at.v_cache - d_kv_;
+                b.qkv_stride = Q;
+                b.out_stride = A;
+                DCK(launch_attn_decode_batch(c, b, batch, use_pdl));
+                break;
+            }
+            case OP_ARGMAX:
+                DCK(launch_argmax_rows(c, d_blogits_, batch, V, d_bnext_, use_pdl));
+                break;
+            default:
+                return cudaErrorNotSupported;
+        }
+        first = false;
+    }
+    return cudaSuccess;
+}
+
+namespace {
+// capture `body` on `s` into an executable graph: with programmatic edges first, plain edges if the driver refuses them
+template <typename Body>
+cudaError_t capture_graph(cudaStream_t s, bool pdl, Body body, cudaGraphExec_t *out) {
+    for (int attempt = pdl ? 0 : 1; attempt < 2; attempt++) {
+        cudaGraph_t g = nullptr;
+        cudaError_t e = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal);
+        if (e != cudaSuccess) return e;
+        e = body(attempt == 0);
+        cudaError_t e2 = cudaStreamEndCapture(s, &g);
+        if (e == cudaSuccess) e = e2;
+        if (e == cudaSuccess) e = cudaGraphInstantiate(out, g, 0);
+        if (g) cudaGraphDestroy(g);
+        if (e == cudaSuccess) return e;
+        cudaGetLastError();
+        *out = nullptr;
+        if (attempt == 1) return e;
+    }
+    return cudaErrorUnknown;
+}
+}  // namespace
+
+cudaError_t LlamaDecoder::decode_batch_device(int batch, const int *req_dev, std::string *err) {
+    if (tp_ > 1) return batch_alloc(err);  // not supported, with its message
+    if (batch < 1 || batch > TCE_LLAMA_MAX_BATCH || !req_dev) return cudaErrorInvalidValue;
+    DCK(batch_alloc(err));
+    cudaStream_t s = ctx_->stream;
+    if (!use_graphs_) return enqueue_batch(batch, req_dev, s, ctx_->use_pdl);
+    cudaGraphExec_t &g = g_bdev_[batch];
+    if (g && (g_bdev_src_[batch] != req_dev || g_bdev_gen_[batch] != ctx_->option_gen)) {
+        cudaGraphExecDestroy(g);
+        g = nullptr;
+    }
+    if (!g) {
+        // one eager step first, outside of capture (module loads, kernel attributes); re-running a step rewrites the same K/V rows
+        DCK(cudaStreamSynchronize(s));
+        DCK(enqueue_batch(batch, req_dev, cap_stream_, false));
+        DCK(cudaStreamSynchronize(cap_stream_));
+        cudaError_t e = capture_graph(cap_stream_, ctx_->use_pdl, [&](bool pdl) { return enqueue_batch(batch, req_dev, cap_stream_, pdl); }, &g);
+        if (e != cudaSuccess) {
+            if (err) *err = std::string("batched graph capture failed: ") + cudaGetErrorString(e);
+            return e;
+        }
+        g_bdev_src_[batch] = req_dev;
+        g_bdev_gen_[batch] = ctx_->option_gen;
+    }
+    return cudaGraphLaunch(g, s);
+}
+
+cudaError_t LlamaDecoder::decode_batch_host(int batch, const int *tokens, const int *positions, const int *slots, float *logits_host, int *next_tokens,
+                                            std::string *err) {
+    if (tp_ > 1) return batch_alloc(err);  // not supported, with its message
+    if (batch < 1 || batch > TCE_LLAMA_MAX_BATCH || !tokens || !positions || !slots) return cudaErrorInvalidValue;
+    for (int b = 0; b < batch; b++) {
+        if (tokens[b] < 0 || tokens[b] >= cfg_.vocab_size || positions[b] < 0 || positions[b] >= cfg_.max_ctx || slots[b] < 0 || slots[b] >= n_slots())
+            return cudaErrorInvalidValue;
+        for (int o = 0; o < b; o++)
+            if (slots[o] == slots[b]) return cudaErrorInvalidValue;
+    }
+    DCK(batch_alloc(err));
+    for (int b = 0; b < batch; b++) {
+        h_breq_[3 * b] = tokens[b];
+        h_breq_[3 * b + 1] = positions[b];
+        h_breq_[3 * b + 2] = slots[b];
+    }
+    const int want = logits_host ? 1 : 0;
+    const size_t lbytes = (size_t)batch * cfg_.vocab_size * sizeof(float);
+    cudaStream_t s = ctx_->stream;
+    auto body = [&](cudaStream_t st, bool pdl) {
+        cudaError_t e = cudaMemcpyAsync(d_breq_, h_breq_, (size_t)batch * 3 * sizeof(int), cudaMemcpyHostToDevice, st);
+        if (e == cudaSuccess) e = enqueue_batch(batch, d_breq_, st, pdl);
+        if (e == cudaSuccess && want) e = cudaMemcpyAsync(h_blogits_, d_blogits_, lbytes, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(h_bnext_, d_bnext_, (size_t)batch * sizeof(int), cudaMemcpyDeviceToHost, st);
+        return e;
+    };
+    cudaGraphExec_t &g = g_bhost_[want][batch];
+    if (g && g_bhost_gen_[want][batch] != ctx_->option_gen) {  // an option or the stream changed since capture
+        cudaGraphExecDestroy(g);
+        g = nullptr;
+    }
+    if (use_graphs_ && !g) {
+        DCK(cudaStreamSynchronize(s));
+        DCK(body(cap_stream_, false));  // eager step outside of capture; re-running it rewrites the same K/V rows
+        DCK(cudaStreamSynchronize(cap_stream_));
+        cudaError_t e = capture_graph(cap_stream_, ctx_->use_pdl, [&](bool pdl) { return body(cap_stream_, pdl); }, &g);
+        if (e != cudaSuccess) {
+            if (err) *err = std::string("batched graph capture failed: ") + cudaGetErrorString(e);
+            return e;
+        }
+        g_bhost_gen_[want][batch] = ctx_->option_gen;
+    }
+    if (use_graphs_)
+        DCK(cudaGraphLaunch(g, s));
+    else
+        DCK(body(s, ctx_->use_pdl));
+    DCK(cudaStreamSynchronize(s));
+    if (logits_host) memcpy(logits_host, h_blogits_, lbytes);
+    if (next_tokens) memcpy(next_tokens, h_bnext_, (size_t)batch * sizeof(int));
     return cudaSuccess;
 }
 

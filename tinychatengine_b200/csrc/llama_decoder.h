@@ -20,9 +20,18 @@ class LlamaDecoder {
     cudaError_t generate(int first_token, int pos0, int n_predict, const tce_sampling &sc, const int *history_host, int n_history, int eos_id,
                          int *out_tokens_host, int *n_out, std::string *err);
     // prompt processing: n tokens at positions pos0..pos0+n-1 in one pass (tensor-core GEMMs + causal flash attention)
-    cudaError_t prefill(const int *tokens_host, int n, int pos0, float *logits_host, int *next_token, std::string *err);
+    cudaError_t prefill(const int *tokens_host, int n, int pos0, float *logits_host, int *next_token, std::string *err, int slot = 0);
     const float *logits() const { return d_logits_; }
-    void *kv_cache(int layer, int which) const;
+    void *kv_cache(int layer, int which) const { return kv_cache_slot(0, layer, which); }
+    // batched decode: up to TCE_LLAMA_MAX_BATCH sequences per step, each in its own KV-cache slot (slot 0 = d_kv_)
+    bool tensor_parallel() const { return tp_ > 1; }
+    int n_slots() const { return 1 + (int)slot_kv_.size(); }
+    cudaError_t reserve_slots(int n, std::string *err);
+    void *kv_cache_slot(int slot, int layer, int which) const;
+    cudaError_t decode_batch_device(int batch, const int *req_dev, std::string *err);
+    cudaError_t decode_batch_host(int batch, const int *tokens, const int *positions, const int *slots, float *logits_host, int *next_tokens,
+                                  std::string *err);
+    const float *batch_logits();
     int kernels_per_step() const { return kernels_per_step_; }
     void *debug_buffer(int which) const {
         switch (which) {
@@ -47,6 +56,9 @@ class LlamaDecoder {
     cudaError_t build_graphs(std::string *err);
     void build_ops();
     cudaError_t build_persistent(std::string *err);
+    cudaError_t batch_alloc(std::string *err);  // cudaErrorNotSupported (+ *err) for a model the batched step does not cover
+    cudaError_t enqueue_batch(int batch, const int *req, cudaStream_t s, bool pdl);  // raw kernel sequence of one batched step
+    void drop_batch_graphs();
 
     enum OpType { OP_EMBED, OP_GEMV, OP_ATTN, OP_ARGMAX, OP_TP_SIGNAL, OP_TP_ARGMAX_SCATTER, OP_TP_ARGMAX_FINISH };
     struct StepOp {
@@ -117,6 +129,29 @@ class LlamaDecoder {
     bool graphs_ok_ = false;
     unsigned graphs_gen_ = 0, g_dev_gen_ = 0;       // ctx_->option_gen at capture time
     int *d_tokpos_safe_ = nullptr;  // kernel-per-op path: {token, position} after the device-side range check (+ [2] unused, [3] TP step counter alias)
+    // batched decode state (allocated on first use): the step's buffers hold TCE_LLAMA_MAX_BATCH rows each
+    std::vector<__half *> slot_kv_;    // KV-cache slots 1.. ([L][2][KVH][max_ctx][hd] each)
+    __half **d_slot_table_ = nullptr;  // device table of every slot's base, slot 0 = d_kv_
+    float *d_bresid_ = nullptr;        // [8][E]
+    __half *d_bqkv_ = nullptr;         // [8][(H+2KVH)*hd]
+    __half *d_battn_ = nullptr;        // [8][H*hd]
+    __half *d_bact_ = nullptr;         // [8][F]
+    float *d_blogits_ = nullptr;       // [8][V]
+    int *d_breq_ = nullptr;            // [8][3] {token, position, slot} staged for the host entry point
+    int *d_bsafe_ = nullptr;           // [8][4] {token, position, slot, valid} after the device-side range check
+    int *d_bnext_ = nullptr;           // [8] greedy arg-max
+    float *d_battn_ws_ = nullptr;      // attention split records of 8 sequences at this model's max_ctx
+    size_t battn_ws_floats_ = 0;
+    unsigned *d_battn_counters_ = nullptr;  // [8][KVH] split arrival counters
+    size_t battn_counters_ = 0;
+    int *h_breq_ = nullptr, *h_bnext_ = nullptr;
+    float *h_blogits_ = nullptr;
+    // one graph per batch size: host entry (with / without the logits copy) and device entry (for one request pointer)
+    cudaGraphExec_t g_bhost_[2][TCE_LLAMA_MAX_BATCH + 1] = {};
+    unsigned g_bhost_gen_[2][TCE_LLAMA_MAX_BATCH + 1] = {};
+    cudaGraphExec_t g_bdev_[TCE_LLAMA_MAX_BATCH + 1] = {};
+    const int *g_bdev_src_[TCE_LLAMA_MAX_BATCH + 1] = {};
+    unsigned g_bdev_gen_[TCE_LLAMA_MAX_BATCH + 1] = {};
     bool use_graphs_ = true;
     bool atomic_residual_ = true;  // o_proj/down_proj partial tiles use RED.ADD (TCE_DETERMINISTIC=1 turns it off)
     int kernels_per_step_ = 0;

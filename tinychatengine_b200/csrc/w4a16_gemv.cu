@@ -17,7 +17,8 @@ template <int NCOLS, int CW>
 __global__ void __launch_bounds__(32 * (kProducerWarps + 1 + CW), (NCOLS == 1 && CW == 8) ? 2 : 1) w4a16_gemv_kernel(const __grid_constant__ KArgs a) {
     extern __shared__ __align__(128) uint8_t smem[];
     using L = Layout<NCOLS, CW>;
-    const Smem sm = carve<NCOLS, CW>(smem, a.IC, a.nst);
+    const int xw = NCOLS == 1 ? a.IC : a.sl * 128;  // activation elements staged per column
+    const Smem sm = carve<NCOLS, CW>(smem, a.IC, a.nst, xw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int cta = blockIdx.x, ncta = gridDim.x;
 
@@ -41,7 +42,10 @@ __global__ void __launch_bounds__(32 * (kProducerWarps + 1 + CW), (NCOLS == 1 &&
 
     if (warp < kProducerWarps) {
         RingState rs;
-        produce(a, sm, rs, cta, ncta, lane, l2_policy_evict_first());
+        if constexpr (NCOLS == 1)
+            produce(a, sm, rs, cta, ncta, lane, l2_policy_evict_first());
+        else
+            produce_cols(a, sm, rs, cta, ncta, lane, l2_policy_evict_first());
         // this CTA has requested its last byte of weights: a programmatically dependent kernel may become resident
         pdl_launch_dependents();
         return;
@@ -49,19 +53,32 @@ __global__ void __launch_bounds__(32 * (kProducerWarps + 1 + CW), (NCOLS == 1 &&
     if (warp == kProducerWarps) {
         pdl_wait();  // outputs (and the residual we add into) belong to earlier kernels
         RedState es;
-        epilogue<NCOLS, CW>(a, sm, es, cta, ncta, lane);
+        if constexpr (NCOLS == 1)
+            epilogue<NCOLS, CW>(a, sm, es, cta, ncta, lane);
+        else
+            epilogue_cols<NCOLS, CW>(a, sm, es, cta, ncta, lane);
         if (lane == 0) dbg_stamp(a, cta, 5);
         return;
     }
     const int ctid = tid - 32 * (kProducerWarps + 1);
     const int cw = warp - (kProducerWarps + 1);
     pdl_wait();  // activations belong to the previous kernel until here
-    stage_activations<NCOLS, CW>(a, sm, L::x_pitch(a.IC), ctid, cw, lane);
+    int s0 = 0;
+    if constexpr (NCOLS == 1) {
+        stage_activations<NCOLS, CW>(a, sm, L::x_pitch(a.IC), ctid, cw, lane);
+    } else {
+        if (a.x_mode == X_RMSNORM_F32) rms_partials<NCOLS, CW>(a, sm, ctid, cw, lane);
+        s0 = first_slice(a, cta, ncta);
+        stage_slice<NCOLS, CW>(a, sm, L::x_pitch(xw), s0, ctid, cw, lane);
+    }
     if (ctid == 0) dbg_stamp(a, cta, 2);
     asm volatile("bar.sync 3, %0;" ::"r"(32 * (kProducerWarps + 1 + CW)) : "memory");
     RingState rs;
     RedState cs;
-    consume<NCOLS, CW>(a, sm, rs, cs, L::x_pitch(a.IC), cta, ncta, cw, lane);
+    if constexpr (NCOLS == 1)
+        consume<NCOLS, CW>(a, sm, rs, cs, L::x_pitch(a.IC), cta, ncta, cw, lane);
+    else
+        consume_cols<NCOLS, CW>(a, sm, rs, cs, L::x_pitch(xw), s0, cta, ncta, ctid, cw, lane);
     if (ctid == 0) dbg_stamp(a, cta, 4);
 }
 
@@ -238,6 +255,8 @@ KArgs make_kargs(Ctx *ctx, const W4GemvParams &p, int *total_rows) {
     a.aligned = 0;
     a.sg = a.NG < kStageGroups ? a.NG : kStageGroups;
     a.full = (a.NG % kStageGroups == 0) ? 1 : 0;
+    a.sl = a.NG;
+    a.nsl = 1;
     a.tp_size = p.tp_size;
     a.tp_in = p.tp_in;
     a.tp_flags = p.tp_flags;
@@ -256,10 +275,31 @@ KArgs make_kargs(Ctx *ctx, const W4GemvParams &p, int *total_rows) {
     return a;
 }
 
+// The one rule for what fits in shared memory: the deepest TMA ring of 2..max_nst stages next to `xw` staged activation elements per column,
+// within `budget` bytes; 0 when not even two stages fit.
+template <int NCOLS, int CW>
+int ring_fit(int IC, int xw, int budget, int max_nst) {
+    for (int nst = max_nst; nst >= 2; nst--)
+        if ((int)Layout<NCOLS, CW>::bytes(IC, nst, xw) <= budget) return nst;
+    return 0;
+}
+
+// K-slice of the multi-column kernel: the whole row when it fits next to a kStages ring, else the widest whole number of 16-group stages
+// that does (at least one stage's worth of groups, with the shallowest ring)
+template <int CW>
+int pick_slice(int IC, int budget) {
+    const int NG = IC / kW4Group;
+    if (ring_fit<8, CW>(IC, IC, budget, kStages) == kStages) return NG;
+    for (int sl = (NG - 1) / kStageGroups * kStageGroups; sl >= kStageGroups; sl -= kStageGroups)
+        if (ring_fit<8, CW>(IC, sl * kW4Group, budget, kStages) >= kStages) return sl;
+    return ring_fit<8, CW>(IC, kStageGroups * kW4Group, budget, kStages) ? kStageGroups : 0;
+}
+
 template <int NCOLS, int CW>
 cudaError_t launch_mma(Ctx *ctx, const KArgs &a_in, bool pdl) {
     KArgs a = a_in;
-    if ((int)Layout<NCOLS, CW>::bytes(a.IC, kStages) > ctx->smem_optin) return cudaErrorInvalidConfiguration;
+    const int xw = NCOLS == 1 ? a.IC : a.sl * kW4Group;
+    if (!ring_fit<NCOLS, CW>(a.IC, xw, ctx->smem_optin, kStages)) return cudaErrorInvalidConfiguration;
     static DeviceOnce attr_once;  // per template instantiation
     if (attr_once.pending(ctx->device)) {
         cudaError_t e = cudaFuncSetAttribute(w4a16_gemv_kernel<NCOLS, CW>, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->smem_optin);
@@ -279,10 +319,15 @@ cudaError_t launch_mma(Ctx *ctx, const KArgs &a_in, bool pdl) {
     if (nc > ctx->gemv_max_ctas) nc = ctx->gemv_max_ctas;
     const long long cuts = a.full ? U / kStageGroups : U;  // stream-K cuts fall on whole stages when every stage is full
     if ((long long)nc > cuts) nc = (int)cuts;
+    if (a.nsl > 1) {
+        // CTA ranges are cut at (slice, tile) segment boundaries: one fix-up record per segment
+        if ((long long)nc > (long long)a.num_tiles * a.nsl) nc = a.num_tiles * a.nsl;
+        if ((long long)a.num_tiles * a.nsl > ctx->gemv_partial_records) return cudaErrorInvalidValue;  // launch_w4a16_gemv reserves them
+    }
     // Epilogues that need a single ordered writer per output (stores, SiLU*mul, deterministic residual) avoid split
     // tiles altogether when there is at least one whole tile per CTA: the fix-up protocol adds a tail to every
-    // launch, more than the <= 1/tiles_per_cta imbalance it removes.
-    a.aligned = (!a.atomic_add && a.num_tiles >= nc) ? 1 : 0;
+    // launch, more than the <= 1/tiles_per_cta imbalance it removes.  Slice-major units have no whole tiles.
+    a.aligned = (!a.atomic_add && a.num_tiles >= nc && a.nsl == 1) ? 1 : 0;
     // Ring depth = bytes in flight per SM.  HBM latency under load (~1.2 us) x 3.35 TB/s / 132 SMs = ~30 KB must be in flight per SM
     // all the time, and a slot is only re-requested after it was consumed: the deepest ring that fits the per-CTA share of shared
     // memory (1 KiB per CTA is reserved by the driver), at most kMaxStages and no more stages than the CTA has work for.
@@ -290,12 +335,13 @@ cudaError_t launch_mma(Ctx *ctx, const KArgs &a_in, bool pdl) {
         const int budget = ctx->smem_optin / per_sm - (per_sm > 1 ? 1024 : 0);
         int nst = ctx->gemv_stages > 0 ? ctx->gemv_stages : kMaxStages;
         if (nst > kMaxStages) nst = kMaxStages;
-        while (nst > 2 && (int)Layout<NCOLS, CW>::bytes(a.IC, nst) > budget) nst--;
+        const int fit = ring_fit<NCOLS, CW>(a.IC, xw, budget, nst);
+        nst = fit ? fit : 2;
         const long long stages_per_cta = (U / nc + a.sg - 1) / a.sg + 1;
         if (nst > stages_per_cta && stages_per_cta >= 2) nst = (int)stages_per_cta;
         a.nst = nst;
     }
-    const size_t smem = Layout<NCOLS, CW>::bytes(a.IC, a.nst);
+    const size_t smem = Layout<NCOLS, CW>::bytes(a.IC, a.nst, xw);
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(nc);
     cfg.blockDim = dim3(32 * (kProducerWarps + 1 + CW));
@@ -311,11 +357,6 @@ cudaError_t launch_mma(Ctx *ctx, const KArgs &a_in, bool pdl) {
 
 }  // namespace
 
-size_t w4a16_gemv_smem_bytes(int ncols, int cw, int IC) {
-    if (ncols == 1) return cw == 16 ? Layout<1, 16>::bytes(IC, kStages) : Layout<1, 8>::bytes(IC, kStages);
-    return cw == 16 ? Layout<8, 16>::bytes(IC, kStages) : Layout<8, 8>::bytes(IC, kStages);
-}
-
 cudaError_t launch_w4a16_gemv_simple(Ctx *ctx, const W4GemvParams &p) {
     if (p.pair_mode || p.x_mode != X_HALF) return cudaErrorNotSupported;
     int rows;
@@ -323,6 +364,48 @@ cudaError_t launch_w4a16_gemv_simple(Ctx *ctx, const W4GemvParams &p) {
     const int warps = 8;
     w4a16_gemv_simple_kernel<<<(rows + warps - 1) / warps, warps * 32, 0, ctx->stream>>>(a, rows);
     return cudaGetLastError();
+}
+
+namespace {
+// 16 consumer warps pay off on long rows (down_proj, IC = 14336), where one CTA per SM stages a long activation
+// vector and the 2-CTA mode is off; 8 warps (x 2 CTAs on large launches) everywhere else
+int consumer_warps(const Ctx *ctx, const W4GemvParams &p) {
+    return ctx->gemv_consumer_warps == 16 ? 16 : (ctx->gemv_consumer_warps == 8 ? 8 : (p.IC > 8192 && p.M == 1 ? 16 : 8));
+}
+// K-slice of a multi-column launch (groups; 0 = nothing fits)
+int slice_of(const Ctx *ctx, const W4GemvParams &p) {
+    return consumer_warps(ctx, p) == 16 ? pick_slice<16>(p.IC, ctx->smem_optin) : pick_slice<8>(p.IC, ctx->smem_optin);
+}
+}  // namespace
+
+long long w4a16_gemv_fixup_records(const Ctx *ctx, const W4GemvParams &p) {
+    if (p.M <= 1 || p.IC < kW4Group) return 0;
+    const int NG = p.IC / kW4Group, sl = slice_of(ctx, p);
+    if (sl <= 0 || sl >= NG) return 0;
+    int rows = 0;
+    for (int i = 0; i < p.nseg && i < 3; i++) rows += p.seg[i].rows;
+    return (long long)(rows / 16) * ((NG + sl - 1) / sl);
+}
+
+cudaError_t gemv_partials_reserve(Ctx *ctx, long long records) {
+    if (records <= ctx->gemv_partial_records) return cudaSuccess;
+    if (records > (1ll << 24)) return cudaErrorInvalidValue;
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    cudaError_t e = cudaStreamIsCapturing(ctx->stream, &st);
+    if (e != cudaSuccess) return e;
+    if (st != cudaStreamCaptureStatusNone) return cudaErrorStreamCaptureUnsupported;  // grow it with one launch outside of capture first
+    float *p = nullptr;
+    e = cudaMalloc(&p, (size_t)records * 16 * 8 * sizeof(float));
+    if (e != cudaSuccess) return e;
+    e = cudaFree(ctx->gemv_partials);  // synchronises: no launch still uses the old records
+    if (e != cudaSuccess) {
+        cudaFree(p);
+        return e;
+    }
+    ctx->gemv_partials = p;
+    ctx->gemv_partial_records = (int)records;
+    ctx->option_gen++;  // graphs captured on this context hold the old pointer
+    return cudaSuccess;
 }
 
 cudaError_t launch_w4a16_gemv(Ctx *ctx, const W4GemvParams &p) {
@@ -337,25 +420,19 @@ cudaError_t launch_w4a16_gemv(Ctx *ctx, const W4GemvParams &p) {
         cudaError_t e = encode_w4_tmap(&a.tmap[i], p.seg[i].w, p.seg[i].rows, p.IC, a.sg, p.pair_mode ? 8 : 16);
         if (e != cudaSuccess) return e;
     }
-    // 16 consumer warps pay off on long rows (down_proj, IC = 14336), where one CTA per SM stages a long activation
-    // vector and the 2-CTA mode is off; 8 warps (x 2 CTAs on large launches) everywhere else
-    const int cw = ctx->gemv_consumer_warps == 16 ? 16 : (ctx->gemv_consumer_warps == 8 ? 8 : (p.IC > 8192 && p.M == 1 ? 16 : 8));
-    if (p.M > 1 && (int)w4a16_gemv_smem_bytes(8, cw, p.IC) > ctx->smem_optin) {
-        // the 8-column activation tile does not fit next to the weight ring: one pass per activation row
-        if (p.pair_mode && p.ldy == 0) return cudaErrorInvalidValue;
-        for (int m = 0; m < p.M; m++) {
-            KArgs am = a;
-            am.M = 1;
-            const size_t xel = (p.x_mode == X_RMSNORM_F32) ? sizeof(float) : sizeof(__half);
-            am.x = reinterpret_cast<const uint8_t *>(a.x) + (size_t)m * a.ldx * xel;
-            const size_t yel = (p.pair_mode || p.epi == EPI_STORE_HALF) ? sizeof(__half) : sizeof(float);
-            am.y = reinterpret_cast<uint8_t *>(a.y) + (size_t)m * a.ldy * yel;
-            cudaError_t e = (cw == 16) ? launch_mma<1, 16>(ctx, am, p.pdl) : launch_mma<1, 8>(ctx, am, p.pdl);
-            if (e != cudaSuccess) return e;
-        }
-        return cudaSuccess;
-    }
+    const int cw = consumer_warps(ctx, p);
     if (p.M == 1) return (cw == 16) ? launch_mma<1, 16>(ctx, a, p.pdl) : launch_mma<1, 8>(ctx, a, p.pdl);
+    // M = 2..8: one pass over the weights, the activation rows staged one K-slice at a time where the whole rows do not fit
+    if (p.tp_size > 1) return cudaErrorNotSupported;
+    a.sl = slice_of(ctx, p);
+    if (a.sl == 0) return cudaErrorInvalidConfiguration;
+    a.nsl = (a.NG + a.sl - 1) / a.sl;
+    if (a.nsl > kMaxSlices) return cudaErrorInvalidConfiguration;
+    if (a.nsl > 1) {  // one fix-up record per (slice, row tile)
+        cudaError_t e = gemv_partials_reserve(ctx, (long long)a.num_tiles * a.nsl);
+        if (e != cudaSuccess) return e;
+        a.partials = ctx->gemv_partials;
+    }
     return (cw == 16) ? launch_mma<8, 16>(ctx, a, p.pdl) : launch_mma<8, 8>(ctx, a, p.pdl);
 }
 

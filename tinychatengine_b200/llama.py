@@ -296,21 +296,54 @@ class LlamaModel:
                                                  out.ctypes.data_as(C.c_void_p), C.byref(n)), "tce_llama_generate")
         return out[:n.value].tolist()
 
-    def prefill(self, tokens, pos0: int = 0, logits_host=None) -> int:
-        """Prompt processing: all `tokens` (host ints) at positions pos0.. in one pass; returns the greedy next token."""
+    def prefill(self, tokens, pos0: int = 0, logits_host=None, slot: int = 0) -> int:
+        """Prompt processing: all `tokens` (host ints) at positions pos0.. in one pass into KV-cache slot `slot`; returns the greedy next
+        token."""
         arr = (C.c_int * len(tokens))(*[int(t) for t in tokens])
         nxt = C.c_int(-1)
         p = None if logits_host is None else C.c_void_p(logits_host.data_ptr())
-        _lib.check(self.ctx.L.tce_llama_prefill(self.h, arr, len(tokens), int(pos0), p, C.byref(nxt)), "tce_llama_prefill")
+        if slot == 0:
+            _lib.check(self.ctx.L.tce_llama_prefill(self.h, arr, len(tokens), int(pos0), p, C.byref(nxt)), "tce_llama_prefill")
+        else:
+            _lib.check(self.ctx.L.tce_llama_prefill_slot(self.h, int(slot), arr, len(tokens), int(pos0), p, C.byref(nxt)), "tce_llama_prefill_slot")
         return nxt.value
+
+    MAX_BATCH = 8  # TCE_LLAMA_MAX_BATCH
+
+    def reserve_slots(self, n_slots: int):
+        """Grow the number of KV-cache slots to `n_slots` (slot 0 is the single-sequence cache; never shrinks)."""
+        _lib.check(self.ctx.L.tce_llama_reserve_slots(self.h, int(n_slots)), "tce_llama_reserve_slots")
+
+    def decode_batch(self, req_dev: torch.Tensor):
+        """One batched step from a device int32 [batch, 3] tensor of {token, position, slot}; logits land in batch_logits()."""
+        assert req_dev.dtype == torch.int32 and req_dev.is_contiguous() and req_dev.dim() == 2 and req_dev.shape[1] == 3
+        _lib.check(self.ctx.L.tce_llama_decode_batch(self.h, int(req_dev.shape[0]), C.c_void_p(req_dev.data_ptr())), "tce_llama_decode_batch")
+
+    def decode_batch_host(self, tokens, positions, slots, logits_host=None):
+        """One batched step from host lists; fills logits_host (float32 [batch, vocab], may be None) and returns the greedy tokens."""
+        n = len(tokens)
+        arr = lambda v: (C.c_int * max(1, n))(*[int(x) for x in v])
+        nxt = (C.c_int * max(1, n))()
+        p = None if logits_host is None else C.c_void_p(logits_host.data_ptr())
+        _lib.check(self.ctx.L.tce_llama_decode_batch_host(self.h, n, arr(tokens), arr(positions), arr(slots), p, nxt), "tce_llama_decode_batch_host")
+        return list(nxt[:n])
+
+    def batch_logits(self) -> torch.Tensor:
+        """View of the device logits of the batched step (float32 [MAX_BATCH, vocab])."""
+        ptr = self.ctx.L.tce_llama_batch_logits(self.h)
+        if not ptr:
+            raise _lib.TceError("tce_llama_batch_logits: no batched-step buffers (tensor-parallel model?)")
+        return _tensor_from_ptr(ptr, (self.MAX_BATCH, self.geom.vocab_size), torch.float32, self.ctx.device)
 
     def logits(self) -> torch.Tensor:
         """View of the device logits buffer (float32 [vocab])."""
         ptr = self.ctx.L.tce_llama_logits(self.h)
         return _tensor_from_ptr(ptr, (self.geom.vocab_size,), torch.float32, self.ctx.device)
 
-    def kv_cache(self, layer: int, which: int) -> torch.Tensor:
-        ptr = self.ctx.L.tce_llama_kv_cache(self.h, layer, which)
+    def kv_cache(self, layer: int, which: int, slot: int = 0) -> torch.Tensor:
+        ptr = self.ctx.L.tce_llama_kv_cache(self.h, layer, which) if slot == 0 else self.ctx.L.tce_llama_kv_cache_slot(self.h, slot, layer, which)
+        if slot != 0 and not ptr:
+            raise _lib.TceError(f"no KV cache for slot {slot}, layer {layer}, which {which}")
         return _tensor_from_ptr(ptr, (self.geom.num_kv_heads, self.max_ctx, self.geom.head_dim), torch.float16, self.ctx.device)
 
     def debug_buffer(self, which: int) -> torch.Tensor:

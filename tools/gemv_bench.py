@@ -16,7 +16,7 @@ sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 from tinychatengine_b200.runtime import Context, random_w4  # noqa: E402
 
 SHAPES = {"o_proj 4096x4096": (4096, 4096), "qkv 6144x4096": (6144, 4096), "gate_up 28672x4096": (28672, 4096),
-          "down 4096x14336": (4096, 14336), "lm_head 128256x4096": (128256, 4096)}
+          "down 4096x14336": (4096, 14336), "down 4096x11008": (4096, 11008), "lm_head 128256x4096": (128256, 4096)}
 
 
 def alg_bytes(oc, ic):
