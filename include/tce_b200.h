@@ -228,6 +228,28 @@ TCE_API int tce_llama_decode_batch(tce_llama *m, int batch, const int *req_dev);
 TCE_API int tce_llama_decode_batch_host(tce_llama *m, int batch, const int *tokens, const int *positions, const int *slots, float *logits_host,
                                         int *next_tokens);
 TCE_API const float *tce_llama_batch_logits(tce_llama *m);    /* device float[TCE_LLAMA_MAX_BATCH][vocab] */
+/* Prompt processing of n_seqs prompts, 1 <= n_seqs <= TCE_LLAMA_MAX_BATCH, in ONE pass over the weights (the int4 weights are expanded to
+ * fp16 once for all of them).  tokens_host = the prompts concatenated; prompt s has lengths[s] >= 1 tokens at positions pos0s[s].. in slot
+ * slots[s].  logits_host float[n_seqs][vocab] (last position of each prompt) and next_tokens int[n_seqs] (greedy) may be NULL.
+ * TCE_ERR_INVALID, before anything is enqueued, for n_seqs outside [1, TCE_LLAMA_MAX_BATCH], a length < 1, pos0 + length > max_ctx, a slot
+ * >= the reserved count or named twice, or a token outside [0, vocab).  Synchronous.                                                   */
+TCE_API int tce_llama_prefill_batch(tce_llama *m, int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots,
+                                    float *logits_host, int *next_tokens);
+typedef struct tce_gen_request {
+    int first_token, pos0, slot;   /* decode first_token at pos0 in slot, as tce_llama_generate does for slot 0 */
+    int n_predict, eos_id;         /* per-sequence budget and stop id (-1: none) */
+    const int *history;            /* host, oldest first, may be NULL */
+    int n_history;
+    tce_sampling sampling;         /* per-sequence chain and seed */
+} tce_gen_request;
+/* Generate loop of `batch` sequences, 1 <= batch <= TCE_LLAMA_MAX_BATCH: per token one batched step and one device sampler launch (a block
+ * per sequence, each with its own chain, seed, history window, EOS and budget).  A sequence stops when it draws its eos_id, when it has
+ * n_predict ids (clamped to max_ctx - pos0, as tce_llama_generate clamps) or when its next position would be max_ctx; from then on it
+ * appends no KV row.  On return slot s holds exactly n_out[s] new rows, at pos0 .. pos0 + n_out[s] - 1 (the last id is not decoded).
+ * out_tokens_host int[batch][out_stride], n_out int[batch].  Only ids cross PCIe.  TCE_ERR_INVALID, before anything is enqueued, for a bad
+ * batch, slot (unreserved or repeated), first_token, pos0, n_predict < 0, n_history outside [0, max_ctx], out_stride below a clamped
+ * n_predict or a NULL pointer; TCE_ERR_UNSUPPORTED for temp > 0 without 1 <= top_k <= 1024.                                           */
+TCE_API int tce_llama_generate_batch(tce_llama *m, int batch, const tce_gen_request *reqs, int *out_tokens_host, int out_stride, int *n_out);
 TCE_API const float *tce_llama_logits(tce_llama *m);          /* device float[vocab] */
 TCE_API void *tce_llama_kv_cache(tce_llama *m, int layer, int which); /* which: 0 K, 1 V; half[KVH][max_ctx][hd] */
 TCE_API int tce_llama_kernels_per_step(tce_llama *m);

@@ -37,6 +37,11 @@ class Sampling(C.Structure):
                 ("presence_penalty", C.c_float), ("repeat_last_n", C.c_int), ("seed", C.c_ulonglong)]
 
 
+class GenRequest(C.Structure):
+    """tce_gen_request (include/tce_b200.h): one sequence of tce_llama_generate_batch."""
+    _fields_ = [("first_token", C.c_int), ("pos0", C.c_int), ("slot", C.c_int), ("n_predict", C.c_int), ("eos_id", C.c_int),
+                ("history", C.POINTER(C.c_int)), ("n_history", C.c_int), ("sampling", Sampling)]
+
 
 # every symbol include/tce_b200.h declares (tests/test_capi_symbols.py checks header <-> library <-> this table)
 SIGNATURES = {
@@ -78,6 +83,8 @@ SIGNATURES = {
     "tce_llama_prefill_slot": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "tce_llama_decode_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     "tce_llama_decode_batch_host": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tce_llama_prefill_batch": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 6),
+    "tce_llama_generate_batch": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(GenRequest), C.c_void_p, C.c_int, C.c_void_p]),
     "tce_llama_batch_logits": (C.c_void_p, [C.c_void_p]),
     "tce_llama_logits": (C.c_void_p, [C.c_void_p]),
     "tce_llama_kv_cache": (C.c_void_p, [C.c_void_p, C.c_int, C.c_int]),

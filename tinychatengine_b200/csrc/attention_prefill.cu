@@ -6,6 +6,8 @@
 //      O += P V on mma.sync m16n8k16 (fp16 in, fp32 accumulate), causal mask by position, online softmax in fp32 -- no [n][T] score
 //      tensor in HBM (the reference materialises it, plus a V transpose, per layer).
 // head_dim is 128 (every Llama geometry of the reference, llm/include/model.h:71-83).
+// One launch takes up to kMaxPrefillSeqs prompts with their rows concatenated (AttnPrefillArgs::seq, in row order): a token row and a
+// query block find their sequence in that table and use its positions and its KV cache.  A single prompt is the one-entry table.
 #include "common.cuh"
 #include "kernels_attn.h"
 
@@ -17,12 +19,24 @@ constexpr int kQB = 64;        // query rows per CTA (16 per warp)
 constexpr int kKT = 64;        // cached rows per tile
 constexpr int kPitch = HD + 8; // halves; 272-byte rows: conflict-free fragment loads and 16-byte aligned ldmatrix rows
 
+// query blocks of 64 rows of one sequence; block qb sees keys 0 .. block_keys(q, qb) - 1, a number that rises strictly with qb
+__host__ __device__ inline int q_blocks(const AttnPrefillSeq &q) { return (q.n + kQB - 1) / kQB; }
+TCE_DEVINL int block_keys(const AttnPrefillSeq &q, int qb) { return q.pos0 + min(q.n, (qb + 1) * kQB); }
+TCE_DEVINL int blocks_upto(const AttnPrefillSeq &q, int keys) {  // blocks of q that see at most `keys` keys
+    if (keys >= q.pos0 + q.n) return q_blocks(q);
+    return keys < q.pos0 + kQB ? 0 : min((keys - q.pos0) / kQB, q_blocks(q) - 1);
+}
+
 // one 256-thread block per token; a warp per head slot (q heads, then kv heads), a lane per pair of adjacent dims and their rotate-half
 // partners: 4-byte loads / stores, the position's cos / sin rows read as float2
 __global__ void __launch_bounds__(256) rope_kv_append_kernel(const AttnPrefillArgs a) {
     const int i = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int QKV = (a.num_heads + 2 * a.num_kv_heads) * HD;
-    const int pos = a.pos0 + i;
+    int s = 0;
+    for (int j = 1; j < a.n_seqs; j++)
+        if (i >= a.seq[j].row0) s = j;
+    const AttnPrefillSeq &sq = a.seq[s];
+    const int pos = sq.pos0 + (i - sq.row0);
     const float2 c0 = *reinterpret_cast<const float2 *>(a.cos + (size_t)pos * HD + 2 * lane), c1 = *reinterpret_cast<const float2 *>(a.cos + (size_t)pos * HD + HD / 2 + 2 * lane);
     const float2 s0 = *reinterpret_cast<const float2 *>(a.sin + (size_t)pos * HD + 2 * lane), s1 = *reinterpret_cast<const float2 *>(a.sin + (size_t)pos * HD + HD / 2 + 2 * lane);
     for (int hh = warp; hh < a.num_heads + a.num_kv_heads; hh += 8) {
@@ -35,7 +49,7 @@ __global__ void __launch_bounds__(256) rope_kv_append_kernel(const AttnPrefillAr
             *reinterpret_cast<__half2 *>(row + HD / 2 + 2 * lane) = r1;
         } else {
             const int kvh = hh - a.num_heads;
-            __half *kc = a.k_cache + ((size_t)kvh * a.max_ctx + pos) * HD, *vc = a.v_cache + ((size_t)kvh * a.max_ctx + pos) * HD;
+            __half *kc = sq.k_cache + ((size_t)kvh * a.max_ctx + pos) * HD, *vc = sq.v_cache + ((size_t)kvh * a.max_ctx + pos) * HD;
             const __half *v = a.qkv + (size_t)i * QKV + (size_t)(a.num_heads + a.num_kv_heads + kvh) * HD;
             *reinterpret_cast<__half2 *>(kc + 2 * lane) = r0;
             *reinterpret_cast<__half2 *>(kc + HD / 2 + 2 * lane) = r1;
@@ -51,24 +65,43 @@ TCE_DEVINL void ldmatrix_x4_trans(uint32_t &r0, uint32_t &r1, uint32_t &r2, uint
 __global__ void __launch_bounds__(128) attn_prefill_kernel(const AttnPrefillArgs a) {
     __shared__ __align__(16) __half sK[kKT * kPitch];
     __shared__ __align__(16) __half sV[kKT * kPitch];
-    const int qb = gridDim.x - 1 - blockIdx.x;  // longest blocks first
-    const int h = blockIdx.y, kvh = h / (a.num_heads / a.num_kv_heads);
+    __shared__ int pick;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, grp = lane >> 2, qd = lane & 3;
+    // longest blocks first over all sequences: CTA x takes the block of rank x in the order (keys seen descending, sequence ascending).
+    // Candidate c (blocks numbered sequence by sequence) counts the blocks ahead of it; exactly one candidate has rank blockIdx.x.
+    for (int c = tid; c < (int)gridDim.x; c += blockDim.x) {
+        int t = 0, b = c;
+        while (b >= q_blocks(a.seq[t])) b -= q_blocks(a.seq[t++]);
+        const int keys = block_keys(a.seq[t], b);
+        int rank = 0;
+        for (int u = 0; u < a.n_seqs; u++) {
+            const int upto = blocks_upto(a.seq[u], keys);
+            rank += q_blocks(a.seq[u]) - upto;
+            if (u < t) rank += upto - blocks_upto(a.seq[u], keys - 1);
+        }
+        if (rank == (int)blockIdx.x) pick = (t << 16) | b;
+    }
+    __syncthreads();
+    const AttnPrefillSeq &sq = a.seq[pick >> 16];
+    const int qb = pick & 0xffff;
+    const int h = blockIdx.y, kvh = h / (a.num_heads / a.num_kv_heads);
     const int QKV = (a.num_heads + 2 * a.num_kv_heads) * HD;
-    const int r_lo = qb * kQB + warp * 16 + grp, r_hi = r_lo + 8;  // this thread's two query rows (index within the call)
-    const __half *Kc = a.k_cache + (size_t)kvh * a.max_ctx * HD, *Vc = a.v_cache + (size_t)kvh * a.max_ctx * HD;
+    const int n = sq.n;
+    const int r_lo = qb * kQB + warp * 16 + grp, r_hi = r_lo + 8;  // this thread's two query rows (index within the sequence)
+    const __half *Kc = sq.k_cache + (size_t)kvh * a.max_ctx * HD, *Vc = sq.v_cache + (size_t)kvh * a.max_ctx * HD;
+    __half *const qkv = a.qkv + (size_t)sq.row0 * QKV, *const out = a.out + (size_t)sq.row0 * a.num_heads * HD;
 
     // Q fragments (A operand, row-major 16 x 128): 8 k-steps x 4 registers, straight from the rotated projections
     uint32_t qf[8][4];
     {
-        const __half *q_lo = a.qkv + (size_t)r_lo * QKV + (size_t)h * HD, *q_hi = a.qkv + (size_t)r_hi * QKV + (size_t)h * HD;
+        const __half *q_lo = qkv + (size_t)r_lo * QKV + (size_t)h * HD, *q_hi = qkv + (size_t)r_hi * QKV + (size_t)h * HD;
 #pragma unroll
         for (int ks = 0; ks < 8; ks++) {
             const int c = ks * 16 + qd * 2;
-            qf[ks][0] = r_lo < a.n ? *reinterpret_cast<const uint32_t *>(q_lo + c) : 0u;
-            qf[ks][1] = r_hi < a.n ? *reinterpret_cast<const uint32_t *>(q_hi + c) : 0u;
-            qf[ks][2] = r_lo < a.n ? *reinterpret_cast<const uint32_t *>(q_lo + c + 8) : 0u;
-            qf[ks][3] = r_hi < a.n ? *reinterpret_cast<const uint32_t *>(q_hi + c + 8) : 0u;
+            qf[ks][0] = r_lo < n ? *reinterpret_cast<const uint32_t *>(q_lo + c) : 0u;
+            qf[ks][1] = r_hi < n ? *reinterpret_cast<const uint32_t *>(q_hi + c) : 0u;
+            qf[ks][2] = r_lo < n ? *reinterpret_cast<const uint32_t *>(q_lo + c + 8) : 0u;
+            qf[ks][3] = r_hi < n ? *reinterpret_cast<const uint32_t *>(q_hi + c + 8) : 0u;
         }
     }
     float o[16][4];
@@ -76,9 +109,8 @@ __global__ void __launch_bounds__(128) attn_prefill_kernel(const AttnPrefillArgs
     for (int d = 0; d < 16; d++) o[d][0] = o[d][1] = o[d][2] = o[d][3] = 0.f;
     float m_lo = -INFINITY, m_hi = -INFINITY, l_lo = 0.f, l_hi = 0.f;
     const float sc = a.alpha * 1.4426950408889634f;  // scores kept in log2 units
-    const int qpos_lo = a.pos0 + r_lo, qpos_hi = a.pos0 + r_hi;
-    const int rows_here = min(kQB, a.n - qb * kQB);
-    const int kv_len = a.pos0 + qb * kQB + rows_here;  // keys this block can see
+    const int qpos_lo = sq.pos0 + r_lo, qpos_hi = sq.pos0 + r_hi;
+    const int kv_len = block_keys(sq, qb);  // keys this block can see
     const int tiles = (kv_len + kKT - 1) / kKT;
 
     for (int kt = 0; kt < tiles; kt++) {
@@ -169,19 +201,26 @@ __global__ void __launch_bounds__(128) attn_prefill_kernel(const AttnPrefillArgs
 #pragma unroll
     for (int d = 0; d < 16; d++) {
         const int c = d * 8 + qd * 2;
-        if (r_lo < a.n) *reinterpret_cast<uint32_t *>(a.out + (size_t)r_lo * ldo + (size_t)h * HD + c) = pack_half2(o[d][0] * inv_lo, o[d][1] * inv_lo);
-        if (r_hi < a.n) *reinterpret_cast<uint32_t *>(a.out + (size_t)r_hi * ldo + (size_t)h * HD + c) = pack_half2(o[d][2] * inv_hi, o[d][3] * inv_hi);
+        if (r_lo < n) *reinterpret_cast<uint32_t *>(out + (size_t)r_lo * ldo + (size_t)h * HD + c) = pack_half2(o[d][0] * inv_lo, o[d][1] * inv_lo);
+        if (r_hi < n) *reinterpret_cast<uint32_t *>(out + (size_t)r_hi * ldo + (size_t)h * HD + c) = pack_half2(o[d][2] * inv_hi, o[d][3] * inv_hi);
     }
 }
 
 }  // namespace
 
 cudaError_t launch_attn_prefill(Ctx *ctx, const AttnPrefillArgs &a) {
-    if (a.head_dim != HD || a.n < 1 || a.pos0 < 0 || a.pos0 + a.n > a.max_ctx || a.num_heads % a.num_kv_heads) return cudaErrorInvalidValue;
-    rope_kv_append_kernel<<<a.n, 256, 0, ctx->stream>>>(a);
+    if (a.head_dim != HD || a.num_heads % a.num_kv_heads || a.n_seqs < 1 || a.n_seqs > kMaxPrefillSeqs) return cudaErrorInvalidValue;
+    int rows = 0, blocks = 0;
+    for (int s = 0; s < a.n_seqs; s++) {
+        const AttnPrefillSeq &q = a.seq[s];
+        if (q.row0 != rows || q.n < 1 || q.pos0 < 0 || q.pos0 + q.n > a.max_ctx || !q.k_cache || !q.v_cache) return cudaErrorInvalidValue;
+        rows += q.n;
+        blocks += q_blocks(q);
+    }
+    rope_kv_append_kernel<<<rows, 256, 0, ctx->stream>>>(a);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
-    attn_prefill_kernel<<<dim3((a.n + kQB - 1) / kQB, a.num_heads), 128, 0, ctx->stream>>>(a);
+    attn_prefill_kernel<<<dim3(blocks, a.num_heads), 128, 0, ctx->stream>>>(a);
     return cudaGetLastError();
 }
 

@@ -349,14 +349,12 @@ int tce_attn_prefill(tce_ctx *ctx, void *qkv, void *k_cache, void *v_cache, cons
     CK(cudaSetDevice(ctx->c.device), "cudaSetDevice");
     AttnPrefillArgs a = {};
     a.qkv = (__half *)qkv;
-    a.k_cache = (__half *)k_cache;
-    a.v_cache = (__half *)v_cache;
     a.cos = cosb;
     a.sin = sinb;
     a.out = (__half *)out;
     a.alpha = alpha;
-    a.n = n;
-    a.pos0 = pos0;
+    a.n_seqs = 1;
+    a.seq[0] = AttnPrefillSeq{0, n, pos0, (__half *)k_cache, (__half *)v_cache};
     a.num_heads = num_heads;
     a.num_kv_heads = num_kv_heads;
     a.head_dim = head_dim;
@@ -549,6 +547,19 @@ int tce_llama_decode_batch_host(tce_llama *m, int batch, const int *tokens, cons
     std::string err;
     cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->decode_batch_host(batch, tokens, positions, slots, logits_host, next_tokens, &err);
     return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_decode_batch_host", err);
+}
+int tce_llama_prefill_batch(tce_llama *m, int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, float *logits_host,
+                            int *next_tokens) {
+    if (!m || !tokens_host || !lengths || !pos0s || !slots) return fail(TCE_ERR_INVALID, "tce_llama_prefill_batch: null argument");
+    std::string err;
+    cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->prefill_batch(n_seqs, tokens_host, lengths, pos0s, slots, logits_host, next_tokens, &err);
+    return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_prefill_batch", err);
+}
+int tce_llama_generate_batch(tce_llama *m, int batch, const tce_gen_request *reqs, int *out_tokens_host, int out_stride, int *n_out) {
+    if (!m || !reqs || !n_out) return fail(TCE_ERR_INVALID, "tce_llama_generate_batch: null argument");
+    std::string err;
+    cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->generate_batch(batch, reqs, out_tokens_host, out_stride, n_out, &err);
+    return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_generate_batch", err);
 }
 const float *tce_llama_batch_logits(tce_llama *m) { return m ? reinterpret_cast<LlamaDecoder *>(m)->batch_logits() : nullptr; }
 const float *tce_llama_logits(tce_llama *m) { return m ? reinterpret_cast<LlamaDecoder *>(m)->logits() : nullptr; }

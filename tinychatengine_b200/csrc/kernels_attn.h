@@ -37,15 +37,22 @@ cudaError_t launch_attn_decode_batch(Ctx *ctx, AttnBatchArgs b, int batch, bool 
 // floats of split workspace the batched kernel needs per sequence
 size_t attn_batch_ws_floats(int num_heads, int max_ctx, int chunk);
 
-// prompt processing (sqlen = n > 1): RoPE + KV append for rows pos0..pos0+n-1, causal attention over the cache
-struct AttnPrefillArgs {
-    __half *qkv;         // [n][(H + 2*KVH) * head_dim]; q is rotated in place
+// prompt processing (sqlen = n > 1): RoPE + KV append for rows pos0..pos0+n-1, causal attention over the cache.  Up to
+// kMaxPrefillSeqs prompts in one launch: their rows are concatenated, and each has its own positions and KV cache.
+constexpr int kMaxPrefillSeqs = 8;
+struct AttnPrefillSeq {
+    int row0, n, pos0;   // rows row0..row0+n-1 of qkv / out are positions pos0..pos0+n-1 of this sequence
     __half *k_cache;     // [KVH][max_ctx][head_dim]
     __half *v_cache;
+};
+struct AttnPrefillArgs {
+    __half *qkv;         // [rows][(H + 2*KVH) * head_dim]; q is rotated in place
     const float *cos, *sin;
-    __half *out;         // [n][H * head_dim]
+    __half *out;         // [rows][H * head_dim]
     float alpha;
-    int n, pos0, num_heads, num_kv_heads, head_dim, max_ctx;
+    int num_heads, num_kv_heads, head_dim, max_ctx;
+    int n_seqs;          // 1..kMaxPrefillSeqs; seq[s + 1].row0 == seq[s].row0 + seq[s].n, seq[0].row0 == 0
+    AttnPrefillSeq seq[kMaxPrefillSeqs];
 };
 cudaError_t launch_attn_prefill(Ctx *ctx, const AttnPrefillArgs &a);
 cudaError_t launch_embedding_rows(Ctx *ctx, const __half *table, const int *tokens, float *resid, int n, int E);
@@ -81,11 +88,15 @@ struct SampleArgs {
     int *out_count = nullptr;
     int out_cap = 0;
     int *stop = nullptr;      // set to 1 when eos_id is drawn; a set flag turns the kernel into a no-op
+    int out_limit = 0;        // > 0: also stop once *out_count reaches it
+    int pos_limit = 0;        // > 0: also stop when the next position reaches it; on stopping, tokpos[1] is set to pos_limit
     int *dbg_ids = nullptr;   // optional: surviving candidates (sorted) and their final probabilities
     float *dbg_probs = nullptr;
     int *dbg_size = nullptr;
 };
 cudaError_t launch_sample(Ctx *ctx, const SampleArgs &a, cudaStream_t stream);
+// rows_dev = device SampleArgs[rows]: row b is sampled by block b (the generate loop of the batched step; host-checked arguments)
+cudaError_t launch_sample_rows(const SampleArgs *rows_dev, int rows, cudaStream_t stream);
 // standalone RMSNorm fp16 -> fp16 with fp32 gamma (reference LlamaRMSNorm_cuda, ops/cuda/LlamaRMSNorm.cu:68-115)
 cudaError_t launch_rmsnorm_f16(Ctx *ctx, const __half *x, const float *gamma, __half *y, int rows, int dim, float eps);
 // LayerNormQ::forward (llm/src/ops/LayerNormQ.cc:12-52), bit-exact (serial fp32 sums in the reference's order)

@@ -186,6 +186,8 @@ LlamaDecoder::~LlamaDecoder() {
     cudaFree(d_bnext_);
     cudaFree(d_battn_ws_);
     cudaFree(d_battn_counters_);
+    cudaFree(d_bgen_);
+    cudaFree(d_bsample_);
     if (h_breq_) cudaFreeHost(h_breq_);
     if (h_bnext_) cudaFreeHost(h_bnext_);
     if (h_blogits_) cudaFreeHost(h_blogits_);
@@ -895,14 +897,9 @@ cudaError_t LlamaDecoder::pf_expand_job(int j) {
     return cudaEventRecord(pf_expanded_[b], pf_side_);
 }
 
-cudaError_t LlamaDecoder::prefill(const int *tokens_host, int n, int pos0, float *logits_host, int *next_token, std::string *err, int slot) {
-    if (tp_ > 1) {
-        if (err) *err = "prefill is single-GPU in this build (tensor-parallel ranks process the prompt with decode steps)";
-        return cudaErrorNotSupported;
-    }
-    if (!tokens_host || n < 1 || pos0 < 0 || pos0 + n > cfg_.max_ctx || slot < 0 || slot >= n_slots()) return cudaErrorInvalidValue;
-    for (int i = 0; i < n; i++)
-        if (tokens_host[i] < 0 || tokens_host[i] >= cfg_.vocab_size) return cudaErrorInvalidValue;
+cudaError_t LlamaDecoder::prefill_rows(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots) {
+    int n = 0;
+    for (int i = 0; i < n_seqs; i++) n += lengths[i];
     DCK(prefill_reserve(n));
     if (pf_jobs_.empty()) {
         size_t need = 0;
@@ -935,30 +932,46 @@ cudaError_t LlamaDecoder::prefill(const int *tokens_host, int n, int pos0, float
     const long long Q = (long long)(H + 2 * KVH) * hd;
     DCK(cudaMemcpyAsync(pf_tok_, tokens_host, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
     DCK(launch_embedding_rows(ctx_, (const __half *)w_.embed_f16, pf_tok_, pf_x_, n, E));
+    AttnPrefillArgs a{};
+    a.qkv = pf_qkv_;
+    a.cos = d_cos_;
+    a.sin = d_sin_;
+    a.out = pf_att_;
+    a.alpha = cfg_.qk_alpha > 0 ? cfg_.qk_alpha : 1.0f / sqrtf((float)hd);
+    a.num_heads = H;
+    a.num_kv_heads = KVH;
+    a.head_dim = hd;
+    a.max_ctx = cfg_.max_ctx;
+    a.n_seqs = n_seqs;
+    for (int i = 0, row0 = 0; i < n_seqs; row0 += lengths[i++]) a.seq[i] = AttnPrefillSeq{row0, lengths[i], pos0s[i], nullptr, nullptr};
     for (int l = 0; l < cfg_.num_layers; l++) {
         const tce_llama_layer &L = layers_[l];
         DCK(launch_rmsnorm_rows_f32(ctx_, pf_x_, L.input_norm, pf_xn_, n, E, cfg_.rms_eps));
         DCK(prefill_linear(4 * l, pf_xn_, pf_qkv_, Q, n, EPI_STORE_HALF));
-        AttnPrefillArgs a{};
-        a.qkv = pf_qkv_;
-        a.k_cache = (__half *)kv_cache_slot(slot, l, 0);
-        a.v_cache = (__half *)kv_cache_slot(slot, l, 1);
-        a.cos = d_cos_;
-        a.sin = d_sin_;
-        a.out = pf_att_;
-        a.alpha = cfg_.qk_alpha > 0 ? cfg_.qk_alpha : 1.0f / sqrtf((float)hd);
-        a.n = n;
-        a.pos0 = pos0;
-        a.num_heads = H;
-        a.num_kv_heads = KVH;
-        a.head_dim = hd;
-        a.max_ctx = cfg_.max_ctx;
+        for (int i = 0; i < n_seqs; i++) {
+            a.seq[i].k_cache = (__half *)kv_cache_slot(slots[i], l, 0);
+            a.seq[i].v_cache = (__half *)kv_cache_slot(slots[i], l, 1);
+        }
         DCK(launch_attn_prefill(ctx_, a));
         DCK(prefill_linear(4 * l + 1, pf_att_, pf_x_, E, n, EPI_ADD_F32));  // residual add in the GEMM epilogue
         DCK(launch_rmsnorm_rows_f32(ctx_, pf_x_, L.post_norm, pf_xn_, n, E, cfg_.rms_eps));
         DCK(prefill_linear(4 * l + 2, pf_xn_, pf_act_, F, n, EPI_SILU_MUL_HALF));  // SiLU(gate) * up in the GEMM epilogue: gate|up never reach HBM
         DCK(prefill_linear(4 * l + 3, pf_act_, pf_x_, E, n, EPI_ADD_F32));
     }
+    return cudaSuccess;
+}
+
+cudaError_t LlamaDecoder::prefill(const int *tokens_host, int n, int pos0, float *logits_host, int *next_token, std::string *err, int slot) {
+    if (tp_ > 1) {
+        if (err) *err = "prefill is single-GPU in this build (tensor-parallel ranks process the prompt with decode steps)";
+        return cudaErrorNotSupported;
+    }
+    if (!tokens_host || n < 1 || pos0 < 0 || pos0 + n > cfg_.max_ctx || slot < 0 || slot >= n_slots()) return cudaErrorInvalidValue;
+    for (int i = 0; i < n; i++)
+        if (tokens_host[i] < 0 || tokens_host[i] >= cfg_.vocab_size) return cudaErrorInvalidValue;
+    DCK(prefill_rows(1, tokens_host, &n, &pos0, &slot));
+    cudaStream_t s = ctx_->stream;
+    const int E = cfg_.embed_dim;
     // only the last position feeds the sampler: final RMSNorm + lm_head as the decode step's last GEMV, then arg-max
     DCK(cudaMemcpyAsync(d_resid_, pf_x_ + (size_t)(n - 1) * E, (size_t)E * sizeof(float), cudaMemcpyDeviceToDevice, s));
     const StepOp *lm = nullptr;
@@ -994,6 +1007,10 @@ void LlamaDecoder::drop_batch_graphs() {
             cudaGraphExecDestroy(g_bdev_[b]);
             g_bdev_[b] = nullptr;
         }
+        if (g_bgen_[b]) {
+            cudaGraphExecDestroy(g_bgen_[b]);
+            g_bgen_[b] = nullptr;
+        }
     }
 }
 
@@ -1025,9 +1042,10 @@ cudaError_t LlamaDecoder::batch_alloc(std::string *err) {
     };
     float *resid, *logits, *ws;
     __half *qkv, *attn, *act, **table;
-    int *req, *safe, *next, *hreq, *hnext;
+    int *req, *safe, *next, *hreq, *hnext, *gen;
     unsigned *counters;
     float *hlogits;
+    SampleArgs *sample;
     D((void **)&resid, B * E * sizeof(float));
     D((void **)&qkv, B * Q * sizeof(__half));
     D((void **)&attn, B * A * sizeof(__half));
@@ -1039,6 +1057,8 @@ cudaError_t LlamaDecoder::batch_alloc(std::string *err) {
     D((void **)&ws, ws_floats * sizeof(float));
     D((void **)&counters, n_counters * sizeof(unsigned));
     D((void **)&table, sizeof(__half *));
+    D((void **)&gen, (B * 4 + 2 * B * cfg_.max_ctx) * sizeof(int));
+    D((void **)&sample, B * sizeof(SampleArgs));
     Hst((void **)&hreq, B * 3 * sizeof(int));
     Hst((void **)&hnext, B * sizeof(int));
     Hst((void **)&hlogits, B * V * sizeof(float));
@@ -1066,6 +1086,8 @@ cudaError_t LlamaDecoder::batch_alloc(std::string *err) {
     h_breq_ = hreq;
     h_bnext_ = hnext;
     h_blogits_ = hlogits;
+    d_bgen_ = gen;
+    d_bsample_ = sample;
     d_slot_table_ = table;  // last: a non-null table means every buffer above exists
     return cudaSuccess;
 }
@@ -1283,6 +1305,163 @@ cudaError_t LlamaDecoder::decode_batch_host(int batch, const int *tokens, const 
     DCK(cudaStreamSynchronize(s));
     if (logits_host) memcpy(logits_host, h_blogits_, lbytes);
     if (next_tokens) memcpy(next_tokens, h_bnext_, (size_t)batch * sizeof(int));
+    return cudaSuccess;
+}
+
+// ------------------------------------------------------------------------------------------------ batched prompt pass and generate loop
+cudaError_t LlamaDecoder::prefill_batch(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, float *logits_host,
+                                        int *next_tokens, std::string *err) {
+    if (tp_ > 1) return batch_alloc(err);  // not supported, with its message
+    if (n_seqs < 1 || n_seqs > TCE_LLAMA_MAX_BATCH || !tokens_host || !lengths || !pos0s || !slots) return cudaErrorInvalidValue;
+    int n = 0;
+    for (int b = 0; b < n_seqs; b++) {
+        if (lengths[b] < 1 || pos0s[b] < 0 || pos0s[b] > cfg_.max_ctx - lengths[b] || slots[b] < 0 || slots[b] >= n_slots()) return cudaErrorInvalidValue;
+        for (int o = 0; o < b; o++)
+            if (slots[o] == slots[b]) return cudaErrorInvalidValue;
+        n += lengths[b];
+    }
+    for (int i = 0; i < n; i++)
+        if (tokens_host[i] < 0 || tokens_host[i] >= cfg_.vocab_size) return cudaErrorInvalidValue;
+    DCK(batch_alloc(err));
+    DCK(prefill_rows(n_seqs, tokens_host, lengths, pos0s, slots));
+    cudaStream_t s = ctx_->stream;
+    const int E = cfg_.embed_dim, V = cfg_.vocab_size;
+    // the last row of each prompt becomes row b of the batched step's residual: final RMSNorm + lm_head as that step's GEMV (M = n_seqs)
+    for (int b = 0, row = 0; b < n_seqs; b++) {
+        row += lengths[b];
+        DCK(cudaMemcpyAsync(d_bresid_ + (size_t)b * E, pf_x_ + (size_t)(row - 1) * E, (size_t)E * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    }
+    const StepOp *lm = nullptr;
+    for (const StepOp &op : ops_)
+        if (op.type == OP_GEMV) lm = &op;
+    if (!lm) return cudaErrorUnknown;
+    W4GemvParams p = lm->g;
+    p.M = n_seqs;
+    p.x = d_bresid_;
+    p.ldx = E;
+    p.y = d_blogits_;
+    p.ldy = V;
+    p.pdl = false;
+    DCK(launch_w4a16_gemv(ctx_, p));
+    DCK(launch_argmax_rows(ctx_, d_blogits_, n_seqs, V, d_bnext_, false));
+    if (logits_host) DCK(cudaMemcpyAsync(h_blogits_, d_blogits_, (size_t)n_seqs * V * sizeof(float), cudaMemcpyDeviceToHost, s));
+    DCK(cudaMemcpyAsync(h_bnext_, d_bnext_, (size_t)n_seqs * sizeof(int), cudaMemcpyDeviceToHost, s));
+    DCK(cudaStreamSynchronize(s));
+    if (logits_host) memcpy(logits_host, h_blogits_, (size_t)n_seqs * V * sizeof(float));
+    if (next_tokens) memcpy(next_tokens, h_bnext_, (size_t)n_seqs * sizeof(int));
+    return cudaSuccess;
+}
+
+// The generate loop of `generate` for up to TCE_LLAMA_MAX_BATCH sequences: every token is one batched step on the request buffer d_breq_ and
+// one sampler launch with a block per row, which writes each row's next {token, position} into that buffer.  A row that stops gets an
+// out-of-range position there, so the batched embedding refuses it and it appends no KV row in any later step.  Stopped rows still ride
+// along as rows of the GEMVs.
+cudaError_t LlamaDecoder::generate_batch(int batch, const tce_gen_request *reqs, int *out_tokens_host, int out_stride, int *n_out, std::string *err) {
+    if (tp_ > 1) return batch_alloc(err);  // not supported, with its message
+    if (batch < 1 || batch > TCE_LLAMA_MAX_BATCH || !reqs || !n_out || out_stride < 0) return cudaErrorInvalidValue;
+    const int cap = cfg_.max_ctx, V = cfg_.vocab_size, B = TCE_LLAMA_MAX_BATCH;
+    int n_pred[TCE_LLAMA_MAX_BATCH], steps = 0;
+    for (int b = 0; b < batch; b++) {
+        const tce_gen_request &r = reqs[b];
+        if (r.slot < 0 || r.slot >= n_slots() || r.first_token < 0 || r.first_token >= V || r.pos0 < 0 || r.pos0 >= cap || r.n_predict < 0 ||
+            r.n_history < 0 || r.n_history > cap || (r.n_history > 0 && !r.history))
+            return cudaErrorInvalidValue;
+        for (int o = 0; o < b; o++)
+            if (reqs[o].slot == r.slot) return cudaErrorInvalidValue;
+        n_pred[b] = r.n_predict < cap - r.pos0 ? r.n_predict : cap - r.pos0;
+        if (out_stride < n_pred[b]) return cudaErrorInvalidValue;
+        steps = n_pred[b] > steps ? n_pred[b] : steps;
+    }
+    if (steps > 0 && !out_tokens_host) return cudaErrorInvalidValue;
+    for (int b = 0; b < batch; b++) {
+        const tce_sampling &sc = reqs[b].sampling;
+        if (sc.temp > 0.f && (sc.top_k <= 0 || sc.top_k > 1024) && V > 1024) {
+            if (err) *err = "generate: temp > 0 needs 1 <= top_k <= 1024";
+            return cudaErrorNotSupported;
+        }
+    }
+    DCK(batch_alloc(err));
+    cudaStream_t s = ctx_->stream;
+    int *ctl = d_bgen_, *hist = d_bgen_ + 4 * B, *out_list = hist + (size_t)B * cap;  // per row: {history head, output count, stop flag, unused}
+    int ctl_h[4 * TCE_LLAMA_MAX_BATCH] = {};
+    SampleArgs args[TCE_LLAMA_MAX_BATCH];
+    for (int b = 0; b < batch; b++) {
+        const tce_gen_request &r = reqs[b];
+        if (r.n_history > 0)
+            DCK(cudaMemcpyAsync(hist + (size_t)b * cap, r.history, (size_t)r.n_history * sizeof(int), cudaMemcpyHostToDevice, s));
+        ctl_h[4 * b] = r.n_history;
+        ctl_h[4 * b + 2] = n_pred[b] == 0;  // nothing to generate: stopped from the start
+        h_breq_[3 * b] = r.first_token;
+        h_breq_[3 * b + 1] = n_pred[b] == 0 ? cap : r.pos0;
+        h_breq_[3 * b + 2] = r.slot;
+        SampleArgs &a = args[b];
+        a = SampleArgs{};
+        a.logits = d_blogits_ + (size_t)b * V;
+        a.n_vocab = V;
+        a.top_k = r.sampling.top_k;
+        a.top_p = r.sampling.top_p;
+        a.temp = r.sampling.temp;
+        a.repeat_penalty = r.sampling.repeat_penalty;
+        a.frequency_penalty = r.sampling.frequency_penalty;
+        a.presence_penalty = r.sampling.presence_penalty;
+        a.repeat_last_n = r.sampling.repeat_last_n;
+        a.seed = r.sampling.seed;
+        a.draw_index = 0;
+        a.hist = hist + (size_t)b * cap;
+        a.hist_head = ctl + 4 * b;
+        a.hist_cap = cap;
+        a.eos_id = r.eos_id;
+        a.tokpos = d_breq_ + 3 * b;
+        a.out_list = out_list + (size_t)b * cap;
+        a.out_count = ctl + 4 * b + 1;
+        a.out_cap = cap;
+        a.stop = ctl + 4 * b + 2;
+        a.out_limit = n_pred[b];
+        a.pos_limit = cap;
+    }
+    DCK(cudaMemcpyAsync(ctl, ctl_h, (size_t)4 * batch * sizeof(int), cudaMemcpyHostToDevice, s));
+    DCK(cudaMemcpyAsync(d_bsample_, args, (size_t)batch * sizeof(SampleArgs), cudaMemcpyHostToDevice, s));
+    DCK(cudaMemcpyAsync(d_breq_, h_breq_, (size_t)batch * 3 * sizeof(int), cudaMemcpyHostToDevice, s));
+    auto body = [&](cudaStream_t st, bool pdl) {
+        cudaError_t e = enqueue_batch(batch, d_breq_, st, pdl);
+        if (e == cudaSuccess) e = launch_sample_rows(d_bsample_, batch, st);
+        return e;
+    };
+    cudaGraphExec_t &g = g_bgen_[batch];
+    if (g && g_bgen_gen_[batch] != ctx_->option_gen) {  // an option or the stream changed since capture
+        cudaGraphExecDestroy(g);
+        g = nullptr;
+    }
+    constexpr int kCheckEvery = 16;
+    for (int i = 0; i < steps; i++) {
+        if (use_graphs_ && !g && i > 0) {
+            // captured after one eager token (modules loaded, kernel attributes set, GEMV fix-up records grown); capture runs nothing
+            cudaError_t e = capture_graph(cap_stream_, ctx_->use_pdl, [&](bool pdl) { return body(cap_stream_, pdl); }, &g);
+            if (e != cudaSuccess) {
+                if (err) *err = std::string("batched generate graph capture failed: ") + cudaGetErrorString(e);
+                return e;
+            }
+            g_bgen_gen_[batch] = ctx_->option_gen;
+        }
+        if (use_graphs_ && g)
+            DCK(cudaGraphLaunch(g, s));
+        else
+            DCK(body(s, ctx_->use_pdl));
+        if ((i + 1) % kCheckEvery == 0 && i + 1 < steps) {
+            DCK(cudaMemcpyAsync(ctl_h, ctl, (size_t)4 * batch * sizeof(int), cudaMemcpyDeviceToHost, s));
+            DCK(cudaStreamSynchronize(s));
+            bool all = true;
+            for (int b = 0; b < batch; b++) all = all && ctl_h[4 * b + 2];
+            if (all) break;
+        }
+    }
+    DCK(cudaMemcpyAsync(ctl_h, ctl, (size_t)4 * batch * sizeof(int), cudaMemcpyDeviceToHost, s));
+    DCK(cudaStreamSynchronize(s));
+    for (int b = 0; b < batch; b++) {
+        const int n = ctl_h[4 * b + 1] < n_pred[b] ? ctl_h[4 * b + 1] : n_pred[b];
+        if (n > 0) DCK(cudaMemcpy(out_tokens_host + (size_t)b * out_stride, out_list + (size_t)b * cap, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
+        n_out[b] = n;
+    }
     return cudaSuccess;
 }
 

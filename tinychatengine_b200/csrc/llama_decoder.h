@@ -21,6 +21,9 @@ class LlamaDecoder {
                          int *out_tokens_host, int *n_out, std::string *err);
     // prompt processing: n tokens at positions pos0..pos0+n-1 in one pass (tensor-core GEMMs + causal flash attention)
     cudaError_t prefill(const int *tokens_host, int n, int pos0, float *logits_host, int *next_token, std::string *err, int slot = 0);
+    // n_seqs prompts (concatenated in tokens_host) into their own slots in one pass over the weights; logits / greedy token of each last row
+    cudaError_t prefill_batch(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, float *logits_host,
+                              int *next_tokens, std::string *err);
     const float *logits() const { return d_logits_; }
     void *kv_cache(int layer, int which) const { return kv_cache_slot(0, layer, which); }
     // batched decode: up to TCE_LLAMA_MAX_BATCH sequences per step, each in its own KV-cache slot (slot 0 = d_kv_)
@@ -32,6 +35,8 @@ class LlamaDecoder {
     cudaError_t decode_batch_host(int batch, const int *tokens, const int *positions, const int *slots, float *logits_host, int *next_tokens,
                                   std::string *err);
     const float *batch_logits();
+    // generate loop of up to TCE_LLAMA_MAX_BATCH sequences: one batched step + one sampler launch (a block per row) per token
+    cudaError_t generate_batch(int batch, const tce_gen_request *reqs, int *out_tokens_host, int out_stride, int *n_out, std::string *err);
     int kernels_per_step() const { return kernels_per_step_; }
     void *debug_buffer(int which) const {
         switch (which) {
@@ -52,6 +57,8 @@ class LlamaDecoder {
     LlamaDecoder() = default;
     cudaError_t prefill_reserve(int n);
     cudaError_t prefill_linear(int j, const __half *x, void *C, long long ldc, int n, EpiMode epi);
+    // the prompt pass over n_seqs concatenated prompts (host-checked arguments); leaves the final residual rows in pf_x_
+    cudaError_t prefill_rows(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots);
     cudaError_t enqueue_step(const int *tokpos, cudaStream_t s, bool pdl, bool gemv_only = false);  // raw kernel sequence
     cudaError_t build_graphs(std::string *err);
     void build_ops();
@@ -146,12 +153,18 @@ class LlamaDecoder {
     size_t battn_counters_ = 0;
     int *h_breq_ = nullptr, *h_bnext_ = nullptr;
     float *h_blogits_ = nullptr;
+    // batched generate loop: [8][4] control words {history head, output count, stop flag, unused}, then [8][max_ctx] history rings and
+    // [8][max_ctx] output lists; the sampler arguments of each row
+    int *d_bgen_ = nullptr;
+    SampleArgs *d_bsample_ = nullptr;
     // one graph per batch size: host entry (with / without the logits copy) and device entry (for one request pointer)
     cudaGraphExec_t g_bhost_[2][TCE_LLAMA_MAX_BATCH + 1] = {};
     unsigned g_bhost_gen_[2][TCE_LLAMA_MAX_BATCH + 1] = {};
     cudaGraphExec_t g_bdev_[TCE_LLAMA_MAX_BATCH + 1] = {};
     const int *g_bdev_src_[TCE_LLAMA_MAX_BATCH + 1] = {};
     unsigned g_bdev_gen_[TCE_LLAMA_MAX_BATCH + 1] = {};
+    cudaGraphExec_t g_bgen_[TCE_LLAMA_MAX_BATCH + 1] = {};  // generate loop: one batched step on d_breq_ + the row sampler
+    unsigned g_bgen_gen_[TCE_LLAMA_MAX_BATCH + 1] = {};
     bool use_graphs_ = true;
     bool atomic_residual_ = true;  // o_proj/down_proj partial tiles use RED.ADD (TCE_DETERMINISTIC=1 turns it off)
     int kernels_per_step_ = 0;

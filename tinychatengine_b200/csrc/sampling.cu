@@ -63,8 +63,8 @@ TCE_DEVINL unsigned block_flag_scan(bool flag, unsigned *warp_tot, unsigned &tot
     return before + __popc(bal & ((1u << lane) - 1u));
 }
 
-__global__ void __launch_bounds__(kSampleThreads, 1) sample_kernel(SampleArgs a) {
-    __shared__ SampleShared sh;
+// the whole chain for one sequence, on one kSampleThreads-thread block
+TCE_DEVINL void sample_one(const SampleArgs &a, SampleShared &sh) {
     const int tid = threadIdx.x;
     if (a.stop && *a.stop) return;  // the sequence has ended (EOS drawn earlier): leave every buffer as it is
     float *logits = a.logits;
@@ -264,7 +264,15 @@ __global__ void __launch_bounds__(kSampleThreads, 1) sample_kernel(SampleArgs a)
             if (n < a.out_cap) a.out_list[n] = result;
             *a.out_count = n + 1;
         }
-        if (a.stop && result == a.eos_id) *a.stop = 1;
+        // stop at eos_id, at out_limit outputs, or when the next position would be pos_limit; a stopped batched row's request gets an
+        // out-of-range position, so the batched step appends nothing more for it
+        bool done = result == a.eos_id;
+        if (a.out_limit > 0 && a.out_count && *a.out_count >= a.out_limit) done = true;
+        if (a.pos_limit > 0 && a.tokpos && a.tokpos[1] >= a.pos_limit) done = true;
+        if (a.stop && done) {
+            *a.stop = 1;
+            if (a.pos_limit > 0 && a.tokpos) a.tokpos[1] = a.pos_limit;
+        }
     }
     __syncthreads();
     // optional: the candidate set and its final probabilities (tests)
@@ -278,7 +286,24 @@ __global__ void __launch_bounds__(kSampleThreads, 1) sample_kernel(SampleArgs a)
     }
 }
 
+__global__ void __launch_bounds__(kSampleThreads, 1) sample_kernel(SampleArgs a) {
+    __shared__ SampleShared sh;
+    sample_one(a, sh);
+}
+
+// one block per row of a batch, each with its own arguments (logits row, history ring, output list, control words, request triple)
+__global__ void __launch_bounds__(kSampleThreads, 1) sample_rows_kernel(const SampleArgs *__restrict__ rows) {
+    __shared__ SampleShared sh;
+    sample_one(rows[blockIdx.x], sh);
+}
+
 }  // namespace
+
+cudaError_t launch_sample_rows(const SampleArgs *rows_dev, int rows, cudaStream_t stream) {
+    if (!rows_dev || rows < 1) return cudaErrorInvalidValue;
+    sample_rows_kernel<<<rows, kSampleThreads, 0, stream>>>(rows_dev);
+    return cudaGetLastError();
+}
 
 cudaError_t launch_sample(Ctx *ctx, const SampleArgs &a, cudaStream_t stream) {
     if (!a.logits || a.n_vocab < 1) return cudaErrorInvalidValue;

@@ -328,6 +328,46 @@ class LlamaModel:
         _lib.check(self.ctx.L.tce_llama_decode_batch_host(self.h, n, arr(tokens), arr(positions), arr(slots), p, nxt), "tce_llama_decode_batch_host")
         return list(nxt[:n])
 
+    def prefill_batch(self, prompts, slots, pos0s=None, logits_host=None) -> list[int]:
+        """Prompt processing of up to MAX_BATCH prompts (lists of host ints) in one pass over the weights, prompt s into KV-cache slot
+        slots[s] at positions pos0s[s].. (default 0); fills logits_host (float32 [n_prompts, vocab], may be None) with the logits of each
+        prompt's last position and returns the greedy next tokens."""
+        n = len(prompts)
+        pos0s = [0] * n if pos0s is None else list(pos0s)
+        flat = [int(t) for p in prompts for t in p]
+        arr = lambda v: (C.c_int * max(1, len(v)))(*[int(x) for x in v])
+        nxt = (C.c_int * max(1, n))()
+        p = None if logits_host is None else C.c_void_p(logits_host.data_ptr())
+        _lib.check(self.ctx.L.tce_llama_prefill_batch(self.h, n, arr(flat), arr([len(q) for q in prompts]), arr(pos0s), arr(slots), p, nxt),
+                   "tce_llama_prefill_batch")
+        return list(nxt[:n])
+
+    def generate_batch(self, requests) -> list[list[int]]:
+        """Device generate loop of up to MAX_BATCH sequences (one batched step + one sampler launch per token, only the ids come back).
+        Each request is a dict with first_token, pos0, slot, n_predict and optional history, eos_id and the sampling fields of generate(),
+        with the same defaults (the reference's opt_params)."""
+        defaults = dict(history=(), eos_id=-1, top_k=40, top_p=0.95, temp=0.8, repeat_penalty=1.1, frequency_penalty=0.0, presence_penalty=0.0,
+                        repeat_last_n=64, seed=0)
+        n = len(requests)
+        reqs = (_lib.GenRequest * max(1, n))()
+        keep = []
+        for i, r in enumerate(requests):
+            unknown = set(r) - set(defaults) - {"first_token", "pos0", "slot", "n_predict"}
+            if unknown:
+                raise TypeError(f"generate_batch: unknown request fields {sorted(unknown)}")
+            q = {**defaults, **r}
+            hist = (C.c_int * max(1, len(q["history"])))(*[int(t) for t in q["history"]])
+            keep.append(hist)
+            reqs[i] = _lib.GenRequest(int(q["first_token"]), int(q["pos0"]), int(q["slot"]), int(q["n_predict"]), int(q["eos_id"]),
+                                      C.cast(hist, C.POINTER(C.c_int)) if len(q["history"]) else None, len(q["history"]),
+                                      _lib.Sampling(int(q["top_k"]), float(q["top_p"]), float(q["temp"]), float(q["repeat_penalty"]),
+                                                    float(q["frequency_penalty"]), float(q["presence_penalty"]), int(q["repeat_last_n"]), int(q["seed"])))
+        stride = max([1] + [max(0, int(r["n_predict"])) for r in requests])
+        out = (C.c_int * (max(1, n) * stride))()
+        n_out = (C.c_int * max(1, n))()
+        _lib.check(self.ctx.L.tce_llama_generate_batch(self.h, n, reqs, out, stride, n_out), "tce_llama_generate_batch")
+        return [list(out[i * stride:i * stride + n_out[i]]) for i in range(n)]
+
     def batch_logits(self) -> torch.Tensor:
         """View of the device logits of the batched step (float32 [MAX_BATCH, vocab])."""
         ptr = self.ctx.L.tce_llama_batch_logits(self.h)
