@@ -235,6 +235,18 @@ TCE_API const float *tce_llama_batch_logits(tce_llama *m);    /* device float[TC
  * >= the reserved count or named twice, or a token outside [0, vocab).  Synchronous.                                                   */
 TCE_API int tce_llama_prefill_batch(tce_llama *m, int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots,
                                     float *logits_host, int *next_tokens);
+/* Teacher-forced scoring: the prompt pass of tce_llama_prefill_batch (same prompts, slots, positions, checks, and the same KV rows written),
+ * plus the lm_head over EVERY row.  n = sum of lengths.  targets_host int[n]: the token whose log-probability row i reports, -1 for none;
+ * NULL = the next token of the same prompt, and -1 on each prompt's last row.  Outputs, each may be NULL:
+ *   logprobs_host float[n]  log_softmax(logits_i)[target_i], NaN where the target is -1
+ *   greedy_host int[n]      arg-max of logits_i (lowest id on ties)
+ *   greedy_logprobs_host float[n]
+ *   logits_dev              device float[n][vocab] receiving every row's logits (the reference's logits[1][sqlen][vocab]); NULL = none are stored
+ * The logits come from the fp16-expanded lm_head on the tensor cores (not the decode GEMV), and each row's results are bit-identical
+ * whatever other prompts share the call.  TCE_ERR_INVALID, before anything is enqueued, for everything tce_llama_prefill_batch refuses
+ * and for a target outside [-1, vocab); TCE_ERR_UNSUPPORTED with tp_size > 1.  Synchronous.                                             */
+TCE_API int tce_llama_score_batch(tce_llama *m, int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots,
+                                  const int *targets_host, float *logprobs_host, int *greedy_host, float *greedy_logprobs_host, float *logits_dev);
 typedef struct tce_gen_request {
     int first_token, pos0, slot;   /* decode first_token at pos0 in slot, as tce_llama_generate does for slot 0 */
     int n_predict, eos_id;         /* per-sequence budget and stop id (-1: none) */

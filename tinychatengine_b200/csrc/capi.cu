@@ -555,6 +555,14 @@ int tce_llama_prefill_batch(tce_llama *m, int n_seqs, const int *tokens_host, co
     cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->prefill_batch(n_seqs, tokens_host, lengths, pos0s, slots, logits_host, next_tokens, &err);
     return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_prefill_batch", err);
 }
+int tce_llama_score_batch(tce_llama *m, int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, const int *targets_host,
+                          float *logprobs_host, int *greedy_host, float *greedy_logprobs_host, float *logits_dev) {
+    if (!m || !tokens_host || !lengths || !pos0s || !slots) return fail(TCE_ERR_INVALID, "tce_llama_score_batch: null argument");
+    std::string err;
+    cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->score_batch(n_seqs, tokens_host, lengths, pos0s, slots, targets_host, logprobs_host, greedy_host,
+                                                                     greedy_logprobs_host, logits_dev, &err);
+    return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_score_batch", err);
+}
 int tce_llama_generate_batch(tce_llama *m, int batch, const tce_gen_request *reqs, int *out_tokens_host, int out_stride, int *n_out) {
     if (!m || !reqs || !n_out) return fail(TCE_ERR_INVALID, "tce_llama_generate_batch: null argument");
     std::string err;

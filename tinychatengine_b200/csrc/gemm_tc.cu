@@ -17,7 +17,7 @@ using tc::GemmArgs;
 // ------------------------------------------------------------------------------------------------ epilogues
 template <int VARIANT>
 struct EpiW8 {  // int32 accumulator -> the four W8A8 epilogues (same float op order as w8a8.cu / kernels/ref)
-    static constexpr bool kSilu = false;
+    static constexpr bool kSilu = false, kRowStats = false;
     TCE_DEVINL static void apply(const GemmArgs &a, int row, int col, int v0, int v1) {
         const size_t o = (size_t)row * a.ldc + col;
         const int v[2] = {v0, v1};

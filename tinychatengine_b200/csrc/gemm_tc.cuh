@@ -43,6 +43,13 @@ struct GemmArgs {
     const float *biasf;
     float alpha, beta;
     int q_min, q_max;
+    // Epi::kRowStats (lm_head scoring, gemm_tc2.cu): per-row log-softmax statistics of every 128 columns, the target logits, and C (may
+    // be null) receiving the fp32 logits
+    LmStat *stats;                // [M][stats_ld]: record of columns 128r .. 128r + 127 at [row][r]
+    int stats_ld;
+    int col0;                     // vocabulary id of column 0
+    const int *target;            // [M] vocabulary id of each row's target, -1 for none
+    float *tgt;                   // [M] receives the target's logit
 };
 
 TCE_DEVINL void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -132,7 +139,8 @@ inline int pick_block_n(long long row_blocks, int N, int ctas) {
 }
 
 // Epilogues see the wgmma fragment two columns at a time: Epi::apply(args, row, col, v0, v1) owns C[row][col], C[row][col + 1] (col even,
-// col < N).  Epi::kSilu: apply(args, row, col, g0, g1, u0, u1) with the gate / up accumulators of channels col, col + 1.
+// col < N).  Epi::kSilu: apply(args, row, col, g0, g1, u0, u1) with the gate / up accumulators of channels col, col + 1.  Epi::kRowStats:
+// half(args, acc, row0, c0, cq) sees a whole 128-column half of the fragment (columns c0 + 8i + cq + {0, 1} of rows row0 and row0 + 8).
 template <int BLOCK_N, int STAGES, bool I8, int CL, class Epi>
 __global__ void __launch_bounds__(kThreads, 1) gemm_wg_kernel(const __grid_constant__ GemmArgs a) {
     static_assert(BLOCK_N == 128 || BLOCK_N == 256, "BLOCK_N");
@@ -197,7 +205,10 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wg_kernel(const __grid_const
             // fragment: thread (warp w, lane l) holds rows 16w + l/4 (+8), n-tile i: columns 8i + 2(l%4) + {0,1}
             const int row0 = mb * kBlockM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
             const int cq = 2 * (lane & 3);
-            if constexpr (Epi::kSilu) {
+            if constexpr (Epi::kRowStats) {
+#pragma unroll
+                for (int h = 0; h < NH; h++) Epi::half(a, acc[h], row0, nb * BLOCK_N + h * 128, cq);
+            } else if constexpr (Epi::kSilu) {
 #pragma unroll
                 for (int i = 0; i < 16; i++) {
                     const int col = nb * 128 + 8 * i + cq;
@@ -315,7 +326,7 @@ cudaError_t launch_wg(Ctx *ctx, GemmArgs &a) {
 
 // ------------------------------------------------------------------------------------------------ epilogues of the fp16 GEMM (gemm_tc2.cu)
 struct EpiHalf {  // fp32 accumulator -> fp16 C
-    static constexpr bool kSilu = false;
+    static constexpr bool kSilu = false, kRowStats = false;
     TCE_DEVINL static void apply(const GemmArgs &a, int row, int col, float v0, float v1) {
         __half *dst = reinterpret_cast<__half *>(a.C) + (size_t)row * a.ldc + col;
         if (col + 1 < a.N && (a.ldc & 1) == 0) {
@@ -328,7 +339,7 @@ struct EpiHalf {  // fp32 accumulator -> fp16 C
 };
 
 struct EpiAddF32 {  // fp32 accumulator added into an fp32 C (residual stream)
-    static constexpr bool kSilu = false;
+    static constexpr bool kSilu = false, kRowStats = false;
     TCE_DEVINL static void apply(const GemmArgs &a, int row, int col, float v0, float v1) {
         float *dst = reinterpret_cast<float *>(a.C) + (size_t)row * a.ldc + col;
         if (col + 1 < a.N && (a.ldc & 1) == 0) {

@@ -122,6 +122,21 @@ cudaError_t launch_gemm_f16_pair(Ctx *ctx, const __half *X, long long ldx, const
 cudaError_t launch_gemm_f16_pair_silu(Ctx *ctx, const __half *X, long long ldx, const __half *W, long long ldw, __half *act, long long ldc, int M, int F, int K);
 cudaError_t w4_scratch_reserve(Ctx *ctx, size_t elems);  // grows ctx->w16_scratch (may synchronise the device)
 
+// lm_head scoring: log-softmax statistics of 128 logits of one row (m = max, s = sum of exp(x - m), id = lowest vocabulary id of the max)
+struct alignas(16) LmStat {
+    float m, s;
+    int id, unused;
+};
+// the lm_head GEMM of one vocabulary chunk (W = its fp16 rows [N][K], vocabulary ids col0 .. col0 + N - 1) with the log-softmax epilogue:
+// stats[row][c / 128] for every 128 columns, tgt[row] = the logit of target[row] when the target falls in this chunk, and, when logits is
+// not null, logits[row * ld_logits + col0 + c] = every logit.  The [M][N] logits never reach HBM otherwise.
+cudaError_t launch_gemm_f16_pair_stats(Ctx *ctx, const __half *X, long long ldx, const __half *W, long long ldw, int M, int N, int K, int col0, LmStat *stats,
+                                       int stats_ld, const int *target, float *tgt, float *logits, long long ld_logits);
+// folds the n_rec records of each row (in column order) into the running state[row]; with `last`, also writes logprob[row] =
+// tgt[row] - logsumexp (NaN where target[row] < 0), greedy[row] and greedy_logprob[row]
+cudaError_t launch_lm_stats_merge(Ctx *ctx, const LmStat *stats, int stats_ld, int n_rec, int rows, bool first, bool last, LmStat *state, const int *target,
+                                  const float *tgt, float *logprob, int *greedy, float *greedy_logprob);
+
 // host-side mirror of the stream-K partition used by the kernel (unit-tested on the CPU)
 struct StreamK {
     long long U;   // total units = tiles * groups

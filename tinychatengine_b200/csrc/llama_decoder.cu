@@ -162,6 +162,11 @@ LlamaDecoder::~LlamaDecoder() {
     cudaFree(pf_att_);
     cudaFree(pf_act_);
     cudaFree(pf_tok_);
+    cudaFree(sc_rec_);
+    cudaFree(sc_state_);
+    cudaFree(sc_target_);
+    cudaFree(sc_tgt_);
+    cudaFree(sc_out_);
     for (void *p : pk_allocs_) cudaFree(p);
     for (int p = 0; p < tp_; p++)
         if (p != cfg_.tp_rank && tp_peer_[p]) cudaIpcCloseMemHandle(tp_peer_[p]);
@@ -867,17 +872,23 @@ cudaError_t LlamaDecoder::prefill_reserve(int n) {
 // (job = gate|up, C = SiLU(gate) * up)
 cudaError_t LlamaDecoder::prefill_linear(int j, const __half *x, void *C, long long ldc, int n, EpiMode epi) {
     const PfJob &job = pf_jobs_[j];
-    const int ic = job.ts[0]->ic, b = j & 1;
+    const int ic = job.ts[0]->ic;
     size_t rows = 0;
-    for (int i = 0; i < job.count; i++) rows += (size_t)job.ts[i]->oc;
-    // queue the next job's expansion, then run this one
-    if (j + 1 < (int)pf_jobs_.size()) DCK(pf_expand_job(j + 1));
-    DCK(cudaStreamWaitEvent(ctx_->stream, pf_expanded_[b], 0));
+    for (int i = 0; i < job.count; i++) rows += (size_t)job.rows[i];
+    const __half *w16 = nullptr;
+    DCK(pf_job_begin(j, &w16));
     if (epi == EPI_SILU_MUL_HALF)
-        DCK(launch_gemm_f16_pair_silu(ctx_, x, ic, pf_w16_[b], ic, (__half *)C, ldc, n, (int)(rows / 2), ic));
+        DCK(launch_gemm_f16_pair_silu(ctx_, x, ic, w16, ic, (__half *)C, ldc, n, (int)(rows / 2), ic));
     else
-        DCK(launch_gemm_f16_pair(ctx_, x, ic, pf_w16_[b], ic, C, ldc, n, (int)rows, ic, epi == EPI_ADD_F32 ? 1 : 0));
-    return cudaEventRecord(pf_consumed_[b], ctx_->stream);
+        DCK(launch_gemm_f16_pair(ctx_, x, ic, w16, ic, C, ldc, n, (int)rows, ic, epi == EPI_ADD_F32 ? 1 : 0));
+    return cudaEventRecord(pf_consumed_[j & 1], ctx_->stream);
+}
+
+cudaError_t LlamaDecoder::pf_job_begin(int j, const __half **w16) {
+    if (j + 1 < pf_njobs_) DCK(pf_expand_job(j + 1));
+    DCK(cudaStreamWaitEvent(ctx_->stream, pf_expanded_[j & 1], 0));
+    *w16 = pf_w16_[j & 1];
+    return cudaSuccess;
 }
 
 // expansion of job j into scratch half (j & 1) on the side stream, after the GEMM that last read that half
@@ -888,41 +899,63 @@ cudaError_t LlamaDecoder::pf_expand_job(int j) {
     side.stream = pf_side_;
     if (j >= 2) DCK(cudaStreamWaitEvent(pf_side_, pf_consumed_[b], 0));
     size_t r0 = 0;
-    const int ic = job.ts[0]->ic;
+    const int ic = job.ts[0]->ic, zw = zeros_width(ic, kW4Group);
     for (int i = 0; i < job.count; i++) {
         const tce_w4_tensor &t = *job.ts[i];
-        DCK(launch_w4_expand(&side, (const uint32_t *)t.w, (const uint32_t *)t.zeros, (const __half *)t.scales, pf_w16_[b] + r0 * ic, t.oc, ic));
-        r0 += (size_t)t.oc;
+        const size_t r = (size_t)job.r0[i];  // first row of the range: offset pointers into the packed words, zeros and scales
+        DCK(launch_w4_expand(&side, (const uint32_t *)t.w + r * (ic / 8), (const uint32_t *)t.zeros + r * zw, (const __half *)t.scales + r * zw * 8,
+                             pf_w16_[b] + r0 * ic, job.rows[i], ic));
+        r0 += (size_t)job.rows[i];
     }
     return cudaEventRecord(pf_expanded_[b], pf_side_);
 }
 
-cudaError_t LlamaDecoder::prefill_rows(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots) {
+// the job list, the double-buffered scratch, its events and the side stream, on first use
+cudaError_t LlamaDecoder::pf_setup() {
+    if (!pf_jobs_.empty()) return cudaSuccess;
+    auto job = [](const tce_w4_tensor *a, const tce_w4_tensor *b, const tce_w4_tensor *c) {
+        PfJob j{{a, b, c}, c ? 3 : (b ? 2 : 1), {0, 0, 0}, {0, 0, 0}};
+        for (int i = 0; i < j.count; i++) j.rows[i] = j.ts[i]->oc;
+        return j;
+    };
+    for (int l = 0; l < cfg_.num_layers; l++) {
+        const tce_llama_layer &L = layers_[l];
+        pf_jobs_.push_back(job(&L.q, &L.k, &L.v));
+        pf_jobs_.push_back(job(&L.o, nullptr, nullptr));
+        pf_jobs_.push_back(job(&L.gate, &L.up, nullptr));
+        pf_jobs_.push_back(job(&L.down, nullptr, nullptr));
+    }
+    size_t need = 0;
+    for (const PfJob &jb : pf_jobs_) {
+        size_t e = 0;
+        for (int i = 0; i < jb.count; i++) e += (size_t)jb.ts[i]->oc * jb.ts[i]->ic;
+        need = e > need ? e : need;
+    }
+    // the lm_head does not fit a half at real vocabularies (Llama-3-8B: 1.05 GB of fp16 against 235 MB): it is expanded in chunks of whole
+    // 256-row blocks (the CTA-pair GEMM's weight tile) that do; q|k|v alone is >= 384 rows of E, so a chunk is at least one block
+    const int E = cfg_.embed_dim, V = cfg_.vocab_size;
+    pf_lm_chunk_ = (int)(need / (size_t)E / 256 * 256);
+    for (int r0 = 0; r0 < V; r0 += pf_lm_chunk_) {
+        PfJob j = job(&w_.lm_head, nullptr, nullptr);
+        j.r0[0] = r0;
+        j.rows[0] = V - r0 < pf_lm_chunk_ ? V - r0 : pf_lm_chunk_;
+        pf_jobs_.push_back(j);
+    }
+    for (int b = 0; b < 2; b++) {
+        DCK(cudaMalloc((void **)&pf_w16_[b], need * sizeof(__half)));
+        DCK(cudaEventCreateWithFlags(&pf_expanded_[b], cudaEventDisableTiming));
+        DCK(cudaEventCreateWithFlags(&pf_consumed_[b], cudaEventDisableTiming));
+    }
+    pf_w16_elems_ = need;
+    return cudaStreamCreateWithFlags(&pf_side_, cudaStreamNonBlocking);
+}
+
+cudaError_t LlamaDecoder::prefill_rows(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, bool score) {
     int n = 0;
     for (int i = 0; i < n_seqs; i++) n += lengths[i];
     DCK(prefill_reserve(n));
-    if (pf_jobs_.empty()) {
-        size_t need = 0;
-        for (int l = 0; l < cfg_.num_layers; l++) {
-            const tce_llama_layer &L = layers_[l];
-            pf_jobs_.push_back(PfJob{{&L.q, &L.k, &L.v}, 3});
-            pf_jobs_.push_back(PfJob{{&L.o, nullptr, nullptr}, 1});
-            pf_jobs_.push_back(PfJob{{&L.gate, &L.up, nullptr}, 2});
-            pf_jobs_.push_back(PfJob{{&L.down, nullptr, nullptr}, 1});
-        }
-        for (const PfJob &jb : pf_jobs_) {
-            size_t e = 0;
-            for (int i = 0; i < jb.count; i++) e += (size_t)jb.ts[i]->oc * jb.ts[i]->ic;
-            need = e > need ? e : need;
-        }
-        for (int b = 0; b < 2; b++) {
-            DCK(cudaMalloc((void **)&pf_w16_[b], need * sizeof(__half)));
-            DCK(cudaEventCreateWithFlags(&pf_expanded_[b], cudaEventDisableTiming));
-            DCK(cudaEventCreateWithFlags(&pf_consumed_[b], cudaEventDisableTiming));
-        }
-        pf_w16_elems_ = need;
-        DCK(cudaStreamCreateWithFlags(&pf_side_, cudaStreamNonBlocking));
-    }
+    DCK(pf_setup());
+    pf_njobs_ = score ? (int)pf_jobs_.size() : 4 * cfg_.num_layers;
     // the side stream starts after everything already queued on the main stream (a previous prompt's GEMMs read the scratch)
     DCK(cudaEventRecord(pf_consumed_[0], ctx_->stream));
     DCK(cudaStreamWaitEvent(pf_side_, pf_consumed_[0], 0));
@@ -1309,19 +1342,26 @@ cudaError_t LlamaDecoder::decode_batch_host(int batch, const int *tokens, const 
 }
 
 // ------------------------------------------------------------------------------------------------ batched prompt pass and generate loop
-cudaError_t LlamaDecoder::prefill_batch(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, float *logits_host,
-                                        int *next_tokens, std::string *err) {
-    if (tp_ > 1) return batch_alloc(err);  // not supported, with its message
+cudaError_t LlamaDecoder::check_prompts(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, int *n) const {
     if (n_seqs < 1 || n_seqs > TCE_LLAMA_MAX_BATCH || !tokens_host || !lengths || !pos0s || !slots) return cudaErrorInvalidValue;
-    int n = 0;
+    int rows = 0;
     for (int b = 0; b < n_seqs; b++) {
         if (lengths[b] < 1 || pos0s[b] < 0 || pos0s[b] > cfg_.max_ctx - lengths[b] || slots[b] < 0 || slots[b] >= n_slots()) return cudaErrorInvalidValue;
         for (int o = 0; o < b; o++)
             if (slots[o] == slots[b]) return cudaErrorInvalidValue;
-        n += lengths[b];
+        rows += lengths[b];
     }
-    for (int i = 0; i < n; i++)
+    for (int i = 0; i < rows; i++)
         if (tokens_host[i] < 0 || tokens_host[i] >= cfg_.vocab_size) return cudaErrorInvalidValue;
+    *n = rows;
+    return cudaSuccess;
+}
+
+cudaError_t LlamaDecoder::prefill_batch(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, float *logits_host,
+                                        int *next_tokens, std::string *err) {
+    if (tp_ > 1) return batch_alloc(err);  // not supported, with its message
+    int n = 0;
+    DCK(check_prompts(n_seqs, tokens_host, lengths, pos0s, slots, &n));
     DCK(batch_alloc(err));
     DCK(prefill_rows(n_seqs, tokens_host, lengths, pos0s, slots));
     cudaStream_t s = ctx_->stream;
@@ -1350,6 +1390,74 @@ cudaError_t LlamaDecoder::prefill_batch(int n_seqs, const int *tokens_host, cons
     if (logits_host) memcpy(logits_host, h_blogits_, (size_t)n_seqs * V * sizeof(float));
     if (next_tokens) memcpy(next_tokens, h_bnext_, (size_t)n_seqs * sizeof(int));
     return cudaSuccess;
+}
+
+// ------------------------------------------------------------------------------------------------ teacher-forced scoring
+cudaError_t LlamaDecoder::score_reserve(int n) {
+    if (n <= sc_cap_) return cudaSuccess;
+    DCK(cudaStreamSynchronize(ctx_->stream));
+    cudaFree(sc_rec_);
+    cudaFree(sc_state_);
+    cudaFree(sc_target_);
+    cudaFree(sc_tgt_);
+    cudaFree(sc_out_);
+    sc_rec_ = nullptr; sc_state_ = nullptr; sc_target_ = nullptr; sc_tgt_ = nullptr; sc_out_ = nullptr;
+    sc_cap_ = 0;
+    DCK(cudaMalloc(&sc_rec_, (size_t)n * (pf_lm_chunk_ / 128) * sizeof(LmStat)));
+    DCK(cudaMalloc(&sc_state_, (size_t)n * sizeof(LmStat)));
+    DCK(cudaMalloc(&sc_target_, (size_t)n * sizeof(int)));
+    DCK(cudaMalloc(&sc_tgt_, (size_t)n * sizeof(float)));
+    DCK(cudaMalloc(&sc_out_, (size_t)3 * n * sizeof(float)));
+    sc_cap_ = n;
+    return cudaSuccess;
+}
+
+// The prompt pass of prefill_batch, then the final RMSNorm over all n rows and the lm_head as the W4A16 prompt-pass GEMM, chunk by chunk on the
+// same double-buffered expansion (the first chunk expands while the last down_proj runs).  The GEMM epilogue reduces each row's 128-column
+// slices to {max, sum of exp, arg-max} records; a merge kernel folds them in column order into a running state per row and, after the last
+// chunk, writes the log-probabilities.  Every reduction has a fixed order: the results do not depend on the other rows of the call.
+cudaError_t LlamaDecoder::score_batch(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, const int *targets_host,
+                                      float *logprobs_host, int *greedy_host, float *greedy_logprobs_host, float *logits_dev, std::string *err) {
+    if (tp_ > 1) {
+        if (err) *err = "scoring is single-GPU in this build (tp_size > 1)";
+        return cudaErrorNotSupported;
+    }
+    int n = 0;
+    DCK(check_prompts(n_seqs, tokens_host, lengths, pos0s, slots, &n));
+    const int E = cfg_.embed_dim, V = cfg_.vocab_size;
+    std::vector<int> target(n);
+    if (targets_host) {
+        for (int i = 0; i < n; i++) {
+            if (targets_host[i] < -1 || targets_host[i] >= V) return cudaErrorInvalidValue;
+            target[i] = targets_host[i];
+        }
+    } else {  // the next token of the same prompt; none after a prompt's last row
+        for (int b = 0, row = 0; b < n_seqs; row += lengths[b++])
+            for (int i = 0; i < lengths[b]; i++) target[row + i] = i + 1 < lengths[b] ? tokens_host[row + i + 1] : -1;
+    }
+    DCK(prefill_reserve(n));
+    DCK(pf_setup());
+    DCK(score_reserve(n));
+    DCK(prefill_rows(n_seqs, tokens_host, lengths, pos0s, slots, true));
+    cudaStream_t s = ctx_->stream;
+    DCK(cudaMemcpyAsync(sc_target_, target.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
+    DCK(launch_rmsnorm_rows_f32(ctx_, pf_x_, w_.final_norm, pf_xn_, n, E, cfg_.rms_eps));
+    float *logprob = sc_out_, *glp = sc_out_ + 2 * (size_t)n;
+    int *greedy = reinterpret_cast<int *>(sc_out_ + n);
+    const int rec_ld = pf_lm_chunk_ / 128, first = 4 * cfg_.num_layers;
+    for (int j = first; j < pf_njobs_; j++) {
+        const PfJob &job = pf_jobs_[j];
+        const __half *w16 = nullptr;
+        DCK(pf_job_begin(j, &w16));
+        DCK(launch_gemm_f16_pair_stats(ctx_, pf_xn_, E, w16, E, n, job.rows[0], E, job.r0[0], sc_rec_, rec_ld, sc_target_, sc_tgt_, logits_dev, V));
+        DCK(cudaEventRecord(pf_consumed_[j & 1], s));
+        DCK(launch_lm_stats_merge(ctx_, sc_rec_, rec_ld, (job.rows[0] + 127) / 128, n, j == first, j + 1 == pf_njobs_, sc_state_, sc_target_, sc_tgt_,
+                                  logprob, greedy, glp));
+    }
+    if (logprobs_host) DCK(cudaMemcpyAsync(logprobs_host, logprob, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, s));
+    if (greedy_host) DCK(cudaMemcpyAsync(greedy_host, greedy, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, s));
+    if (greedy_logprobs_host) DCK(cudaMemcpyAsync(greedy_logprobs_host, glp, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, s));
+    return cudaStreamSynchronize(s);
 }
 
 // The generate loop of `generate` for up to TCE_LLAMA_MAX_BATCH sequences: every token is one batched step on the request buffer d_breq_ and

@@ -24,6 +24,10 @@ class LlamaDecoder {
     // n_seqs prompts (concatenated in tokens_host) into their own slots in one pass over the weights; logits / greedy token of each last row
     cudaError_t prefill_batch(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, float *logits_host,
                               int *next_tokens, std::string *err);
+    // teacher-forced scoring: the prompt pass of prefill_batch plus the lm_head over every row, reduced to log-probabilities in the GEMM
+    // epilogue (tce_llama_score_batch)
+    cudaError_t score_batch(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, const int *targets_host,
+                            float *logprobs_host, int *greedy_host, float *greedy_logprobs_host, float *logits_dev, std::string *err);
     const float *logits() const { return d_logits_; }
     void *kv_cache(int layer, int which) const { return kv_cache_slot(0, layer, which); }
     // batched decode: up to TCE_LLAMA_MAX_BATCH sequences per step, each in its own KV-cache slot (slot 0 = d_kv_)
@@ -57,8 +61,11 @@ class LlamaDecoder {
     LlamaDecoder() = default;
     cudaError_t prefill_reserve(int n);
     cudaError_t prefill_linear(int j, const __half *x, void *C, long long ldc, int n, EpiMode epi);
-    // the prompt pass over n_seqs concatenated prompts (host-checked arguments); leaves the final residual rows in pf_x_
-    cudaError_t prefill_rows(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots);
+    // the checks of a batch of prompts (prefill_batch, score_batch): cudaErrorInvalidValue, or the total row count in *n
+    cudaError_t check_prompts(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, int *n) const;
+    // the prompt pass over n_seqs concatenated prompts (host-checked arguments); leaves the final residual rows in pf_x_.  With score, the
+    // expansion of the first lm_head chunk is queued behind the last down_proj GEMM.
+    cudaError_t prefill_rows(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, bool score = false);
     cudaError_t enqueue_step(const int *tokpos, cudaStream_t s, bool pdl, bool gemv_only = false);  // raw kernel sequence
     cudaError_t build_graphs(std::string *err);
     void build_ops();
@@ -120,10 +127,24 @@ class LlamaDecoder {
     size_t pf_w16_elems_ = 0;
     cudaStream_t pf_side_ = nullptr;
     cudaEvent_t pf_expanded_[2] = {nullptr, nullptr}, pf_consumed_[2] = {nullptr, nullptr};
-    // one job per linear of the prompt pass, in launch order: job 4 * layer + {0: q|k|v, 1: o, 2: gate|up, 3: down}
-    struct PfJob { const tce_w4_tensor *ts[3]; int count; };
+    // one job per linear of the prompt pass, in launch order: job 4 * layer + {0: q|k|v, 1: o, 2: gate|up, 3: down}, then the lm_head in
+    // chunks of pf_lm_chunk_ rows (scoring only); job j expands rows r0[i] .. r0[i] + rows[i] - 1 of each of its tensors, stacked
+    struct PfJob { const tce_w4_tensor *ts[3]; int count; int r0[3], rows[3]; };
     std::vector<PfJob> pf_jobs_;
+    int pf_njobs_ = 0;      // jobs the current pass runs: 4 * layers, or all of them when it scores
+    int pf_lm_chunk_ = 0;   // lm_head rows per chunk: whole 256-row blocks that fit one scratch half
+    cudaError_t pf_setup();
     cudaError_t pf_expand_job(int j);
+    cudaError_t pf_job_begin(int j, const __half **w16);  // queues job j + 1's expansion, then waits for job j's weights
+    // scoring buffers, [sc_cap_] rows each (allocated on first use): one chunk's records, the running state across chunks, the targets and
+    // their logits, the outputs {logprob, greedy id, greedy logprob}
+    int sc_cap_ = 0;
+    LmStat *sc_rec_ = nullptr;      // [n][pf_lm_chunk_ / 128]
+    LmStat *sc_state_ = nullptr;    // [n]
+    int *sc_target_ = nullptr;      // [n]
+    float *sc_tgt_ = nullptr;       // [n]
+    float *sc_out_ = nullptr;       // [3][n]
+    cudaError_t score_reserve(int n);
     // pinned host staging for the end-to-end entry point
     int *h_tokpos_ = nullptr;
     float *h_logits_ = nullptr;

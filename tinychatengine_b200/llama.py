@@ -342,6 +342,43 @@ class LlamaModel:
                    "tce_llama_prefill_batch")
         return list(nxt[:n])
 
+    def score_batch(self, prompts, slots, pos0s=None, targets=None, logits=None):
+        """Teacher-forced scoring of up to MAX_BATCH prompts in one prompt pass (the KV rows prefill_batch would write are written too).
+        targets: per prompt, the token whose log-probability each position reports (-1 for none); default: the next token of the prompt,
+        -1 at its last position.  logits: optional CUDA float32 tensor [n, vocab] (n = all positions of all prompts) that receives every
+        position's logits.  Returns, per prompt, (logprobs float32, greedy ids int32, greedy logprobs float32) numpy arrays; logprobs are
+        NaN where the target is -1."""
+        import numpy as np
+
+        n_seqs = len(prompts)
+        pos0s = [0] * n_seqs if pos0s is None else list(pos0s)
+        lengths = [len(q) for q in prompts]
+        n = sum(lengths)
+        flat = np.ascontiguousarray(np.asarray([int(t) for q in prompts for t in q] or [0], dtype=np.int32))
+        arr = lambda v: (C.c_int * max(1, len(v)))(*[int(x) for x in v])
+        tg = None
+        if targets is not None:
+            if [len(t) for t in targets] != lengths:
+                raise ValueError("score_batch: targets must have one entry per prompt position")
+            tg = np.ascontiguousarray(np.asarray([int(t) for q in targets for t in q] or [0], dtype=np.int32))
+        lp = np.empty(max(1, n), dtype=np.float32)
+        gr = np.empty(max(1, n), dtype=np.int32)
+        glp = np.empty(max(1, n), dtype=np.float32)
+        lg = None
+        if logits is not None:
+            V = self.geom.vocab_size
+            if not (logits.is_cuda and logits.dtype == torch.float32 and logits.is_contiguous() and tuple(logits.shape) == (n, V)):
+                raise ValueError(f"score_batch: logits must be a contiguous CUDA float32 tensor of shape ({n}, {V})")
+            lg = C.c_void_p(logits.data_ptr())
+        ptr = lambda a: a.ctypes.data_as(C.c_void_p)
+        _lib.check(self.ctx.L.tce_llama_score_batch(self.h, n_seqs, ptr(flat), arr(lengths), arr(pos0s), arr(slots),
+                                                    None if tg is None else ptr(tg), ptr(lp), ptr(gr), ptr(glp), lg), "tce_llama_score_batch")
+        out, r = [], 0
+        for m in lengths:
+            out.append((lp[r:r + m].copy(), gr[r:r + m].copy(), glp[r:r + m].copy()))
+            r += m
+        return out
+
     def generate_batch(self, requests) -> list[list[int]]:
         """Device generate loop of up to MAX_BATCH sequences (one batched step + one sampler launch per token, only the ids come back).
         Each request is a dict with first_token, pos0, slot, n_predict and optional history, eos_id and the sampling fields of generate(),
