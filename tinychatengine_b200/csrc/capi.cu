@@ -470,17 +470,7 @@ int tce_sample(tce_ctx *ctx, float *logits_dev, int n_vocab, const int *window_h
     const int ctl[4] = {0, n_window, 0, 0};
     cudaError_t e = cudaMemcpyAsync(scratch, ctl, sizeof(ctl), cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess && n_window > 0) e = cudaMemcpyAsync(win, window_host, (size_t)n_window * sizeof(int), cudaMemcpyHostToDevice, s);
-    SampleArgs a{};
-    a.logits = logits_dev;
-    a.n_vocab = n_vocab;
-    a.top_k = cfg->top_k;
-    a.top_p = cfg->top_p;
-    a.temp = cfg->temp;
-    a.repeat_penalty = cfg->repeat_penalty;
-    a.frequency_penalty = cfg->frequency_penalty;
-    a.presence_penalty = cfg->presence_penalty;
-    a.repeat_last_n = cfg->repeat_last_n;
-    a.seed = cfg->seed;
+    SampleArgs a = sample_args(*cfg, logits_dev, n_vocab);
     a.draw_index = draw_index;
     if (n_window > 0) {
         a.hist = win;

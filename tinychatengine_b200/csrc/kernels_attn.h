@@ -2,6 +2,8 @@
 #pragma once
 #include "kernels.h"
 
+struct tce_sampling;  // include/tce_b200.h
+
 namespace tce {
 
 struct AttnDecodeArgs {
@@ -94,6 +96,10 @@ struct SampleArgs {
     float *dbg_probs = nullptr;
     int *dbg_size = nullptr;
 };
+// the sampler arguments of one chain: the fields of tce_sampling, draw index 0, no history, outputs or limits
+SampleArgs sample_args(const tce_sampling &sc, float *logits, int n_vocab);
+// temp > 0 over a vocabulary of more than 1024 ids needs 1 <= top_k <= 1024 (launch_sample returns cudaErrorNotSupported otherwise)
+bool sampling_supported(float temp, int top_k, int n_vocab);
 cudaError_t launch_sample(Ctx *ctx, const SampleArgs &a, cudaStream_t stream);
 // rows_dev = device SampleArgs[rows]: row b is sampled by block b (the generate loop of the batched step; host-checked arguments)
 cudaError_t launch_sample_rows(const SampleArgs *rows_dev, int rows, cudaStream_t stream);

@@ -56,29 +56,29 @@ LlamaDecoder *LlamaDecoder::create(Ctx *ctx, int attn_chunk, const tce_llama_con
     d->atomic_residual_ = getenv("TCE_DETERMINISTIC") == nullptr;
     const size_t kv_elems = (size_t)cfg.num_layers * 2 * KVH * cfg.max_ctx * hd;
     cudaError_t e = cudaSuccess;
-    auto A = [&](void **p, size_t bytes) {
-        if (e == cudaSuccess) e = cudaMalloc(p, bytes);
+    auto A = [&](auto &p, size_t count) {
+        if (e == cudaSuccess) e = dev_alloc(p, count);
     };
-    A((void **)&d->d_kv_, kv_elems * sizeof(__half));
-    A((void **)&d->d_resid_, (size_t)2 * E * sizeof(float));  // two buffers: the tensor-parallel path ping-pongs the residual
-    A((void **)&d->d_qkv_, (size_t)(H + 2 * KVH) * hd * sizeof(__half));
-    A((void **)&d->d_attn_, (size_t)H * hd * sizeof(__half));
-    A((void **)&d->d_act_, (size_t)F * sizeof(__half));
-    A((void **)&d->d_logits_, (size_t)V * sizeof(float));
-    A((void **)&d->d_tokpos_, 4 * sizeof(int));
-    A((void **)&d->d_next_, sizeof(int));
-    if (e == cudaSuccess) e = cudaMemset(d->d_kv_, 0, kv_elems * sizeof(__half));
-    if (e == cudaSuccess) e = cudaMemset(d->d_tokpos_, 0, 4 * sizeof(int));  // [3] = tensor-parallel step counter, advanced on the device
-    if (e == cudaSuccess) e = cudaMalloc((void **)&d->d_tokpos_safe_, 4 * sizeof(int));
-    if (e == cudaSuccess) e = cudaMemset(d->d_tokpos_safe_, 0, 4 * sizeof(int));
-    if (e == cudaSuccess) e = cudaMallocHost((void **)&d->h_tokpos_, 4 * sizeof(int));
-    if (e == cudaSuccess) e = cudaMallocHost((void **)&d->h_logits_, (size_t)V * sizeof(float));
-    if (e == cudaSuccess) e = cudaMallocHost((void **)&d->h_next_, sizeof(int));
+    A(d->d_kv_, kv_elems);
+    A(d->d_resid_, (size_t)2 * E);  // two buffers: the tensor-parallel path ping-pongs the residual
+    A(d->d_qkv_, (size_t)(H + 2 * KVH) * hd);
+    A(d->d_attn_, (size_t)H * hd);
+    A(d->d_act_, (size_t)F);
+    A(d->d_logits_, (size_t)V);
+    A(d->d_tokpos_, 4);
+    A(d->d_next_, 1);
+    if (e == cudaSuccess) e = cudaMemset(d->d_kv_.get(), 0, kv_elems * sizeof(__half));
+    if (e == cudaSuccess) e = cudaMemset(d->d_tokpos_.get(), 0, 4 * sizeof(int));  // [3] = tensor-parallel step counter, advanced on the device
+    A(d->d_tokpos_safe_, 4);
+    if (e == cudaSuccess) e = cudaMemset(d->d_tokpos_safe_.get(), 0, 4 * sizeof(int));
+    if (e == cudaSuccess) e = host_alloc(d->h_tokpos_, 4);
+    if (e == cudaSuccess) e = host_alloc(d->h_logits_, (size_t)V);
+    if (e == cudaSuccess) e = host_alloc(d->h_next_, 1);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&d->cap_stream_, cudaStreamNonBlocking);
     if (e == cudaSuccess) {
         if (w.rope_cos && w.rope_sin) {
-            d->d_cos_ = const_cast<float *>(w.rope_cos);
-            d->d_sin_ = const_cast<float *>(w.rope_sin);
+            d->d_cos_ = w.rope_cos;
+            d->d_sin_ = w.rope_sin;
         } else {
             // HF rotate-half tables: cos/sin(pos * theta^(-2i/hd)) duplicated over both halves
             std::vector<float> hc((size_t)cfg.max_ctx * hd), hs((size_t)cfg.max_ctx * hd);
@@ -90,11 +90,11 @@ LlamaDecoder *LlamaDecoder::create(Ctx *ctx, int attn_chunk, const tce_llama_con
                     hc[(size_t)p * hd + i] = hc[(size_t)p * hd + i + hd / 2] = (float)cos(ang);
                     hs[(size_t)p * hd + i] = hs[(size_t)p * hd + i + hd / 2] = (float)sin(ang);
                 }
-            A((void **)&d->d_cos_, hc.size() * sizeof(float));
-            A((void **)&d->d_sin_, hs.size() * sizeof(float));
-            d->own_rope_ = true;
-            if (e == cudaSuccess) e = cudaMemcpy(d->d_cos_, hc.data(), hc.size() * sizeof(float), cudaMemcpyHostToDevice);
-            if (e == cudaSuccess) e = cudaMemcpy(d->d_sin_, hs.data(), hs.size() * sizeof(float), cudaMemcpyHostToDevice);
+            A(d->rope_, 2 * hc.size());
+            if (e == cudaSuccess) e = cudaMemcpy(d->rope_.get(), hc.data(), hc.size() * sizeof(float), cudaMemcpyHostToDevice);
+            if (e == cudaSuccess) e = cudaMemcpy(d->rope_.get() + hc.size(), hs.data(), hs.size() * sizeof(float), cudaMemcpyHostToDevice);
+            d->d_cos_ = d->rope_.get();
+            d->d_sin_ = d->rope_.get() + hc.size();
         }
     }
     if (e != cudaSuccess) {
@@ -111,13 +111,12 @@ LlamaDecoder *LlamaDecoder::create(Ctx *ctx, int attn_chunk, const tce_llama_con
         // persistent kernel layout: two delta buffers of P x E {float, tag} words + P x 2 key words
         const size_t pk_bytes = ((size_t)2 * d->tp_ * E + (size_t)2 * d->tp_) * sizeof(uint2);
         if (d->tp_bytes_ < pk_bytes) d->tp_bytes_ = pk_bytes;
-        if (cudaMalloc((void **)&d->tp_buf_, d->tp_bytes_) != cudaSuccess || cudaMemset(d->tp_buf_, 0, d->tp_bytes_) != cudaSuccess) {
+        if (dev_alloc(d->tp_buf_, d->tp_bytes_) != cudaSuccess || cudaMemset(d->tp_buf_.get(), 0, d->tp_bytes_) != cudaSuccess) {
             *err = "tensor-parallel buffer allocation failed";
             delete d;
             return nullptr;
         }
         cudaDeviceSynchronize();
-        d->kernels_per_step_ = d->persistent_ ? 1 : 1 + 7 * cfg.num_layers + 4;
         return d;  // the op list needs the peers' pointers: built in tp_connect()
     }
     d->build_ops();
@@ -132,76 +131,24 @@ LlamaDecoder *LlamaDecoder::create(Ctx *ctx, int attn_chunk, const tce_llama_con
             return nullptr;
         }
     }
-    d->kernels_per_step_ = d->persistent_ ? 1 : 1 + 5 * cfg.num_layers + 2;
     return d;
 }
 
 LlamaDecoder::~LlamaDecoder() {
-    if (g_host_) cudaGraphExecDestroy(g_host_);
-    if (g_dev_) cudaGraphExecDestroy(g_dev_);
     if (cap_stream_) cudaStreamDestroy(cap_stream_);
-    cudaFree(d_kv_);
-    cudaFree(d_resid_);
-    cudaFree(d_qkv_);
-    cudaFree(d_attn_);
-    cudaFree(d_act_);
-    cudaFree(d_logits_);
-    cudaFree(d_tokpos_);
-    cudaFree(d_gen_);
-    cudaFree(d_tokpos_safe_);
     for (int b = 0; b < 2; b++) {
-        cudaFree(pf_w16_[b]);
         if (pf_expanded_[b]) cudaEventDestroy(pf_expanded_[b]);
         if (pf_consumed_[b]) cudaEventDestroy(pf_consumed_[b]);
     }
     if (pf_side_) cudaStreamDestroy(pf_side_);
-    cudaFree(d_next_);
-    cudaFree(pf_x_);
-    cudaFree(pf_xn_);
-    cudaFree(pf_qkv_);
-    cudaFree(pf_att_);
-    cudaFree(pf_act_);
-    cudaFree(pf_tok_);
-    cudaFree(sc_rec_);
-    cudaFree(sc_state_);
-    cudaFree(sc_target_);
-    cudaFree(sc_tgt_);
-    cudaFree(sc_out_);
-    for (void *p : pk_allocs_) cudaFree(p);
     for (int p = 0; p < tp_; p++)
         if (p != cfg_.tp_rank && tp_peer_[p]) cudaIpcCloseMemHandle(tp_peer_[p]);
-    cudaFree(tp_buf_);
-    if (own_rope_) {
-        cudaFree(d_cos_);
-        cudaFree(d_sin_);
-    }
-    if (h_tokpos_) cudaFreeHost(h_tokpos_);
-    if (h_logits_) cudaFreeHost(h_logits_);
-    if (h_next_) cudaFreeHost(h_next_);
-    drop_batch_graphs();
-    for (__half *p : slot_kv_) cudaFree(p);
-    cudaFree(d_slot_table_);
-    cudaFree(d_bresid_);
-    cudaFree(d_bqkv_);
-    cudaFree(d_battn_);
-    cudaFree(d_bact_);
-    cudaFree(d_blogits_);
-    cudaFree(d_breq_);
-    cudaFree(d_bsafe_);
-    cudaFree(d_bnext_);
-    cudaFree(d_battn_ws_);
-    cudaFree(d_battn_counters_);
-    cudaFree(d_bgen_);
-    cudaFree(d_bsample_);
-    if (h_breq_) cudaFreeHost(h_breq_);
-    if (h_bnext_) cudaFreeHost(h_bnext_);
-    if (h_blogits_) cudaFreeHost(h_blogits_);
 }
 
 void *LlamaDecoder::kv_cache_slot(int slot, int layer, int which) const {
     if (slot < 0 || slot >= n_slots() || layer < 0 || layer >= cfg_.num_layers || which < 0 || which > 1) return nullptr;
     const size_t per = (size_t)cfg_.num_kv_heads * cfg_.max_ctx * cfg_.head_dim;
-    return (slot == 0 ? d_kv_ : slot_kv_[slot - 1]) + ((size_t)layer * 2 + which) * per;
+    return (slot == 0 ? d_kv_ : slot_kv_[slot - 1]).get() + ((size_t)layer * 2 + which) * per;
 }
 
 static W4Seg seg_of(const tce_w4_tensor &t) { return W4Seg{(const uint32_t *)t.w, (const uint32_t *)t.zeros, (const __half *)t.scales, t.oc}; }
@@ -209,13 +156,13 @@ static W4Seg seg_of(const tce_w4_tensor &t) { return W4Seg{(const uint32_t *)t.w
 cudaError_t LlamaDecoder::enqueue_gemvs(int *count) {
     if (tp_ > 1) return cudaErrorNotSupported;  // the GEMVs of a tensor-parallel step poll their peers: without the rest of the step they would spin
     *count = 4 * cfg_.num_layers + 1;
-    return enqueue_step(d_tokpos_, ctx_->stream, false, true);
+    return enqueue_step(d_tokpos_.get(), ctx_->stream, false, true);
 }
 
 cudaError_t LlamaDecoder::tp_handle(void *out64) {
     if (tp_ <= 1 || !tp_buf_) return cudaErrorInvalidValue;
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "handle size");
-    return cudaIpcGetMemHandle(reinterpret_cast<cudaIpcMemHandle_t *>(out64), tp_buf_);
+    return cudaIpcGetMemHandle(reinterpret_cast<cudaIpcMemHandle_t *>(out64), tp_buf_.get());
 }
 
 cudaError_t LlamaDecoder::tp_connect(const void *handles) {
@@ -223,7 +170,7 @@ cudaError_t LlamaDecoder::tp_connect(const void *handles) {
     const cudaIpcMemHandle_t *h = reinterpret_cast<const cudaIpcMemHandle_t *>(handles);
     for (int p = 0; p < tp_; p++) {
         if (p == cfg_.tp_rank) {
-            tp_peer_[p] = tp_buf_;
+            tp_peer_[p] = tp_buf_.get();
         } else {
             DCK(cudaIpcOpenMemHandle((void **)&tp_peer_[p], h[p], cudaIpcMemLazyEnablePeerAccess));
         }
@@ -235,7 +182,6 @@ cudaError_t LlamaDecoder::tp_connect(const void *handles) {
         cudaError_t e = build_persistent(&why);
         if (e == cudaErrorNotSupported) {
             persistent_ = false;
-            kernels_per_step_ = 1 + 7 * cfg_.num_layers + 4;
         } else if (e != cudaSuccess) {
             return e;
         }
@@ -253,7 +199,7 @@ void LlamaDecoder::build_ops() {
     ops_.push_back(emb);
     // ---- tensor-parallel plumbing (tp_ == 1: every helper below is a no-op) ----
     const int P = tp_, per_step = 2 * cfg_.num_layers + 1;
-    float *resid[2] = {d_resid_, d_resid_ + E};
+    float *resid[2] = {d_resid_.get(), d_resid_.get() + E};
     int cur = 0;  // residual buffer holding the stream
     auto gather_of = [&](int peer, int buf) { return reinterpret_cast<float *>(tp_peer_[peer]) + ((size_t)buf * P) * E; };            // [P][E]
     auto flags_of = [&](int peer, int buf) { return reinterpret_cast<unsigned *>(reinterpret_cast<float *>(tp_peer_[peer]) + tp_gather_floats_) + buf * kMaxTP; };
@@ -266,7 +212,7 @@ void LlamaDecoder::build_ops() {
         p.x = resid[cur];
         p.tp_in = gather_of(me, buf);
         p.tp_flags = flags_of(me, buf);
-        p.tp_step = d_tokpos_ + 3;
+        p.tp_step = d_tokpos_.get() + 3;
         p.tp_k = k;
         p.tp_per_step = per_step;
         p.resid_out = resid[cur ^ 1];
@@ -278,7 +224,7 @@ void LlamaDecoder::build_ops() {
         p.tp_sig_counter = flags_of(me, 0) + 32 + buf;  // spare words of the local flag block
         for (int q = 0; q < P; q++) p.tp_sig_flag[q] = flags_of(q, buf) + me;
         p.tp_sig_k = k;
-        p.tp_step = d_tokpos_ + 3;
+        p.tp_step = d_tokpos_.get() + 3;
         p.tp_per_step = per_step;
         p.epi = EPI_TP_SCATTER_F32;
         p.atomic_residual = false;
@@ -291,7 +237,7 @@ void LlamaDecoder::build_ops() {
         op.sig = TpSignalArgs{};
         for (int q = 0; q < P; q++) op.sig.peer_flag[q] = flags_of(q, buf) + me;
         op.sig.tp_size = P;
-        op.sig.step = d_tokpos_ + 3;
+        op.sig.step = d_tokpos_.get() + 3;
         op.sig.k = k;
         op.sig.per_step = per_step;
         ops_.push_back(op);
@@ -308,12 +254,12 @@ void LlamaDecoder::build_ops() {
             p.seg[2] = seg_of(L.v);
             p.IC = E;
             p.M = 1;
-            p.x = d_resid_;
+            p.x = d_resid_.get();
             p.x_mode = X_RMSNORM_F32;
             p.ldx = E;
             p.gamma = L.input_norm;
             p.eps = cfg_.rms_eps;
-            p.y = d_qkv_;
+            p.y = d_qkv_.get();
             p.epi = EPI_STORE_HALF;
             p.x = resid[cur];
             if (l > 0) tp_recv(p, 1, 2 * (l - 1) + 1);
@@ -324,12 +270,12 @@ void LlamaDecoder::build_ops() {
             op.type = OP_ATTN;
             AttnDecodeArgs &a = op.at;
             a = AttnDecodeArgs{};
-            a.qkv = d_qkv_;
+            a.qkv = d_qkv_.get();
             a.k_cache = (__half *)kv_cache(l, 0);
             a.v_cache = (__half *)kv_cache(l, 1);
             a.cos = d_cos_;
             a.sin = d_sin_;
-            a.out = d_attn_;
+            a.out = d_attn_.get();
             a.alpha = cfg_.qk_alpha > 0 ? cfg_.qk_alpha : 1.0f / sqrtf((float)hd);
             a.num_heads = H;
             a.num_kv_heads = KVH;
@@ -346,7 +292,7 @@ void LlamaDecoder::build_ops() {
             p.seg[0] = seg_of(L.o);
             p.IC = H * hd;
             p.M = 1;
-            p.x = d_attn_;
+            p.x = d_attn_.get();
             p.x_mode = X_HALF;
             p.y = resid[cur];
             p.epi = EPI_ADD_F32;
@@ -368,7 +314,7 @@ void LlamaDecoder::build_ops() {
             p.x_mode = X_RMSNORM_F32;
             p.gamma = L.post_norm;
             p.eps = cfg_.rms_eps;
-            p.y = d_act_;
+            p.y = d_act_.get();
             p.epi = EPI_SILU_MUL_HALF;
             p.ldy = F;
             tp_recv(p, 0, 2 * l);
@@ -382,7 +328,7 @@ void LlamaDecoder::build_ops() {
             p.seg[0] = seg_of(L.down);
             p.IC = F;
             p.M = 1;
-            p.x = d_act_;
+            p.x = d_act_.get();
             p.x_mode = X_HALF;
             p.y = resid[cur];
             p.epi = EPI_ADD_F32;
@@ -403,17 +349,18 @@ void LlamaDecoder::build_ops() {
         p.x_mode = X_RMSNORM_F32;
         p.gamma = w_.final_norm;
         p.eps = cfg_.rms_eps;
-        p.y = d_logits_;
+        p.y = d_logits_.get();
         p.epi = EPI_STORE_F32;
         tp_recv(p, 1, 2 * (cfg_.num_layers - 1) + 1);
         ops_.push_back(op);
+        lm_gemv_ = p;
     }
     if (P > 1) {
         // greedy token over the vocabulary shards: scatter the local key, signal, pick the global maximum
         StepOp sc;
         sc.type = OP_TP_ARGMAX_SCATTER;
         sc.am = TpArgmaxArgs{};
-        sc.am.logits = d_logits_;
+        sc.am.logits = d_logits_.get();
         sc.am.n_local = cfg_.vocab_size;
         sc.am.index_base = me * cfg_.vocab_size;
         for (int q = 0; q < P; q++) sc.am.peer_key[q] = keys_of(q) + me;
@@ -425,11 +372,11 @@ void LlamaDecoder::build_ops() {
         fin.amf = TpArgmaxFinishArgs{};
         fin.amf.keys = keys_of(me);
         fin.amf.flags = flags_of(me, 2);
-        fin.amf.step = d_tokpos_ + 3;
+        fin.amf.step = d_tokpos_.get() + 3;
         fin.amf.k = 2 * cfg_.num_layers;
         fin.amf.per_step = per_step;
         fin.amf.tp_size = P;
-        fin.amf.next_token = d_next_;
+        fin.amf.next_token = d_next_.get();
         ops_.push_back(fin);
     } else {
         StepOp am;
@@ -494,10 +441,10 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
     a.pair = 0;  // decided below, once the shared-memory footprint is known
 
     auto dalloc = [&](size_t bytes) -> void * {
-        void *p = nullptr;
-        if (cudaMalloc(&p, bytes ? bytes : 16) != cudaSuccess) return nullptr;
-        pk_allocs_.push_back(p);
-        return p;
+        DevPtr<uint8_t> p;
+        if (dev_alloc(p, bytes ? bytes : 16) != cudaSuccess) return nullptr;
+        pk_allocs_.push_back(std::move(p));
+        return pk_allocs_.back().get();
     };
     cudaStream_t s = ctx_->stream;
     // ---- tensor maps: [Lyr][7] + lm_head + KV cache ----
@@ -541,7 +488,7 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         const W4Seg lm[1] = {seg_of(w_.lm_head)};
         DCK(pk::repack_meta(ctx_, lm, 1, 0, o.IC, m, s));
         a.lm_meta = m;
-        DCK(pk::encode_kv_tmap(&maps[(size_t)Lyr * 7 + 1], d_kv_, (long long)Lyr * 2 * per_kv));
+        DCK(pk::encode_kv_tmap(&maps[(size_t)Lyr * 7 + 1], d_kv_.get(), (long long)Lyr * 2 * per_kv));
     }
     CUtensorMap *dmaps = (CUtensorMap *)dalloc(maps.size() * sizeof(CUtensorMap));
     pk::LayerDesc *ddesc = (pk::LayerDesc *)dalloc(descs.size() * sizeof(pk::LayerDesc));
@@ -568,9 +515,9 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
     a.attn_ll = a.qkv_ll + n_qkv;
     a.act_ll = a.attn_ll + n_attn;
     a.part_ll = a.act_ll + n_act;
-    a.logits = d_logits_;
-    a.tokpos = d_tokpos_;
-    a.next_token = d_next_;
+    a.logits = d_logits_.get();
+    a.tokpos = d_tokpos_.get();
+    a.next_token = d_next_.get();
     a.argmax_cell = reinterpret_cast<unsigned long long *>(ctl);
     a.epoch = reinterpret_cast<unsigned *>(ctl + 8);
     a.error = reinterpret_cast<int *>(ctl + 12);
@@ -632,7 +579,8 @@ cudaError_t LlamaDecoder::enqueue_step(const int *tokpos, cudaStream_t s, bool p
             case OP_EMBED:
                 // also range-checks the device-resident {token, position} and publishes the clamped pair for the attention launches of this step
                 if (!gemv_only)
-                    DCK(launch_embedding(c, (const __half *)w_.embed_f16, tokpos, d_resid_, cfg_.embed_dim, false, cfg_.vocab_size * tp_, cfg_.max_ctx, d_tokpos_safe_));
+                    DCK(launch_embedding(c, (const __half *)w_.embed_f16, tokpos, d_resid_.get(), cfg_.embed_dim, false, cfg_.vocab_size * tp_, cfg_.max_ctx,
+                                         d_tokpos_safe_.get()));
                 break;
             case OP_GEMV: {
                 W4GemvParams p = op.g;
@@ -643,12 +591,12 @@ cudaError_t LlamaDecoder::enqueue_step(const int *tokpos, cudaStream_t s, bool p
             case OP_ATTN:
                 if (!gemv_only) {
                     AttnDecodeArgs a = op.at;
-                    a.pos = d_tokpos_safe_ + 1;  // the position after the embedding kernel's range check
+                    a.pos = d_tokpos_safe_.get() + 1;  // the position after the embedding kernel's range check
                     DCK(launch_attn_decode(c, a, use_pdl));
                 }
                 break;
             case OP_ARGMAX:
-                if (!gemv_only) DCK(launch_argmax(c, d_logits_, cfg_.vocab_size, d_next_, use_pdl));
+                if (!gemv_only) DCK(launch_argmax(c, d_logits_.get(), cfg_.vocab_size, d_next_.get(), use_pdl));
                 break;
             case OP_TP_SIGNAL:
                 if (!gemv_only) DCK(launch_tp_signal(c, op.sig));
@@ -665,69 +613,54 @@ cudaError_t LlamaDecoder::enqueue_step(const int *tokpos, cudaStream_t s, bool p
     return cudaSuccess;
 }
 
-cudaError_t LlamaDecoder::build_graphs(std::string *err) {
-    // one eager step first: loads the modules and sets the kernels' shared-memory attributes outside of capture
-    // (re-running a step at the same position is idempotent: the same K/V row is rewritten).  Work queued on the caller's stream
-    // (an asynchronous decode_device) touches the same buffers: drain it before switching to the capture stream.
-    DCK(cudaStreamSynchronize(ctx_->stream));
-    DCK(cudaMemcpyAsync(d_tokpos_, h_tokpos_, 3 * sizeof(int), cudaMemcpyHostToDevice, cap_stream_));
-    DCK(enqueue_step(d_tokpos_, cap_stream_, false));
-    DCK(cudaStreamSynchronize(cap_stream_));
-    // try PDL edges first; if capture/instantiate refuses them, fall back to plain edges
-    for (int attempt = 0; attempt < 2; attempt++) {
-        const bool pdl = ctx_->use_pdl && attempt == 0;
-        cudaGraph_t g = nullptr;
+cudaError_t LlamaDecoder::run_graphed(CachedGraph &g, const void *key, const std::function<cudaError_t(cudaStream_t, bool)> &body) {
+    cudaStream_t s = ctx_->stream;
+    if (!use_graphs_) return body(s, ctx_->use_pdl);
+    if (g.exec && g.key == key && g.gen == ctx_->option_gen) return cudaGraphLaunch(g.exec, s);
+    // a graph holds the context by value: after an option or the stream changed (option_gen) it is rebuilt.  This call runs eagerly, which
+    // also loads the modules, sets kernel attributes and grows the GEMV fix-up records outside of capture; capture itself runs nothing.
+    g.reset();
+    DCK(body(s, ctx_->use_pdl));
+    for (int attempt = ctx_->use_pdl ? 0 : 1; attempt < 2; attempt++) {
+        const bool pdl = attempt == 0;
+        cudaGraph_t graph = nullptr;
         cudaError_t e = cudaStreamBeginCapture(cap_stream_, cudaStreamCaptureModeThreadLocal);
-        if (e != cudaSuccess) return e;
-        e = cudaMemcpyAsync(d_tokpos_, h_tokpos_, 3 * sizeof(int), cudaMemcpyHostToDevice, cap_stream_);
-        if (e == cudaSuccess) e = enqueue_step(d_tokpos_, cap_stream_, pdl);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(h_logits_, d_logits_, (size_t)cfg_.vocab_size * sizeof(float), cudaMemcpyDeviceToHost, cap_stream_);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(h_next_, d_next_, sizeof(int), cudaMemcpyDeviceToHost, cap_stream_);
-        cudaError_t e2 = cudaStreamEndCapture(cap_stream_, &g);
-        if (e == cudaSuccess) e = e2;
-        if (e == cudaSuccess) e = cudaGraphInstantiate(&g_host_, g, 0);
-        if (g) cudaGraphDestroy(g);
         if (e == cudaSuccess) {
-            graphs_ok_ = true;
-            graphs_gen_ = ctx_->option_gen;
+            e = body(cap_stream_, pdl);
+            const cudaError_t e2 = cudaStreamEndCapture(cap_stream_, &graph);
+            if (e == cudaSuccess) e = e2;
+        }
+        if (e == cudaSuccess) e = cudaGraphInstantiate(&g.exec, graph, 0);
+        if (graph) cudaGraphDestroy(graph);
+        if (e == cudaSuccess) {
             if (!pdl) ctx_->use_pdl = false;
+            g.key = key;
+            g.gen = ctx_->option_gen;  // read after the eager run: growing the fix-up records moves it
             return cudaSuccess;
         }
         cudaGetLastError();
-        if (err) *err = std::string("graph capture failed (pdl=") + (pdl ? "1" : "0") + "): " + cudaGetErrorString(e);
-        g_host_ = nullptr;
-        if (!ctx_->use_pdl) return e;
+        g.exec = nullptr;
     }
-    return cudaErrorUnknown;
+    use_graphs_ = false;  // the work above already ran: carry on without graphs
+    return cudaSuccess;
 }
 
 cudaError_t LlamaDecoder::decode_host(int token, int pos, float *logits_host, int *next_token, std::string *err) {
     const int tp = cfg_.tp_size > 1 ? cfg_.tp_size : 1;
     if (pos < 0 || pos >= cfg_.max_ctx || token < 0 || token >= cfg_.vocab_size * tp) return cudaErrorInvalidValue;
     if (tp > 1 && !tp_connected_) return cudaErrorNotReady;
-    h_tokpos_[0] = token;
-    h_tokpos_[1] = pos;
-    h_tokpos_[2] = 0;
-    cudaStream_t s = ctx_->stream;
-    if (graphs_ok_ && graphs_gen_ != ctx_->option_gen) {  // an option or the stream changed since capture: the graph holds the old context by value
-        cudaGraphExecDestroy(g_host_);
-        g_host_ = nullptr;
-        graphs_ok_ = false;
-    }
-    if (use_graphs_ && !graphs_ok_) {
-        cudaError_t e = build_graphs(err);
-        if (e != cudaSuccess) use_graphs_ = false;
-    }
-    if (use_graphs_ && graphs_ok_) {
-        DCK(cudaGraphLaunch(g_host_, s));
-    } else {
-        DCK(cudaMemcpyAsync(d_tokpos_, h_tokpos_, 3 * sizeof(int), cudaMemcpyHostToDevice, s));
-        DCK(enqueue_step(d_tokpos_, s, ctx_->use_pdl));
-        DCK(cudaMemcpyAsync(h_logits_, d_logits_, (size_t)cfg_.vocab_size * sizeof(float), cudaMemcpyDeviceToHost, s));
-        DCK(cudaMemcpyAsync(h_next_, d_next_, sizeof(int), cudaMemcpyDeviceToHost, s));
-    }
-    DCK(cudaStreamSynchronize(s));
-    if (logits_host) memcpy(logits_host, h_logits_, (size_t)cfg_.vocab_size * sizeof(float));
+    int *h = h_tokpos_.get();
+    h[0] = token;
+    h[1] = pos;
+    h[2] = 0;
+    DCK(run_graphed(g_host_, nullptr, [&](cudaStream_t st, bool pdl) {
+        DCK(cudaMemcpyAsync(d_tokpos_.get(), h, 3 * sizeof(int), cudaMemcpyHostToDevice, st));
+        DCK(enqueue_step(d_tokpos_.get(), st, pdl));
+        DCK(cudaMemcpyAsync(h_logits_.get(), d_logits_.get(), (size_t)cfg_.vocab_size * sizeof(float), cudaMemcpyDeviceToHost, st));
+        return cudaMemcpyAsync(h_next_.get(), d_next_.get(), sizeof(int), cudaMemcpyDeviceToHost, st);
+    }));
+    DCK(cudaStreamSynchronize(ctx_->stream));
+    if (logits_host) memcpy(logits_host, h_logits_.get(), (size_t)cfg_.vocab_size * sizeof(float));
     if (next_token) *next_token = *h_next_;
     return cudaSuccess;
 }
@@ -745,55 +678,45 @@ cudaError_t LlamaDecoder::generate(int first_token, int pos0, int n_predict, con
     if (first_token < 0 || first_token >= cfg_.vocab_size || pos0 < 0 || pos0 >= cap || n_predict < 0 || n_history < 0 || n_history > cap || !n_out ||
         (n_predict > 0 && !out_tokens_host))
         return cudaErrorInvalidValue;
-    if (sc.temp > 0.f && (sc.top_k <= 0 || sc.top_k > 1024) && cfg_.vocab_size > 1024) {
+    if (!sampling_supported(sc.temp, sc.top_k, cfg_.vocab_size)) {
         if (err) *err = "generate: temp > 0 needs 1 <= top_k <= 1024";
         return cudaErrorNotSupported;
     }
     if (n_predict > cap - pos0) n_predict = cap - pos0;
     cudaStream_t s = ctx_->stream;
-    if (!d_gen_) DCK(cudaMalloc((void **)&d_gen_, (size_t)(4 + 2 * cap) * sizeof(int)));
-    int *hist = d_gen_ + 4, *out_list = d_gen_ + 4 + cap;
-    DCK(cudaMemsetAsync(d_gen_, 0, (size_t)(4 + 2 * cap) * sizeof(int), s));
+    if (!d_gen_) DCK(dev_alloc(d_gen_, (size_t)(4 + 2 * cap)));
+    int *hist = d_gen_.get() + 4, *out_list = d_gen_.get() + 4 + cap;
+    DCK(cudaMemsetAsync(d_gen_.get(), 0, (size_t)(4 + 2 * cap) * sizeof(int), s));
     if (n_history > 0) DCK(cudaMemcpyAsync(hist, history_host, (size_t)n_history * sizeof(int), cudaMemcpyHostToDevice, s));
     const int ctl0[4] = {n_history, 0, 0, 0};
-    DCK(cudaMemcpyAsync(d_gen_, ctl0, sizeof(ctl0), cudaMemcpyHostToDevice, s));
-    h_tokpos_[0] = first_token;
-    h_tokpos_[1] = pos0;
-    h_tokpos_[2] = 0;
-    DCK(cudaMemcpyAsync(d_tokpos_, h_tokpos_, 3 * sizeof(int), cudaMemcpyHostToDevice, s));
-    SampleArgs a{};
-    a.logits = d_logits_;
-    a.n_vocab = cfg_.vocab_size;
-    a.top_k = sc.top_k;
-    a.top_p = sc.top_p;
-    a.temp = sc.temp;
-    a.repeat_penalty = sc.repeat_penalty;
-    a.frequency_penalty = sc.frequency_penalty;
-    a.presence_penalty = sc.presence_penalty;
-    a.repeat_last_n = sc.repeat_last_n;
-    a.seed = sc.seed;
-    a.draw_index = 0;
+    DCK(cudaMemcpyAsync(d_gen_.get(), ctl0, sizeof(ctl0), cudaMemcpyHostToDevice, s));
+    int *h = h_tokpos_.get();
+    h[0] = first_token;
+    h[1] = pos0;
+    h[2] = 0;
+    DCK(cudaMemcpyAsync(d_tokpos_.get(), h, 3 * sizeof(int), cudaMemcpyHostToDevice, s));
+    SampleArgs a = sample_args(sc, d_logits_.get(), cfg_.vocab_size);
     a.hist = hist;
-    a.hist_head = d_gen_;
+    a.hist_head = d_gen_.get();
     a.hist_cap = cap;
     a.eos_id = eos_id;
-    a.tokpos = d_tokpos_;
+    a.tokpos = d_tokpos_.get();
     a.out_list = out_list;
-    a.out_count = d_gen_ + 1;
+    a.out_count = d_gen_.get() + 1;
     a.out_cap = cap;
-    a.stop = d_gen_ + 2;
+    a.stop = d_gen_.get() + 2;
     int ctl[4] = {0, 0, 0, 0};
     constexpr int kCheckEvery = 16;
     for (int i = 0; i < n_predict; i++) {
-        DCK(enqueue_step(d_tokpos_, s, ctx_->use_pdl));
+        DCK(enqueue_step(d_tokpos_.get(), s, ctx_->use_pdl));
         DCK(launch_sample(ctx_, a, s));
         if ((i + 1) % kCheckEvery == 0 && i + 1 < n_predict) {
-            DCK(cudaMemcpyAsync(ctl, d_gen_, sizeof(ctl), cudaMemcpyDeviceToHost, s));
+            DCK(cudaMemcpyAsync(ctl, d_gen_.get(), sizeof(ctl), cudaMemcpyDeviceToHost, s));
             DCK(cudaStreamSynchronize(s));
             if (ctl[2]) break;
         }
     }
-    DCK(cudaMemcpyAsync(ctl, d_gen_, sizeof(ctl), cudaMemcpyDeviceToHost, s));
+    DCK(cudaMemcpyAsync(ctl, d_gen_.get(), sizeof(ctl), cudaMemcpyDeviceToHost, s));
     DCK(cudaStreamSynchronize(s));
     const int n = ctl[1] < cap ? ctl[1] : cap;
     if (n > 0) DCK(cudaMemcpy(out_tokens_host, out_list, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
@@ -802,39 +725,8 @@ cudaError_t LlamaDecoder::generate(int first_token, int pos0, int n_predict, con
 }
 
 cudaError_t LlamaDecoder::decode_device(const int *tokpos_dev, std::string *err) {
-    cudaStream_t s = ctx_->stream;
     if (tp_ > 1 && !tp_connected_) return cudaErrorNotReady;
-    if (use_graphs_ && (g_dev_ == nullptr || g_dev_src_ != tokpos_dev || g_dev_gen_ != ctx_->option_gen)) {
-        if (g_dev_) {
-            cudaGraphExecDestroy(g_dev_);
-            g_dev_ = nullptr;
-        }
-        DCK(cudaStreamSynchronize(s));
-        DCK(enqueue_step(tokpos_dev, cap_stream_, false));  // eager warm-up outside of capture (idempotent)
-        DCK(cudaStreamSynchronize(cap_stream_));
-        for (int attempt = 0; attempt < 2 && !g_dev_; attempt++) {
-            const bool pdl = ctx_->use_pdl && attempt == 0;
-            cudaGraph_t g = nullptr;
-            cudaError_t e = cudaStreamBeginCapture(cap_stream_, cudaStreamCaptureModeThreadLocal);
-            if (e == cudaSuccess) e = enqueue_step(tokpos_dev, cap_stream_, pdl);
-            cudaError_t e2 = cudaStreamEndCapture(cap_stream_, &g);
-            if (e == cudaSuccess) e = e2;
-            if (e == cudaSuccess) e = cudaGraphInstantiate(&g_dev_, g, 0);
-            if (g) cudaGraphDestroy(g);
-            if (e != cudaSuccess) {
-                cudaGetLastError();
-                g_dev_ = nullptr;
-                if (err) *err = std::string("graph capture failed: ") + cudaGetErrorString(e);
-                if (!pdl) use_graphs_ = false;
-            } else if (!pdl) {
-                ctx_->use_pdl = false;
-            }
-        }
-        g_dev_src_ = tokpos_dev;
-        g_dev_gen_ = ctx_->option_gen;
-    }
-    if (use_graphs_ && g_dev_) return cudaGraphLaunch(g_dev_, s);
-    return enqueue_step(tokpos_dev, s, ctx_->use_pdl);
+    return run_graphed(g_dev_, tokpos_dev, [&](cudaStream_t st, bool pdl) { return enqueue_step(tokpos_dev, st, pdl); });
 }
 
 }  // namespace tce
@@ -845,25 +737,20 @@ cudaError_t LlamaDecoder::decode_device(const int *tokpos_dev, std::string *err)
 namespace tce {
 
 cudaError_t LlamaDecoder::prefill_reserve(int n) {
-    if (n <= pf_cap_) return cudaSuccess;
+    if (n <= pf_.cap) return cudaSuccess;
     DCK(cudaStreamSynchronize(ctx_->stream));
-    cudaFree(pf_x_);
-    cudaFree(pf_xn_);
-    cudaFree(pf_qkv_);
-    cudaFree(pf_att_);
-    cudaFree(pf_act_);
-    cudaFree(pf_tok_);
-    pf_x_ = nullptr; pf_xn_ = nullptr; pf_qkv_ = nullptr; pf_att_ = nullptr; pf_act_ = nullptr; pf_tok_ = nullptr;
-    pf_cap_ = 0;
+    pf_ = PromptBufs{};  // the old buffers go first
     const size_t E = cfg_.embed_dim, F = cfg_.hidden_dim, Q = (size_t)(cfg_.num_heads + 2 * cfg_.num_kv_heads) * cfg_.head_dim,
                  A = (size_t)cfg_.num_heads * cfg_.head_dim;
-    DCK(cudaMalloc(&pf_x_, n * E * sizeof(float)));
-    DCK(cudaMalloc(&pf_xn_, n * E * sizeof(__half)));
-    DCK(cudaMalloc(&pf_qkv_, n * Q * sizeof(__half)));
-    DCK(cudaMalloc(&pf_att_, n * A * sizeof(__half)));
-    DCK(cudaMalloc(&pf_act_, n * F * sizeof(__half)));
-    DCK(cudaMalloc(&pf_tok_, n * sizeof(int)));
-    pf_cap_ = n;
+    PromptBufs b;
+    DCK(dev_alloc(b.x, n * E));
+    DCK(dev_alloc(b.xn, n * E));
+    DCK(dev_alloc(b.qkv, n * Q));
+    DCK(dev_alloc(b.att, n * A));
+    DCK(dev_alloc(b.act, n * F));
+    DCK(dev_alloc(b.tok, (size_t)n));
+    b.cap = n;
+    pf_ = std::move(b);
     return cudaSuccess;
 }
 
@@ -887,7 +774,7 @@ cudaError_t LlamaDecoder::prefill_linear(int j, const __half *x, void *C, long l
 cudaError_t LlamaDecoder::pf_job_begin(int j, const __half **w16) {
     if (j + 1 < pf_njobs_) DCK(pf_expand_job(j + 1));
     DCK(cudaStreamWaitEvent(ctx_->stream, pf_expanded_[j & 1], 0));
-    *w16 = pf_w16_[j & 1];
+    *w16 = pf_w16_[j & 1].get();
     return cudaSuccess;
 }
 
@@ -904,7 +791,7 @@ cudaError_t LlamaDecoder::pf_expand_job(int j) {
         const tce_w4_tensor &t = *job.ts[i];
         const size_t r = (size_t)job.r0[i];  // first row of the range: offset pointers into the packed words, zeros and scales
         DCK(launch_w4_expand(&side, (const uint32_t *)t.w + r * (ic / 8), (const uint32_t *)t.zeros + r * zw, (const __half *)t.scales + r * zw * 8,
-                             pf_w16_[b] + r0 * ic, job.rows[i], ic));
+                             pf_w16_[b].get() + r0 * ic, job.rows[i], ic));
         r0 += (size_t)job.rows[i];
     }
     return cudaEventRecord(pf_expanded_[b], pf_side_);
@@ -913,6 +800,7 @@ cudaError_t LlamaDecoder::pf_expand_job(int j) {
 // the job list, the double-buffered scratch, its events and the side stream, on first use
 cudaError_t LlamaDecoder::pf_setup() {
     if (!pf_jobs_.empty()) return cudaSuccess;
+    std::vector<PfJob> jobs;
     auto job = [](const tce_w4_tensor *a, const tce_w4_tensor *b, const tce_w4_tensor *c) {
         PfJob j{{a, b, c}, c ? 3 : (b ? 2 : 1), {0, 0, 0}, {0, 0, 0}};
         for (int i = 0; i < j.count; i++) j.rows[i] = j.ts[i]->oc;
@@ -920,13 +808,13 @@ cudaError_t LlamaDecoder::pf_setup() {
     };
     for (int l = 0; l < cfg_.num_layers; l++) {
         const tce_llama_layer &L = layers_[l];
-        pf_jobs_.push_back(job(&L.q, &L.k, &L.v));
-        pf_jobs_.push_back(job(&L.o, nullptr, nullptr));
-        pf_jobs_.push_back(job(&L.gate, &L.up, nullptr));
-        pf_jobs_.push_back(job(&L.down, nullptr, nullptr));
+        jobs.push_back(job(&L.q, &L.k, &L.v));
+        jobs.push_back(job(&L.o, nullptr, nullptr));
+        jobs.push_back(job(&L.gate, &L.up, nullptr));
+        jobs.push_back(job(&L.down, nullptr, nullptr));
     }
     size_t need = 0;
-    for (const PfJob &jb : pf_jobs_) {
+    for (const PfJob &jb : jobs) {
         size_t e = 0;
         for (int i = 0; i < jb.count; i++) e += (size_t)jb.ts[i]->oc * jb.ts[i]->ic;
         need = e > need ? e : need;
@@ -939,15 +827,16 @@ cudaError_t LlamaDecoder::pf_setup() {
         PfJob j = job(&w_.lm_head, nullptr, nullptr);
         j.r0[0] = r0;
         j.rows[0] = V - r0 < pf_lm_chunk_ ? V - r0 : pf_lm_chunk_;
-        pf_jobs_.push_back(j);
+        jobs.push_back(j);
     }
     for (int b = 0; b < 2; b++) {
-        DCK(cudaMalloc((void **)&pf_w16_[b], need * sizeof(__half)));
-        DCK(cudaEventCreateWithFlags(&pf_expanded_[b], cudaEventDisableTiming));
-        DCK(cudaEventCreateWithFlags(&pf_consumed_[b], cudaEventDisableTiming));
+        DCK(dev_alloc(pf_w16_[b], need));
+        if (!pf_expanded_[b]) DCK(cudaEventCreateWithFlags(&pf_expanded_[b], cudaEventDisableTiming));
+        if (!pf_consumed_[b]) DCK(cudaEventCreateWithFlags(&pf_consumed_[b], cudaEventDisableTiming));
     }
-    pf_w16_elems_ = need;
-    return cudaStreamCreateWithFlags(&pf_side_, cudaStreamNonBlocking);
+    if (!pf_side_) DCK(cudaStreamCreateWithFlags(&pf_side_, cudaStreamNonBlocking));
+    pf_jobs_ = std::move(jobs);  // last: a non-empty job list means the scratch, events and side stream exist
+    return cudaSuccess;
 }
 
 cudaError_t LlamaDecoder::prefill_rows(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, bool score) {
@@ -963,13 +852,13 @@ cudaError_t LlamaDecoder::prefill_rows(int n_seqs, const int *tokens_host, const
     cudaStream_t s = ctx_->stream;
     const int E = cfg_.embed_dim, F = cfg_.hidden_dim, H = cfg_.num_heads, KVH = cfg_.num_kv_heads, hd = cfg_.head_dim;
     const long long Q = (long long)(H + 2 * KVH) * hd;
-    DCK(cudaMemcpyAsync(pf_tok_, tokens_host, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
-    DCK(launch_embedding_rows(ctx_, (const __half *)w_.embed_f16, pf_tok_, pf_x_, n, E));
+    DCK(cudaMemcpyAsync(pf_.tok.get(), tokens_host, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
+    DCK(launch_embedding_rows(ctx_, (const __half *)w_.embed_f16, pf_.tok.get(), pf_.x.get(), n, E));
     AttnPrefillArgs a{};
-    a.qkv = pf_qkv_;
+    a.qkv = pf_.qkv.get();
     a.cos = d_cos_;
     a.sin = d_sin_;
-    a.out = pf_att_;
+    a.out = pf_.att.get();
     a.alpha = cfg_.qk_alpha > 0 ? cfg_.qk_alpha : 1.0f / sqrtf((float)hd);
     a.num_heads = H;
     a.num_kv_heads = KVH;
@@ -979,17 +868,17 @@ cudaError_t LlamaDecoder::prefill_rows(int n_seqs, const int *tokens_host, const
     for (int i = 0, row0 = 0; i < n_seqs; row0 += lengths[i++]) a.seq[i] = AttnPrefillSeq{row0, lengths[i], pos0s[i], nullptr, nullptr};
     for (int l = 0; l < cfg_.num_layers; l++) {
         const tce_llama_layer &L = layers_[l];
-        DCK(launch_rmsnorm_rows_f32(ctx_, pf_x_, L.input_norm, pf_xn_, n, E, cfg_.rms_eps));
-        DCK(prefill_linear(4 * l, pf_xn_, pf_qkv_, Q, n, EPI_STORE_HALF));
+        DCK(launch_rmsnorm_rows_f32(ctx_, pf_.x.get(), L.input_norm, pf_.xn.get(), n, E, cfg_.rms_eps));
+        DCK(prefill_linear(4 * l, pf_.xn.get(), pf_.qkv.get(), Q, n, EPI_STORE_HALF));
         for (int i = 0; i < n_seqs; i++) {
             a.seq[i].k_cache = (__half *)kv_cache_slot(slots[i], l, 0);
             a.seq[i].v_cache = (__half *)kv_cache_slot(slots[i], l, 1);
         }
         DCK(launch_attn_prefill(ctx_, a));
-        DCK(prefill_linear(4 * l + 1, pf_att_, pf_x_, E, n, EPI_ADD_F32));  // residual add in the GEMM epilogue
-        DCK(launch_rmsnorm_rows_f32(ctx_, pf_x_, L.post_norm, pf_xn_, n, E, cfg_.rms_eps));
-        DCK(prefill_linear(4 * l + 2, pf_xn_, pf_act_, F, n, EPI_SILU_MUL_HALF));  // SiLU(gate) * up in the GEMM epilogue: gate|up never reach HBM
-        DCK(prefill_linear(4 * l + 3, pf_act_, pf_x_, E, n, EPI_ADD_F32));
+        DCK(prefill_linear(4 * l + 1, pf_.att.get(), pf_.x.get(), E, n, EPI_ADD_F32));  // residual add in the GEMM epilogue
+        DCK(launch_rmsnorm_rows_f32(ctx_, pf_.x.get(), L.post_norm, pf_.xn.get(), n, E, cfg_.rms_eps));
+        DCK(prefill_linear(4 * l + 2, pf_.xn.get(), pf_.act.get(), F, n, EPI_SILU_MUL_HALF));  // SiLU(gate) * up in the GEMM epilogue: gate|up never reach HBM
+        DCK(prefill_linear(4 * l + 3, pf_.act.get(), pf_.x.get(), E, n, EPI_ADD_F32));
     }
     return cudaSuccess;
 }
@@ -999,24 +888,19 @@ cudaError_t LlamaDecoder::prefill(const int *tokens_host, int n, int pos0, float
         if (err) *err = "prefill is single-GPU in this build (tensor-parallel ranks process the prompt with decode steps)";
         return cudaErrorNotSupported;
     }
-    if (!tokens_host || n < 1 || pos0 < 0 || pos0 + n > cfg_.max_ctx || slot < 0 || slot >= n_slots()) return cudaErrorInvalidValue;
-    for (int i = 0; i < n; i++)
-        if (tokens_host[i] < 0 || tokens_host[i] >= cfg_.vocab_size) return cudaErrorInvalidValue;
+    int rows = 0;
+    DCK(check_prompts(1, tokens_host, &n, &pos0, &slot, &rows));
     DCK(prefill_rows(1, tokens_host, &n, &pos0, &slot));
     cudaStream_t s = ctx_->stream;
     const int E = cfg_.embed_dim;
     // only the last position feeds the sampler: final RMSNorm + lm_head as the decode step's last GEMV, then arg-max
-    DCK(cudaMemcpyAsync(d_resid_, pf_x_ + (size_t)(n - 1) * E, (size_t)E * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    const StepOp *lm = nullptr;
-    for (const StepOp &op : ops_)
-        if (op.type == OP_GEMV) lm = &op;
-    if (!lm) return cudaErrorUnknown;
-    DCK(launch_w4a16_gemv(ctx_, lm->g));
-    DCK(launch_argmax(ctx_, d_logits_, cfg_.vocab_size, d_next_, false));
-    if (logits_host) DCK(cudaMemcpyAsync(h_logits_, d_logits_, (size_t)cfg_.vocab_size * sizeof(float), cudaMemcpyDeviceToHost, s));
-    DCK(cudaMemcpyAsync(h_next_, d_next_, sizeof(int), cudaMemcpyDeviceToHost, s));
+    DCK(cudaMemcpyAsync(d_resid_.get(), pf_.x.get() + (size_t)(n - 1) * E, (size_t)E * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    DCK(launch_w4a16_gemv(ctx_, lm_gemv_));
+    DCK(launch_argmax(ctx_, d_logits_.get(), cfg_.vocab_size, d_next_.get(), false));
+    if (logits_host) DCK(cudaMemcpyAsync(h_logits_.get(), d_logits_.get(), (size_t)cfg_.vocab_size * sizeof(float), cudaMemcpyDeviceToHost, s));
+    DCK(cudaMemcpyAsync(h_next_.get(), d_next_.get(), sizeof(int), cudaMemcpyDeviceToHost, s));
     DCK(cudaStreamSynchronize(s));
-    if (logits_host) memcpy(logits_host, h_logits_, (size_t)cfg_.vocab_size * sizeof(float));
+    if (logits_host) memcpy(logits_host, h_logits_.get(), (size_t)cfg_.vocab_size * sizeof(float));
     if (next_token) *next_token = *h_next_;
     return cudaSuccess;
 }
@@ -1031,19 +915,10 @@ namespace tce {
 
 void LlamaDecoder::drop_batch_graphs() {
     for (int b = 0; b <= TCE_LLAMA_MAX_BATCH; b++) {
-        for (int h = 0; h < 2; h++)
-            if (g_bhost_[h][b]) {
-                cudaGraphExecDestroy(g_bhost_[h][b]);
-                g_bhost_[h][b] = nullptr;
-            }
-        if (g_bdev_[b]) {
-            cudaGraphExecDestroy(g_bdev_[b]);
-            g_bdev_[b] = nullptr;
-        }
-        if (g_bgen_[b]) {
-            cudaGraphExecDestroy(g_bgen_[b]);
-            g_bgen_[b] = nullptr;
-        }
+        g_bhost_[0][b].reset();
+        g_bhost_[1][b].reset();
+        g_bdev_[b].reset();
+        g_bgen_[b].reset();
     }
 }
 
@@ -1053,79 +928,52 @@ cudaError_t LlamaDecoder::batch_alloc(std::string *err) {
         return cudaErrorNotSupported;
     };
     if (tp_ > 1) return no("the batched step is single-GPU (tp_size > 1)");
-    if (d_slot_table_) return cudaSuccess;
+    if (bs_) return cudaSuccess;
     const int nrep = cfg_.num_heads / cfg_.num_kv_heads;
     if (nrep != 1 && nrep != 2 && nrep != 4 && nrep != 8) return no("the batched attention kernel takes 1, 2, 4 or 8 query heads per KV head");
     const int chunk = attn_chunk_ > 0 ? attn_chunk_ : 128;
     const size_t B = TCE_LLAMA_MAX_BATCH, E = cfg_.embed_dim, F = cfg_.hidden_dim, V = cfg_.vocab_size,
                  Q = (size_t)(cfg_.num_heads + 2 * cfg_.num_kv_heads) * cfg_.head_dim, A = (size_t)cfg_.num_heads * cfg_.head_dim;
-    const size_t ws_floats = B * attn_batch_ws_floats(cfg_.num_heads, cfg_.max_ctx, chunk), n_counters = B * cfg_.num_kv_heads;
-    // all or nothing: a failed allocation releases what this call took, so a later call starts from scratch without leaking
-    std::vector<void *> dev, host;
+    // all or nothing: the set is built aside and published whole; a failed allocation frees what this call took
+    std::unique_ptr<BatchState> st = std::make_unique<BatchState>();
+    st->attn_ws_floats = B * attn_batch_ws_floats(cfg_.num_heads, cfg_.max_ctx, chunk);
+    st->n_counters = B * cfg_.num_kv_heads;
+    __half *kv0 = d_kv_.get();
     cudaError_t e = cudaSuccess;
-    auto D = [&](void **p, size_t bytes) {
-        *p = nullptr;
-        if (e == cudaSuccess) e = cudaMalloc(p, bytes);
-        if (e == cudaSuccess) dev.push_back(*p);
+    auto D = [&](auto &p, size_t count) {
+        if (e == cudaSuccess) e = dev_alloc(p, count);
     };
-    auto Hst = [&](void **p, size_t bytes) {
-        *p = nullptr;
-        if (e == cudaSuccess) e = cudaMallocHost(p, bytes);
-        if (e == cudaSuccess) host.push_back(*p);
+    auto Hst = [&](auto &p, size_t count) {
+        if (e == cudaSuccess) e = host_alloc(p, count);
     };
-    float *resid, *logits, *ws;
-    __half *qkv, *attn, *act, **table;
-    int *req, *safe, *next, *hreq, *hnext, *gen;
-    unsigned *counters;
-    float *hlogits;
-    SampleArgs *sample;
-    D((void **)&resid, B * E * sizeof(float));
-    D((void **)&qkv, B * Q * sizeof(__half));
-    D((void **)&attn, B * A * sizeof(__half));
-    D((void **)&act, B * F * sizeof(__half));
-    D((void **)&logits, B * V * sizeof(float));
-    D((void **)&req, B * 3 * sizeof(int));
-    D((void **)&safe, B * 4 * sizeof(int));
-    D((void **)&next, B * sizeof(int));
-    D((void **)&ws, ws_floats * sizeof(float));
-    D((void **)&counters, n_counters * sizeof(unsigned));
-    D((void **)&table, sizeof(__half *));
-    D((void **)&gen, (B * 4 + 2 * B * cfg_.max_ctx) * sizeof(int));
-    D((void **)&sample, B * sizeof(SampleArgs));
-    Hst((void **)&hreq, B * 3 * sizeof(int));
-    Hst((void **)&hnext, B * sizeof(int));
-    Hst((void **)&hlogits, B * V * sizeof(float));
-    if (e == cudaSuccess) e = cudaMemset(logits, 0, B * V * sizeof(float));
-    if (e == cudaSuccess) e = cudaMemset(counters, 0, n_counters * sizeof(unsigned));  // the split merge re-arms them after every use
-    if (e == cudaSuccess) e = cudaMemcpy(table, &d_kv_, sizeof(__half *), cudaMemcpyHostToDevice);
+    D(st->resid, B * E);
+    D(st->qkv, B * Q);
+    D(st->attn, B * A);
+    D(st->act, B * F);
+    D(st->logits, B * V);
+    D(st->req, B * 3);
+    D(st->safe, B * 4);
+    D(st->next, B);
+    D(st->attn_ws, st->attn_ws_floats);
+    D(st->attn_counters, st->n_counters);
+    D(st->slot_table, 1);
+    D(st->gen, B * 4 + 2 * B * cfg_.max_ctx);
+    D(st->sample, B);
+    Hst(st->h_req, B * 3);
+    Hst(st->h_next, B);
+    Hst(st->h_logits, B * V);
+    if (e == cudaSuccess) e = cudaMemset(st->logits.get(), 0, B * V * sizeof(float));
+    if (e == cudaSuccess) e = cudaMemset(st->attn_counters.get(), 0, st->n_counters * sizeof(unsigned));  // the split merge re-arms them after every use
+    if (e == cudaSuccess) e = cudaMemcpy(st->slot_table.get(), &kv0, sizeof(__half *), cudaMemcpyHostToDevice);
     if (e != cudaSuccess) {
-        for (void *p : dev) cudaFree(p);
-        for (void *p : host) cudaFreeHost(p);
         if (err) *err = std::string("batched-step buffers: ") + cudaGetErrorString(e);
         return e;
     }
-    d_bresid_ = resid;
-    d_bqkv_ = qkv;
-    d_battn_ = attn;
-    d_bact_ = act;
-    d_blogits_ = logits;
-    d_breq_ = req;
-    d_bsafe_ = safe;
-    d_bnext_ = next;
-    d_battn_ws_ = ws;
-    battn_ws_floats_ = ws_floats;
-    d_battn_counters_ = counters;
-    battn_counters_ = n_counters;
-    h_breq_ = hreq;
-    h_bnext_ = hnext;
-    h_blogits_ = hlogits;
-    d_bgen_ = gen;
-    d_bsample_ = sample;
-    d_slot_table_ = table;  // last: a non-null table means every buffer above exists
+    bs_ = std::move(st);
     return cudaSuccess;
 }
 
-const float *LlamaDecoder::batch_logits() { return batch_alloc(nullptr) == cudaSuccess ? d_blogits_ : nullptr; }
+const float *LlamaDecoder::batch_logits() { return batch_alloc(nullptr) == cudaSuccess ? bs_->logits.get() : nullptr; }
 
 cudaError_t LlamaDecoder::reserve_slots(int n, std::string *err) {
     if (tp_ > 1) return batch_alloc(err);  // not supported, with its message
@@ -1137,35 +985,29 @@ cudaError_t LlamaDecoder::reserve_slots(int n, std::string *err) {
     DCK(cudaStreamSynchronize(cap_stream_));
     // all or nothing: the new slots and the table that lists them are built aside and only then published, so the slot count and the
     // device table always agree (a failed call leaves both as they were)
-    const size_t kv_bytes = (size_t)cfg_.num_layers * 2 * cfg_.num_kv_heads * cfg_.max_ctx * cfg_.head_dim * sizeof(__half);
-    std::vector<__half *> added;
-    __half **table = nullptr;
-    cudaError_t e = cudaSuccess;
-    while (e == cudaSuccess && n_slots() + (int)added.size() < n) {
-        __half *p = nullptr;
-        e = cudaMalloc((void **)&p, kv_bytes);
-        if (e == cudaSuccess) {
-            added.push_back(p);
-            e = cudaMemset(p, 0, kv_bytes);
-        }
-    }
+    const size_t kv_elems = (size_t)cfg_.num_layers * 2 * cfg_.num_kv_heads * cfg_.max_ctx * cfg_.head_dim;
+    std::vector<DevPtr<__half>> added;
+    DevPtr<__half *> table;
     std::vector<__half *> h;
-    h.push_back(d_kv_);
-    h.insert(h.end(), slot_kv_.begin(), slot_kv_.end());
-    h.insert(h.end(), added.begin(), added.end());
-    if (e == cudaSuccess) e = cudaMalloc((void **)&table, h.size() * sizeof(__half *));
-    if (e == cudaSuccess) e = cudaMemcpy(table, h.data(), h.size() * sizeof(__half *), cudaMemcpyHostToDevice);
+    h.push_back(d_kv_.get());
+    for (const DevPtr<__half> &p : slot_kv_) h.push_back(p.get());
+    cudaError_t e = cudaSuccess;
+    while (e == cudaSuccess && (int)h.size() < n) {
+        added.emplace_back();
+        e = dev_alloc(added.back(), kv_elems);
+        if (e == cudaSuccess) e = cudaMemset(added.back().get(), 0, kv_elems * sizeof(__half));
+        h.push_back(added.back().get());
+    }
+    if (e == cudaSuccess) e = dev_alloc(table, h.size());
+    if (e == cudaSuccess) e = cudaMemcpy(table.get(), h.data(), h.size() * sizeof(__half *), cudaMemcpyHostToDevice);
     if (e != cudaSuccess) {
         cudaGetLastError();
-        for (__half *p : added) cudaFree(p);
-        cudaFree(table);
         if (err) *err = std::string("slot allocation: ") + cudaGetErrorString(e);
         return e;
     }
     drop_batch_graphs();  // they hold the old table and slot count
-    cudaFree(d_slot_table_);
-    d_slot_table_ = table;
-    slot_kv_.insert(slot_kv_.end(), added.begin(), added.end());
+    bs_->slot_table = std::move(table);
+    for (DevPtr<__half> &p : added) slot_kv_.push_back(std::move(p));
     return cudaSuccess;
 }
 
@@ -1187,11 +1029,11 @@ cudaError_t LlamaDecoder::enqueue_batch(int batch, const int *req, cudaStream_t 
     Ctx *c = &local;
     // single-sequence buffer -> its [8][.] batched counterpart and row pitch
     auto widen = [&](const void *p, int *ld) -> void * {
-        if (p == d_resid_) return *ld = E, d_bresid_;
-        if (p == d_qkv_) return *ld = Q, d_bqkv_;
-        if (p == d_attn_) return *ld = A, d_battn_;
-        if (p == d_act_) return *ld = F, d_bact_;
-        if (p == d_logits_) return *ld = V, d_blogits_;
+        if (p == d_resid_.get()) return *ld = E, bs_->resid.get();
+        if (p == d_qkv_.get()) return *ld = Q, bs_->qkv.get();
+        if (p == d_attn_.get()) return *ld = A, bs_->attn.get();
+        if (p == d_act_.get()) return *ld = F, bs_->act.get();
+        if (p == d_logits_.get()) return *ld = V, bs_->logits.get();
         return nullptr;
     };
     bool first = true;
@@ -1199,7 +1041,8 @@ cudaError_t LlamaDecoder::enqueue_batch(int batch, const int *req, cudaStream_t 
         const bool use_pdl = pdl && !first;
         switch (op.type) {
             case OP_EMBED:
-                DCK(launch_embedding_batch(c, (const __half *)w_.embed_f16, req, d_bresid_, E, batch, V, cfg_.max_ctx, n_slots(), d_bsafe_, use_pdl));
+                DCK(launch_embedding_batch(c, (const __half *)w_.embed_f16, req, bs_->resid.get(), E, batch, V, cfg_.max_ctx, n_slots(), bs_->safe.get(),
+                                           use_pdl));
                 break;
             case OP_GEMV: {
                 W4GemvParams p = op.g;
@@ -1214,23 +1057,23 @@ cudaError_t LlamaDecoder::enqueue_batch(int batch, const int *req, cudaStream_t 
             case OP_ATTN: {
                 AttnBatchArgs b{};
                 b.base = op.at;
-                b.base.qkv = d_bqkv_;
-                b.base.out = d_battn_;
-                b.base.ws = d_battn_ws_;
-                b.base.counters = d_battn_counters_;
-                b.ws_floats = battn_ws_floats_;
-                b.n_counters = battn_counters_;
-                b.req = d_bsafe_;
-                b.slots = d_slot_table_;
-                b.k_off = op.at.k_cache - d_kv_;  // this layer's slabs within a slot
-                b.v_off = op.at.v_cache - d_kv_;
+                b.base.qkv = bs_->qkv.get();
+                b.base.out = bs_->attn.get();
+                b.base.ws = bs_->attn_ws.get();
+                b.base.counters = bs_->attn_counters.get();
+                b.ws_floats = bs_->attn_ws_floats;
+                b.n_counters = bs_->n_counters;
+                b.req = bs_->safe.get();
+                b.slots = bs_->slot_table.get();
+                b.k_off = op.at.k_cache - d_kv_.get();  // this layer's slabs within a slot
+                b.v_off = op.at.v_cache - d_kv_.get();
                 b.qkv_stride = Q;
                 b.out_stride = A;
                 DCK(launch_attn_decode_batch(c, b, batch, use_pdl));
                 break;
             }
             case OP_ARGMAX:
-                DCK(launch_argmax_rows(c, d_blogits_, batch, V, d_bnext_, use_pdl));
+                DCK(launch_argmax_rows(c, bs_->logits.get(), batch, V, bs_->next.get(), use_pdl));
                 break;
             default:
                 return cudaErrorNotSupported;
@@ -1240,115 +1083,56 @@ cudaError_t LlamaDecoder::enqueue_batch(int batch, const int *req, cudaStream_t 
     return cudaSuccess;
 }
 
-namespace {
-// capture `body` on `s` into an executable graph: with programmatic edges first, plain edges if the driver refuses them
-template <typename Body>
-cudaError_t capture_graph(cudaStream_t s, bool pdl, Body body, cudaGraphExec_t *out) {
-    for (int attempt = pdl ? 0 : 1; attempt < 2; attempt++) {
-        cudaGraph_t g = nullptr;
-        cudaError_t e = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal);
-        if (e != cudaSuccess) return e;
-        e = body(attempt == 0);
-        cudaError_t e2 = cudaStreamEndCapture(s, &g);
-        if (e == cudaSuccess) e = e2;
-        if (e == cudaSuccess) e = cudaGraphInstantiate(out, g, 0);
-        if (g) cudaGraphDestroy(g);
-        if (e == cudaSuccess) return e;
-        cudaGetLastError();
-        *out = nullptr;
-        if (attempt == 1) return e;
-    }
-    return cudaErrorUnknown;
-}
-}  // namespace
-
 cudaError_t LlamaDecoder::decode_batch_device(int batch, const int *req_dev, std::string *err) {
     if (tp_ > 1) return batch_alloc(err);  // not supported, with its message
     if (batch < 1 || batch > TCE_LLAMA_MAX_BATCH || !req_dev) return cudaErrorInvalidValue;
     DCK(batch_alloc(err));
-    cudaStream_t s = ctx_->stream;
-    if (!use_graphs_) return enqueue_batch(batch, req_dev, s, ctx_->use_pdl);
-    cudaGraphExec_t &g = g_bdev_[batch];
-    if (g && (g_bdev_src_[batch] != req_dev || g_bdev_gen_[batch] != ctx_->option_gen)) {
-        cudaGraphExecDestroy(g);
-        g = nullptr;
-    }
-    if (!g) {
-        // one eager step first, outside of capture (module loads, kernel attributes); re-running a step rewrites the same K/V rows
-        DCK(cudaStreamSynchronize(s));
-        DCK(enqueue_batch(batch, req_dev, cap_stream_, false));
-        DCK(cudaStreamSynchronize(cap_stream_));
-        cudaError_t e = capture_graph(cap_stream_, ctx_->use_pdl, [&](bool pdl) { return enqueue_batch(batch, req_dev, cap_stream_, pdl); }, &g);
-        if (e != cudaSuccess) {
-            if (err) *err = std::string("batched graph capture failed: ") + cudaGetErrorString(e);
-            return e;
-        }
-        g_bdev_src_[batch] = req_dev;
-        g_bdev_gen_[batch] = ctx_->option_gen;
-    }
-    return cudaGraphLaunch(g, s);
+    return run_graphed(g_bdev_[batch], req_dev, [&](cudaStream_t st, bool pdl) { return enqueue_batch(batch, req_dev, st, pdl); });
 }
 
 cudaError_t LlamaDecoder::decode_batch_host(int batch, const int *tokens, const int *positions, const int *slots, float *logits_host, int *next_tokens,
                                             std::string *err) {
     if (tp_ > 1) return batch_alloc(err);  // not supported, with its message
-    if (batch < 1 || batch > TCE_LLAMA_MAX_BATCH || !tokens || !positions || !slots) return cudaErrorInvalidValue;
-    for (int b = 0; b < batch; b++) {
-        if (tokens[b] < 0 || tokens[b] >= cfg_.vocab_size || positions[b] < 0 || positions[b] >= cfg_.max_ctx || slots[b] < 0 || slots[b] >= n_slots())
-            return cudaErrorInvalidValue;
-        for (int o = 0; o < b; o++)
-            if (slots[o] == slots[b]) return cudaErrorInvalidValue;
-    }
+    if (batch < 1 || batch > TCE_LLAMA_MAX_BATCH || !tokens || !positions || !slots || !slots_ok(batch, slots)) return cudaErrorInvalidValue;
+    for (int b = 0; b < batch; b++)
+        if (tokens[b] < 0 || tokens[b] >= cfg_.vocab_size || positions[b] < 0 || positions[b] >= cfg_.max_ctx) return cudaErrorInvalidValue;
     DCK(batch_alloc(err));
+    int *h_req = bs_->h_req.get();
     for (int b = 0; b < batch; b++) {
-        h_breq_[3 * b] = tokens[b];
-        h_breq_[3 * b + 1] = positions[b];
-        h_breq_[3 * b + 2] = slots[b];
+        h_req[3 * b] = tokens[b];
+        h_req[3 * b + 1] = positions[b];
+        h_req[3 * b + 2] = slots[b];
     }
     const int want = logits_host ? 1 : 0;
     const size_t lbytes = (size_t)batch * cfg_.vocab_size * sizeof(float);
-    cudaStream_t s = ctx_->stream;
-    auto body = [&](cudaStream_t st, bool pdl) {
-        cudaError_t e = cudaMemcpyAsync(d_breq_, h_breq_, (size_t)batch * 3 * sizeof(int), cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = enqueue_batch(batch, d_breq_, st, pdl);
-        if (e == cudaSuccess && want) e = cudaMemcpyAsync(h_blogits_, d_blogits_, lbytes, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(h_bnext_, d_bnext_, (size_t)batch * sizeof(int), cudaMemcpyDeviceToHost, st);
-        return e;
-    };
-    cudaGraphExec_t &g = g_bhost_[want][batch];
-    if (g && g_bhost_gen_[want][batch] != ctx_->option_gen) {  // an option or the stream changed since capture
-        cudaGraphExecDestroy(g);
-        g = nullptr;
-    }
-    if (use_graphs_ && !g) {
-        DCK(cudaStreamSynchronize(s));
-        DCK(body(cap_stream_, false));  // eager step outside of capture; re-running it rewrites the same K/V rows
-        DCK(cudaStreamSynchronize(cap_stream_));
-        cudaError_t e = capture_graph(cap_stream_, ctx_->use_pdl, [&](bool pdl) { return body(cap_stream_, pdl); }, &g);
-        if (e != cudaSuccess) {
-            if (err) *err = std::string("batched graph capture failed: ") + cudaGetErrorString(e);
-            return e;
-        }
-        g_bhost_gen_[want][batch] = ctx_->option_gen;
-    }
-    if (use_graphs_)
-        DCK(cudaGraphLaunch(g, s));
-    else
-        DCK(body(s, ctx_->use_pdl));
-    DCK(cudaStreamSynchronize(s));
-    if (logits_host) memcpy(logits_host, h_blogits_, lbytes);
-    if (next_tokens) memcpy(next_tokens, h_bnext_, (size_t)batch * sizeof(int));
+    DCK(run_graphed(g_bhost_[want][batch], nullptr, [&](cudaStream_t st, bool pdl) {
+        DCK(cudaMemcpyAsync(bs_->req.get(), h_req, (size_t)batch * 3 * sizeof(int), cudaMemcpyHostToDevice, st));
+        DCK(enqueue_batch(batch, bs_->req.get(), st, pdl));
+        if (want) DCK(cudaMemcpyAsync(bs_->h_logits.get(), bs_->logits.get(), lbytes, cudaMemcpyDeviceToHost, st));
+        return cudaMemcpyAsync(bs_->h_next.get(), bs_->next.get(), (size_t)batch * sizeof(int), cudaMemcpyDeviceToHost, st);
+    }));
+    DCK(cudaStreamSynchronize(ctx_->stream));
+    if (logits_host) memcpy(logits_host, bs_->h_logits.get(), lbytes);
+    if (next_tokens) memcpy(next_tokens, bs_->h_next.get(), (size_t)batch * sizeof(int));
     return cudaSuccess;
 }
 
 // ------------------------------------------------------------------------------------------------ batched prompt pass and generate loop
+bool LlamaDecoder::slots_ok(int n, const int *slots) const {
+    for (int b = 0; b < n; b++) {
+        if (slots[b] < 0 || slots[b] >= n_slots()) return false;
+        for (int o = 0; o < b; o++)
+            if (slots[o] == slots[b]) return false;
+    }
+    return true;
+}
+
 cudaError_t LlamaDecoder::check_prompts(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, int *n) const {
-    if (n_seqs < 1 || n_seqs > TCE_LLAMA_MAX_BATCH || !tokens_host || !lengths || !pos0s || !slots) return cudaErrorInvalidValue;
+    if (n_seqs < 1 || n_seqs > TCE_LLAMA_MAX_BATCH || !tokens_host || !lengths || !pos0s || !slots || !slots_ok(n_seqs, slots))
+        return cudaErrorInvalidValue;
     int rows = 0;
     for (int b = 0; b < n_seqs; b++) {
-        if (lengths[b] < 1 || pos0s[b] < 0 || pos0s[b] > cfg_.max_ctx - lengths[b] || slots[b] < 0 || slots[b] >= n_slots()) return cudaErrorInvalidValue;
-        for (int o = 0; o < b; o++)
-            if (slots[o] == slots[b]) return cudaErrorInvalidValue;
+        if (lengths[b] < 1 || pos0s[b] < 0 || pos0s[b] > cfg_.max_ctx - lengths[b]) return cudaErrorInvalidValue;
         rows += lengths[b];
     }
     for (int i = 0; i < rows; i++)
@@ -1369,46 +1153,38 @@ cudaError_t LlamaDecoder::prefill_batch(int n_seqs, const int *tokens_host, cons
     // the last row of each prompt becomes row b of the batched step's residual: final RMSNorm + lm_head as that step's GEMV (M = n_seqs)
     for (int b = 0, row = 0; b < n_seqs; b++) {
         row += lengths[b];
-        DCK(cudaMemcpyAsync(d_bresid_ + (size_t)b * E, pf_x_ + (size_t)(row - 1) * E, (size_t)E * sizeof(float), cudaMemcpyDeviceToDevice, s));
+        DCK(cudaMemcpyAsync(bs_->resid.get() + (size_t)b * E, pf_.x.get() + (size_t)(row - 1) * E, (size_t)E * sizeof(float), cudaMemcpyDeviceToDevice, s));
     }
-    const StepOp *lm = nullptr;
-    for (const StepOp &op : ops_)
-        if (op.type == OP_GEMV) lm = &op;
-    if (!lm) return cudaErrorUnknown;
-    W4GemvParams p = lm->g;
+    W4GemvParams p = lm_gemv_;
     p.M = n_seqs;
-    p.x = d_bresid_;
+    p.x = bs_->resid.get();
     p.ldx = E;
-    p.y = d_blogits_;
+    p.y = bs_->logits.get();
     p.ldy = V;
     p.pdl = false;
     DCK(launch_w4a16_gemv(ctx_, p));
-    DCK(launch_argmax_rows(ctx_, d_blogits_, n_seqs, V, d_bnext_, false));
-    if (logits_host) DCK(cudaMemcpyAsync(h_blogits_, d_blogits_, (size_t)n_seqs * V * sizeof(float), cudaMemcpyDeviceToHost, s));
-    DCK(cudaMemcpyAsync(h_bnext_, d_bnext_, (size_t)n_seqs * sizeof(int), cudaMemcpyDeviceToHost, s));
+    DCK(launch_argmax_rows(ctx_, bs_->logits.get(), n_seqs, V, bs_->next.get(), false));
+    if (logits_host) DCK(cudaMemcpyAsync(bs_->h_logits.get(), bs_->logits.get(), (size_t)n_seqs * V * sizeof(float), cudaMemcpyDeviceToHost, s));
+    DCK(cudaMemcpyAsync(bs_->h_next.get(), bs_->next.get(), (size_t)n_seqs * sizeof(int), cudaMemcpyDeviceToHost, s));
     DCK(cudaStreamSynchronize(s));
-    if (logits_host) memcpy(logits_host, h_blogits_, (size_t)n_seqs * V * sizeof(float));
-    if (next_tokens) memcpy(next_tokens, h_bnext_, (size_t)n_seqs * sizeof(int));
+    if (logits_host) memcpy(logits_host, bs_->h_logits.get(), (size_t)n_seqs * V * sizeof(float));
+    if (next_tokens) memcpy(next_tokens, bs_->h_next.get(), (size_t)n_seqs * sizeof(int));
     return cudaSuccess;
 }
 
 // ------------------------------------------------------------------------------------------------ teacher-forced scoring
 cudaError_t LlamaDecoder::score_reserve(int n) {
-    if (n <= sc_cap_) return cudaSuccess;
+    if (n <= sc_.cap) return cudaSuccess;
     DCK(cudaStreamSynchronize(ctx_->stream));
-    cudaFree(sc_rec_);
-    cudaFree(sc_state_);
-    cudaFree(sc_target_);
-    cudaFree(sc_tgt_);
-    cudaFree(sc_out_);
-    sc_rec_ = nullptr; sc_state_ = nullptr; sc_target_ = nullptr; sc_tgt_ = nullptr; sc_out_ = nullptr;
-    sc_cap_ = 0;
-    DCK(cudaMalloc(&sc_rec_, (size_t)n * (pf_lm_chunk_ / 128) * sizeof(LmStat)));
-    DCK(cudaMalloc(&sc_state_, (size_t)n * sizeof(LmStat)));
-    DCK(cudaMalloc(&sc_target_, (size_t)n * sizeof(int)));
-    DCK(cudaMalloc(&sc_tgt_, (size_t)n * sizeof(float)));
-    DCK(cudaMalloc(&sc_out_, (size_t)3 * n * sizeof(float)));
-    sc_cap_ = n;
+    sc_ = ScoreBufs{};  // the old buffers go first
+    ScoreBufs b;
+    DCK(dev_alloc(b.rec, (size_t)n * (pf_lm_chunk_ / 128)));
+    DCK(dev_alloc(b.state, (size_t)n));
+    DCK(dev_alloc(b.target, (size_t)n));
+    DCK(dev_alloc(b.tgt, (size_t)n));
+    DCK(dev_alloc(b.out, (size_t)3 * n));
+    b.cap = n;
+    sc_ = std::move(b);
     return cudaSuccess;
 }
 
@@ -1440,19 +1216,20 @@ cudaError_t LlamaDecoder::score_batch(int n_seqs, const int *tokens_host, const 
     DCK(score_reserve(n));
     DCK(prefill_rows(n_seqs, tokens_host, lengths, pos0s, slots, true));
     cudaStream_t s = ctx_->stream;
-    DCK(cudaMemcpyAsync(sc_target_, target.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
-    DCK(launch_rmsnorm_rows_f32(ctx_, pf_x_, w_.final_norm, pf_xn_, n, E, cfg_.rms_eps));
-    float *logprob = sc_out_, *glp = sc_out_ + 2 * (size_t)n;
-    int *greedy = reinterpret_cast<int *>(sc_out_ + n);
+    DCK(cudaMemcpyAsync(sc_.target.get(), target.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
+    DCK(launch_rmsnorm_rows_f32(ctx_, pf_.x.get(), w_.final_norm, pf_.xn.get(), n, E, cfg_.rms_eps));
+    float *logprob = sc_.out.get(), *glp = sc_.out.get() + 2 * (size_t)n;
+    int *greedy = reinterpret_cast<int *>(sc_.out.get() + n);
     const int rec_ld = pf_lm_chunk_ / 128, first = 4 * cfg_.num_layers;
     for (int j = first; j < pf_njobs_; j++) {
         const PfJob &job = pf_jobs_[j];
         const __half *w16 = nullptr;
         DCK(pf_job_begin(j, &w16));
-        DCK(launch_gemm_f16_pair_stats(ctx_, pf_xn_, E, w16, E, n, job.rows[0], E, job.r0[0], sc_rec_, rec_ld, sc_target_, sc_tgt_, logits_dev, V));
+        DCK(launch_gemm_f16_pair_stats(ctx_, pf_.xn.get(), E, w16, E, n, job.rows[0], E, job.r0[0], sc_.rec.get(), rec_ld, sc_.target.get(), sc_.tgt.get(),
+                                       logits_dev, V));
         DCK(cudaEventRecord(pf_consumed_[j & 1], s));
-        DCK(launch_lm_stats_merge(ctx_, sc_rec_, rec_ld, (job.rows[0] + 127) / 128, n, j == first, j + 1 == pf_njobs_, sc_state_, sc_target_, sc_tgt_,
-                                  logprob, greedy, glp));
+        DCK(launch_lm_stats_merge(ctx_, sc_.rec.get(), rec_ld, (job.rows[0] + 127) / 128, n, j == first, j + 1 == pf_njobs_, sc_.state.get(),
+                                  sc_.target.get(), sc_.tgt.get(), logprob, greedy, glp));
     }
     if (logprobs_host) DCK(cudaMemcpyAsync(logprobs_host, logprob, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, s));
     if (greedy_host) DCK(cudaMemcpyAsync(greedy_host, greedy, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -1460,7 +1237,7 @@ cudaError_t LlamaDecoder::score_batch(int n_seqs, const int *tokens_host, const 
     return cudaStreamSynchronize(s);
 }
 
-// The generate loop of `generate` for up to TCE_LLAMA_MAX_BATCH sequences: every token is one batched step on the request buffer d_breq_ and
+// The generate loop of `generate` for up to TCE_LLAMA_MAX_BATCH sequences: every token is one batched step on the request buffer bs_->req and
 // one sampler launch with a block per row, which writes each row's next {token, position} into that buffer.  A row that stops gets an
 // out-of-range position there, so the batched embedding refuses it and it appends no KV row in any later step.  Stopped rows still ride
 // along as rows of the GEMVs.
@@ -1468,29 +1245,29 @@ cudaError_t LlamaDecoder::generate_batch(int batch, const tce_gen_request *reqs,
     if (tp_ > 1) return batch_alloc(err);  // not supported, with its message
     if (batch < 1 || batch > TCE_LLAMA_MAX_BATCH || !reqs || !n_out || out_stride < 0) return cudaErrorInvalidValue;
     const int cap = cfg_.max_ctx, V = cfg_.vocab_size, B = TCE_LLAMA_MAX_BATCH;
-    int n_pred[TCE_LLAMA_MAX_BATCH], steps = 0;
+    int n_pred[TCE_LLAMA_MAX_BATCH], slots[TCE_LLAMA_MAX_BATCH], steps = 0;
     for (int b = 0; b < batch; b++) {
         const tce_gen_request &r = reqs[b];
-        if (r.slot < 0 || r.slot >= n_slots() || r.first_token < 0 || r.first_token >= V || r.pos0 < 0 || r.pos0 >= cap || r.n_predict < 0 ||
-            r.n_history < 0 || r.n_history > cap || (r.n_history > 0 && !r.history))
+        if (r.first_token < 0 || r.first_token >= V || r.pos0 < 0 || r.pos0 >= cap || r.n_predict < 0 || r.n_history < 0 || r.n_history > cap ||
+            (r.n_history > 0 && !r.history))
             return cudaErrorInvalidValue;
-        for (int o = 0; o < b; o++)
-            if (reqs[o].slot == r.slot) return cudaErrorInvalidValue;
+        slots[b] = r.slot;
         n_pred[b] = r.n_predict < cap - r.pos0 ? r.n_predict : cap - r.pos0;
         if (out_stride < n_pred[b]) return cudaErrorInvalidValue;
         steps = n_pred[b] > steps ? n_pred[b] : steps;
     }
-    if (steps > 0 && !out_tokens_host) return cudaErrorInvalidValue;
+    if (!slots_ok(batch, slots) || (steps > 0 && !out_tokens_host)) return cudaErrorInvalidValue;
     for (int b = 0; b < batch; b++) {
         const tce_sampling &sc = reqs[b].sampling;
-        if (sc.temp > 0.f && (sc.top_k <= 0 || sc.top_k > 1024) && V > 1024) {
+        if (!sampling_supported(sc.temp, sc.top_k, V)) {
             if (err) *err = "generate: temp > 0 needs 1 <= top_k <= 1024";
             return cudaErrorNotSupported;
         }
     }
     DCK(batch_alloc(err));
     cudaStream_t s = ctx_->stream;
-    int *ctl = d_bgen_, *hist = d_bgen_ + 4 * B, *out_list = hist + (size_t)B * cap;  // per row: {history head, output count, stop flag, unused}
+    int *ctl = bs_->gen.get(), *hist = bs_->gen.get() + 4 * B, *out_list = hist + (size_t)B * cap;  // per row: {history head, output count, stop flag, unused}
+    int *h_req = bs_->h_req.get();
     int ctl_h[4 * TCE_LLAMA_MAX_BATCH] = {};
     SampleArgs args[TCE_LLAMA_MAX_BATCH];
     for (int b = 0; b < batch; b++) {
@@ -1499,27 +1276,16 @@ cudaError_t LlamaDecoder::generate_batch(int batch, const tce_gen_request *reqs,
             DCK(cudaMemcpyAsync(hist + (size_t)b * cap, r.history, (size_t)r.n_history * sizeof(int), cudaMemcpyHostToDevice, s));
         ctl_h[4 * b] = r.n_history;
         ctl_h[4 * b + 2] = n_pred[b] == 0;  // nothing to generate: stopped from the start
-        h_breq_[3 * b] = r.first_token;
-        h_breq_[3 * b + 1] = n_pred[b] == 0 ? cap : r.pos0;
-        h_breq_[3 * b + 2] = r.slot;
+        h_req[3 * b] = r.first_token;
+        h_req[3 * b + 1] = n_pred[b] == 0 ? cap : r.pos0;
+        h_req[3 * b + 2] = r.slot;
         SampleArgs &a = args[b];
-        a = SampleArgs{};
-        a.logits = d_blogits_ + (size_t)b * V;
-        a.n_vocab = V;
-        a.top_k = r.sampling.top_k;
-        a.top_p = r.sampling.top_p;
-        a.temp = r.sampling.temp;
-        a.repeat_penalty = r.sampling.repeat_penalty;
-        a.frequency_penalty = r.sampling.frequency_penalty;
-        a.presence_penalty = r.sampling.presence_penalty;
-        a.repeat_last_n = r.sampling.repeat_last_n;
-        a.seed = r.sampling.seed;
-        a.draw_index = 0;
+        a = sample_args(r.sampling, bs_->logits.get() + (size_t)b * V, V);
         a.hist = hist + (size_t)b * cap;
         a.hist_head = ctl + 4 * b;
         a.hist_cap = cap;
         a.eos_id = r.eos_id;
-        a.tokpos = d_breq_ + 3 * b;
+        a.tokpos = bs_->req.get() + 3 * b;
         a.out_list = out_list + (size_t)b * cap;
         a.out_count = ctl + 4 * b + 1;
         a.out_cap = cap;
@@ -1528,33 +1294,15 @@ cudaError_t LlamaDecoder::generate_batch(int batch, const tce_gen_request *reqs,
         a.pos_limit = cap;
     }
     DCK(cudaMemcpyAsync(ctl, ctl_h, (size_t)4 * batch * sizeof(int), cudaMemcpyHostToDevice, s));
-    DCK(cudaMemcpyAsync(d_bsample_, args, (size_t)batch * sizeof(SampleArgs), cudaMemcpyHostToDevice, s));
-    DCK(cudaMemcpyAsync(d_breq_, h_breq_, (size_t)batch * 3 * sizeof(int), cudaMemcpyHostToDevice, s));
+    DCK(cudaMemcpyAsync(bs_->sample.get(), args, (size_t)batch * sizeof(SampleArgs), cudaMemcpyHostToDevice, s));
+    DCK(cudaMemcpyAsync(bs_->req.get(), h_req, (size_t)batch * 3 * sizeof(int), cudaMemcpyHostToDevice, s));
     auto body = [&](cudaStream_t st, bool pdl) {
-        cudaError_t e = enqueue_batch(batch, d_breq_, st, pdl);
-        if (e == cudaSuccess) e = launch_sample_rows(d_bsample_, batch, st);
-        return e;
+        DCK(enqueue_batch(batch, bs_->req.get(), st, pdl));
+        return launch_sample_rows(bs_->sample.get(), batch, st);
     };
-    cudaGraphExec_t &g = g_bgen_[batch];
-    if (g && g_bgen_gen_[batch] != ctx_->option_gen) {  // an option or the stream changed since capture
-        cudaGraphExecDestroy(g);
-        g = nullptr;
-    }
     constexpr int kCheckEvery = 16;
     for (int i = 0; i < steps; i++) {
-        if (use_graphs_ && !g && i > 0) {
-            // captured after one eager token (modules loaded, kernel attributes set, GEMV fix-up records grown); capture runs nothing
-            cudaError_t e = capture_graph(cap_stream_, ctx_->use_pdl, [&](bool pdl) { return body(cap_stream_, pdl); }, &g);
-            if (e != cudaSuccess) {
-                if (err) *err = std::string("batched generate graph capture failed: ") + cudaGetErrorString(e);
-                return e;
-            }
-            g_bgen_gen_[batch] = ctx_->option_gen;
-        }
-        if (use_graphs_ && g)
-            DCK(cudaGraphLaunch(g, s));
-        else
-            DCK(body(s, ctx_->use_pdl));
+        DCK(run_graphed(g_bgen_[batch], nullptr, body));
         if ((i + 1) % kCheckEvery == 0 && i + 1 < steps) {
             DCK(cudaMemcpyAsync(ctl_h, ctl, (size_t)4 * batch * sizeof(int), cudaMemcpyDeviceToHost, s));
             DCK(cudaStreamSynchronize(s));

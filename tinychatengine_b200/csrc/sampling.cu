@@ -13,6 +13,7 @@
 // Selection of the k largest logits: three histogram passes (11 + 11 + 10 bits of the order-preserving key) find the key of the k-th
 // largest, one ordered compaction pass gathers the candidates (ties at the threshold: lowest ids first), one bitonic sort orders them
 // (logit descending, id ascending).  Everything after that is O(k) work on shared memory.
+#include "../../include/tce_b200.h"
 #include "common.cuh"
 #include "kernels.h"
 #include "kernels_attn.h"
@@ -305,9 +306,27 @@ cudaError_t launch_sample_rows(const SampleArgs *rows_dev, int rows, cudaStream_
     return cudaGetLastError();
 }
 
+SampleArgs sample_args(const tce_sampling &sc, float *logits, int n_vocab) {
+    SampleArgs a{};
+    a.logits = logits;
+    a.n_vocab = n_vocab;
+    a.top_k = sc.top_k;
+    a.top_p = sc.top_p;
+    a.temp = sc.temp;
+    a.repeat_penalty = sc.repeat_penalty;
+    a.frequency_penalty = sc.frequency_penalty;
+    a.presence_penalty = sc.presence_penalty;
+    a.repeat_last_n = sc.repeat_last_n;
+    a.seed = sc.seed;
+    a.draw_index = 0;
+    return a;
+}
+
+bool sampling_supported(float temp, int top_k, int n_vocab) { return !(temp > 0.f && (top_k <= 0 || top_k > kMaxK) && n_vocab > kMaxK); }
+
 cudaError_t launch_sample(Ctx *ctx, const SampleArgs &a, cudaStream_t stream) {
     if (!a.logits || a.n_vocab < 1) return cudaErrorInvalidValue;
-    if (a.temp > 0.f && (a.top_k <= 0 || a.top_k > kMaxK) && a.n_vocab > kMaxK) return cudaErrorNotSupported;
+    if (!sampling_supported(a.temp, a.top_k, a.n_vocab)) return cudaErrorNotSupported;
     (void)ctx;
     sample_kernel<<<1, kSampleThreads, 0, stream>>>(a);
     return cudaGetLastError();
