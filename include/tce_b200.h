@@ -117,6 +117,8 @@ TCE_API int tce_attn_prefill(tce_ctx *ctx, void *qkv, void *k_cache, void *v_cac
 /* ---- small ops either side of the path -------------------------------------------------------------------
  * LlamaRMSNorm_cuda::forward (llm/src/ops/cuda/LlamaRMSNorm.cu:96-115): half in/out, fp32 gamma             */
 TCE_API int tce_rmsnorm_f16(tce_ctx *ctx, const void *x, const float *gamma, void *y, int rows, int dim, float eps);
+/* device int *out = index of the first maximum of device float x[n] (arg_max.cc); an input with no value greater than -inf (all -inf
+ * or NaN) gives 0 */
 TCE_API int tce_argmax_f32(tce_ctx *ctx, const float *x, int n, int *out);
 /* LayerNormQ::forward (llm/src/ops/LayerNormQ.cc:12-52): fp32 [rows][dim] -> int8 [rows][dim], eps 1e-5, std::round.  Bit-exact: the two
  * row sums run serially in the reference's order (the int8 result depends on their last bit near rounding ties).            */
@@ -172,7 +174,8 @@ TCE_API int tce_llama_load_dir(tce_ctx *ctx, const char *dir, const tce_llama_co
  * [oc][ic/32], zero point 8) -> QM_CUDA op arrays (w uint32 [oc][ic/8], scales fp16 [oc][zeros_w*8], zeros uint32 [oc][zeros_w]) on the HOST:
  * exact dequantisation followed by the QM_CUDA quantisation rule (group 128).  Lossy by construction (32- vs 128-channel scales).  */
 TCE_API int tce_w4_import_x86(const void *qs_u8, const float *scales_f32, int oc, int ic, void *w_out, void *scales_f16_out, void *zeros_out);
-/* inputs resident: tokpos = device int[2] {token id, position}; logits stay on the device */
+/* inputs resident: tokpos = device int[2] {token id, position}; logits stay on the device.  The pair is range-checked on the device, on
+ * the persistent kernel and on the kernel-per-op step alike: a token or position out of range is refused and writes no KV row. */
 TCE_API int tce_llama_decode(tce_llama *m, const int *tokpos_dev);
 /* end to end: token/pos from the host, fp32 logits[vocab] copied back to `logits_host` (may be NULL) and the
  * greedy arg-max to *next_token (may be NULL); returns after the copies have completed */
@@ -268,14 +271,17 @@ TCE_API int tce_llama_kernels_per_step(tce_llama *m);
 /* ---- tensor-parallel decode across the GPUs of one box (one process per GPU) --------------------------------
  * cfg.tp_size = P > 1: heads / kv heads / hidden_dim / vocab_size in tce_llama_config are the LOCAL (1/P) sizes and the
  * weights are the local shards (q,k,v,gate,up,lm_head: row shards; o,down: column (input-channel) shards repacked as
- * [E][IC/P]).  The all-reduce after o_proj and down_proj runs over NVLink peer memory inside the GEMV kernels.
+ * [E][IC/P]).  The all-reduce after o_proj and down_proj runs over NVLink peer memory inside the persistent decode kernel, so
+ * tensor parallelism needs that kernel: tce_llama_create refuses tp_size > 1 with TCE_PERSISTENT=0, and tce_llama_tp_connect returns
+ * TCE_ERR_UNSUPPORTED, with the reason, for a local shard outside the kernel's envelope.
  * Setup: every rank exports a 64-byte IPC handle, the host exchanges them (e.g. torch.distributed.all_gather) and
  * every rank connects with the P handles in rank order.  tce_llama_decode_host then returns the local logits shard
  * (float[vocab_local]) and the GLOBAL greedy token; all ranks must call it with the same token/pos sequence.   */
 TCE_API int tce_llama_tp_handle(tce_llama *m, void *handle_out_64_bytes);
 TCE_API int tce_llama_tp_connect(tce_llama *m, const void *handles_P_times_64_bytes);
-/* debugging aid: device pointers of the step's intermediate buffers: 0 residual float[E], 1 qkv half[(H+2KVH)*hd],
- * 2 attention output half[H*hd], 3 SiLU(gate)*up half[F] (values of the LAST layer after a step) */
+/* debugging aid: device pointers of row 0 of the kernel-per-op step's intermediate buffers: 0 residual float[E], 1 qkv half[(H+2KVH)*hd],
+ * 2 attention output half[H*hd], 3 SiLU(gate)*up half[F] (values of the LAST layer after a step); NULL until those buffers exist (the
+ * persistent kernel keeps its intermediates on chip).  4: the persistent kernel's phase timestamps (TCE_PK_DEBUG=1). */
 TCE_API void *tce_llama_debug_buffer(tce_llama *m, int which);
 /* measurement aid: enqueue only the W4A16 GEMV launches of one decode step (4 per layer + lm_head, the same fused
  * kernels with the same arguments) so the dominant kernel can be timed with CUDA events; returns the launch count */

@@ -333,6 +333,21 @@ def test_tensor_parallel_model_is_unsupported():
     ctx.close()
 
 
+def test_tensor_parallel_model_needs_the_persistent_kernel(monkeypatch):
+    """tensor parallelism runs on the persistent kernel only: a tp_size = 2 shard built with TCE_PERSISTENT=0 is refused at creation"""
+    monkeypatch.setenv("TCE_PERSISTENT", "0")
+    from tinychatengine_b200._lib import TceError
+    from tinychatengine_b200.llama import GEOMETRIES, LlamaModel, make_random_weights, shard_weights
+    from tinychatengine_b200.runtime import Context
+
+    ctx = Context(0)
+    g = GEOMETRIES["tiny-gqa"]
+    Wl, gl = shard_weights(make_random_weights(g, torch.device("cuda", 0), 3), g, 0, 2)
+    with pytest.raises(TceError, match="persistent decode kernel"):
+        LlamaModel(ctx, gl, max_ctx=128, weights=Wl, tp_rank=0, tp_size=2)
+    ctx.close()
+
+
 def test_multicolumn_gemv_grows_its_fixup_records():
     """45056 x 11008 at M = 2 takes 2816 row tiles x 6 K-slices of fix-up records, more than a context starts with: the launch grows them"""
     from oracle import capi

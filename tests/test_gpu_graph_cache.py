@@ -76,6 +76,14 @@ def test_single_sequence_graphs_match_eager(monkeypatch, persistent):
                 model.decode(b)
                 out.append(model.logits().cpu().clone())
                 pos += 1
+        model.reserve_slots(3)  # a new slot table: graphs that read the old one must not be replayed
+        for tok in (31, 32, 33):
+            out += [model.decode_host(tok, pos, lg), lg.clone()]
+            pos += 1
+            b.copy_(torch.tensor([tok + 1, pos], dtype=torch.int32))
+            model.decode(b)
+            out.append(model.logits().cpu().clone())
+            pos += 1
         return out, 1
 
     _assert_same(monkeypatch, script, persistent)

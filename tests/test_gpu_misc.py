@@ -69,3 +69,23 @@ def test_layernorm_q_bit_exact(ctx, rows, dim):
     assert np.array_equal(got.cpu().numpy(), want)
     a2 = torch.from_numpy(x).to(dev)
     assert torch.equal(ctx.add_f32(a2, a2), a2 + a2)
+
+
+@pytest.mark.parametrize("n", [1, 1000, 128256])
+def test_argmax_f32_first_index_of_the_maximum(ctx, n):
+    """tce_argmax_f32 against numpy: the lowest index wins when the maximum repeats, a maximum at the last index is found, and an input
+    with no value above -inf returns 0"""
+    rng = np.random.default_rng(n)
+    x = rng.standard_normal(n).astype(np.float32)
+    cases = [x.copy()]
+    rep = x.copy()
+    rep[rng.choice(n, size=min(n, 5), replace=False)] = 7.0
+    cases.append(rep)
+    last = x.copy()
+    last[-1] = 9.0
+    cases.append(last)
+    for c in cases:
+        got = ctx.argmax_f32(torch.from_numpy(c).cuda())
+        assert int(got.item()) == int(np.argmax(c))
+    for fill in (-np.inf, np.nan):
+        assert int(ctx.argmax_f32(torch.full((n,), fill, dtype=torch.float32, device="cuda")).item()) == 0

@@ -387,7 +387,7 @@ int tce_add_f32(tce_ctx *ctx, const float *a, const float *b, float *out, long l
 int tce_argmax_f32(tce_ctx *ctx, const float *x, int n, int *out) {
     if (!ctx || !x || !out || n < 1) return fail(TCE_ERR_INVALID, "tce_argmax_f32: bad argument");
     CK(cudaSetDevice(ctx->c.device), "cudaSetDevice");
-    CK(launch_argmax(&ctx->c, x, n, out, false), "tce_argmax_f32");
+    CK(launch_argmax_rows(&ctx->c, x, 1, n, out, false), "tce_argmax_f32");
     return TCE_OK;
 }
 
@@ -578,7 +578,9 @@ int tce_llama_tp_handle(tce_llama *m, void *out) {
 }
 int tce_llama_tp_connect(tce_llama *m, const void *handles) {
     if (!m || !handles) return fail(TCE_ERR_INVALID, "tce_llama_tp_connect: null argument");
-    cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->tp_connect(handles);
+    std::string err;
+    cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->tp_connect(handles, &err);
+    if (e == cudaErrorNotSupported) return fail(TCE_ERR_UNSUPPORTED, "tce_llama_tp_connect: %s", err.c_str());
     if (e != cudaSuccess) return tce_fail_cuda(e, "tce_llama_tp_connect");
     return TCE_OK;
 }

@@ -7,30 +7,6 @@
 namespace tce {
 namespace {
 
-// `guard` (optional): {rows of the table, max_ctx} bound the device-resident {token, position}; out-of-range values are clamped before any kernel of the
-// step uses them (the attention kernel reads the position from safe[1]) and flagged in safe[2], so a bad id can never index past the table / KV slab
-__global__ void embedding_kernel(const __half *__restrict__ table, const int *__restrict__ token, float *__restrict__ resid, int E, int rows, int max_ctx,
-                                 int *__restrict__ safe) {
-    pdl_launch_dependents();
-    pdl_wait();
-    int tok = *token;
-    if (safe) {
-        const int pos = token[1];
-        const bool bad = tok < 0 || tok >= rows || pos < 0 || pos >= max_ctx;
-        tok = tok < 0 ? 0 : (tok >= rows ? rows - 1 : tok);
-        if (blockIdx.x == 0 && threadIdx.x == 0) {
-            safe[0] = tok;
-            safe[1] = pos < 0 ? 0 : (pos >= max_ctx ? max_ctx - 1 : pos);
-            safe[2] = bad ? 1 : 0;
-        }
-    }
-    const __half2 *row = reinterpret_cast<const __half2 *>(table + (size_t)tok * E);
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < E / 2; i += gridDim.x * blockDim.x) {
-        const float2 f = __half22float2(row[i]);
-        reinterpret_cast<float2 *>(resid)[i] = f;
-    }
-}
-
 // grid (blocks per row, batch): entry b of req = {token, position, slot}
 __global__ void embedding_batch_kernel(const __half *__restrict__ table, const int *__restrict__ req, float *__restrict__ resid, int E, int rows,
                                        int max_ctx, int n_slots, int *__restrict__ safe) {
@@ -86,76 +62,6 @@ __global__ void __launch_bounds__(1024) argmax_rows_kernel(const float *__restri
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) combine(best, bi, __shfl_xor_sync(0xffffffffu, best, o), __shfl_xor_sync(0xffffffffu, bi, o));
         if (lane == 0) out[blockIdx.x] = bi == 0x7fffffff ? 0 : bi;
-    }
-}
-
-// two-phase argmax with a last-block finish; ties resolve to the lowest index
-struct ArgmaxWs {
-    float val[256];
-    int idx[256];
-    unsigned counter;
-};
-__device__ ArgmaxWs g_argmax_ws;
-
-__global__ void argmax_kernel(const float *__restrict__ x, int n, int *__restrict__ out) {
-    __shared__ float sval[32];
-    __shared__ int sidx[32];
-    __shared__ int is_last;
-    pdl_launch_dependents();
-    pdl_wait();
-    float best = -INFINITY;
-    int bi = 0x7fffffff;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const float v = x[i];
-        if (v > best || (v == best && i < bi)) {
-            best = v;
-            bi = i;
-        }
-    }
-    auto combine = [](float &bv, int &bidx, float ov, int oidx) {
-        if (ov > bv || (ov == bv && oidx < bidx)) {
-            bv = ov;
-            bidx = oidx;
-        }
-    };
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) combine(best, bi, __shfl_xor_sync(0xffffffffu, best, o), __shfl_xor_sync(0xffffffffu, bi, o));
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (lane == 0) {
-        sval[warp] = best;
-        sidx[warp] = bi;
-    }
-    __syncthreads();
-    if (warp == 0) {
-        best = (lane < (blockDim.x >> 5)) ? sval[lane] : -INFINITY;
-        bi = (lane < (blockDim.x >> 5)) ? sidx[lane] : 0x7fffffff;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) combine(best, bi, __shfl_xor_sync(0xffffffffu, best, o), __shfl_xor_sync(0xffffffffu, bi, o));
-        if (lane == 0) {
-            g_argmax_ws.val[blockIdx.x] = best;
-            g_argmax_ws.idx[blockIdx.x] = bi;
-            __threadfence();
-            const unsigned prev = atomicAdd(&g_argmax_ws.counter, 1u);
-            is_last = (prev == gridDim.x - 1);
-        }
-    }
-    __syncthreads();
-    if (!is_last) return;
-    __threadfence();
-    if (warp == 0) {
-        best = -INFINITY;
-        bi = 0x7fffffff;
-        for (int b = lane; b < (int)gridDim.x; b += 32) {
-            const float v = *reinterpret_cast<volatile float *>(&g_argmax_ws.val[b]);
-            const int ix = *reinterpret_cast<volatile int *>(&g_argmax_ws.idx[b]);
-            combine(best, bi, v, ix);
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) combine(best, bi, __shfl_xor_sync(0xffffffffu, best, o), __shfl_xor_sync(0xffffffffu, bi, o));
-        if (lane == 0) {
-            *out = bi;
-            g_argmax_ws.counter = 0;
-        }
     }
 }
 
@@ -300,23 +206,6 @@ cudaError_t launch_cfg(cudaLaunchConfig_t &cfg, cudaLaunchAttribute *attr, dim3 
 }
 
 }  // namespace
-
-cudaError_t launch_embedding(Ctx *ctx, const __half *table, const int *token, float *resid, int E, bool pdl, int rows, int max_ctx, int *safe) {
-    cudaLaunchConfig_t cfg;
-    cudaLaunchAttribute attr[1];
-    launch_cfg(cfg, attr, dim3(4), dim3(256), ctx->stream, pdl);
-    return cudaLaunchKernelEx(&cfg, embedding_kernel, table, token, resid, E, rows, max_ctx, safe);
-}
-
-cudaError_t launch_argmax(Ctx *ctx, const float *logits, int n, int *out, bool pdl) {
-    cudaLaunchConfig_t cfg;
-    cudaLaunchAttribute attr[1];
-    int blocks = (n + 1023) / 1024;
-    if (blocks > 128) blocks = 128;
-    if (blocks < 1) blocks = 1;
-    launch_cfg(cfg, attr, dim3(blocks), dim3(256), ctx->stream, pdl);
-    return cudaLaunchKernelEx(&cfg, argmax_kernel, logits, n, out);
-}
 
 cudaError_t launch_embedding_batch(Ctx *ctx, const __half *table, const int *req, float *resid, int E, int batch, int rows, int max_ctx, int n_slots,
                                    int *safe, bool pdl) {

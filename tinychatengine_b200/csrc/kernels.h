@@ -60,7 +60,7 @@ inline int zeros_width(int ic, int group) {  // llm/src/nn_modules/cuda/utils.cu
 }
 
 enum XMode : int { X_HALF = 0, X_RMSNORM_F32 = 1 };
-enum EpiMode : int { EPI_STORE_HALF = 0, EPI_STORE_F32 = 1, EPI_ADD_F32 = 2, EPI_SILU_MUL_HALF = 3, EPI_TP_SCATTER_F32 = 4 };
+enum EpiMode : int { EPI_STORE_HALF = 0, EPI_STORE_F32 = 1, EPI_ADD_F32 = 2, EPI_SILU_MUL_HALF = 3 };
 constexpr int kMaxTP = 8;
 
 struct W4Seg {
@@ -86,21 +86,6 @@ struct W4GemvParams {
     int ldy = 0;        // elements between output rows
     bool pdl = false;   // launch with programmatic stream serialization
     bool atomic_residual = false;  // EPI_ADD_F32 only: allow RED.ADD for split tiles (non-deterministic last bit)
-    // ---- tensor parallel (tp_size > 1) ----
-    int tp_size = 1;
-    // prologue (X_RMSNORM_F32): x = resid + sum_p tp_in[p][:] once tp_flags[p] >= expected, written back to resid_out
-    const float *tp_in = nullptr;        // local gather buffer [tp_size][IC] fp32 (peers store into it)
-    const unsigned *tp_flags = nullptr;  // local arrival flags [tp_size]
-    const int *tp_step = nullptr;        // device int: decode step index (flags carry step * tp_per_step + tp_k + 1)
-    int tp_k = 0, tp_per_step = 1;
-    float *resid_out = nullptr;
-    // epilogue (EPI_TP_SCATTER_F32): the finished fp32 outputs are stored into slot `rank` of every peer's gather buffer
-    float *tp_out[kMaxTP] = {};
-    // ... and, once every CTA of the launch has stored (local arrival counter), the last one release-stores the step-stamped flag
-    // into every peer's flag word: the collective needs no separate signal kernel
-    unsigned *tp_sig_counter = nullptr;
-    unsigned *tp_sig_flag[kMaxTP] = {};
-    int tp_sig_k = 0;
 };
 
 // M = 2..8 at long rows needs one stream-K fix-up record per (K-slice, row tile); the launch grows ctx->gemv_partials when it has too few

@@ -8,7 +8,6 @@
 #include "../../include/tce_b200.h"
 #include "kernels.h"
 #include "kernels_attn.h"
-#include "kernels_tp.h"
 #include "persistent.h"
 
 namespace tce {
@@ -80,20 +79,21 @@ class LlamaDecoder {
     const float *batch_logits();
     // generate loop of up to TCE_LLAMA_MAX_BATCH sequences: one batched step + one sampler launch (a block per row) per token
     cudaError_t generate_batch(int batch, const tce_gen_request *reqs, int *out_tokens_host, int out_stride, int *n_out, std::string *err);
-    int kernels_per_step() const { return persistent_ ? 1 : tp_ > 1 ? 1 + 7 * cfg_.num_layers + 4 : 1 + 5 * cfg_.num_layers + 2; }
+    int kernels_per_step() const { return persistent_ ? 1 : 1 + 5 * cfg_.num_layers + 2; }
+    // 0..3: row 0 of the kernel-per-op step's buffers (null until they exist)
     void *debug_buffer(int which) const {
         switch (which) {
-            case 0: return d_resid_.get();
-            case 1: return d_qkv_.get();
-            case 2: return d_attn_.get();
-            case 3: return d_act_.get();
+            case 0: return bs_ ? bs_->resid.get() : nullptr;
+            case 1: return bs_ ? bs_->qkv.get() : nullptr;
+            case 2: return bs_ ? bs_->attn.get() : nullptr;
+            case 3: return bs_ ? bs_->act.get() : nullptr;
             case 4: return pargs_.dbg;  // persistent-kernel phase timestamps (TCE_PK_DEBUG=1), [#CTAs][5 * layers + 1][4] u64 ns
             default: return nullptr;
         }
     }
     cudaError_t enqueue_gemvs(int *count);
     cudaError_t tp_handle(void *out64);
-    cudaError_t tp_connect(const void *handles);
+    cudaError_t tp_connect(const void *handles, std::string *err);  // cudaErrorNotSupported (+ *err): the persistent kernel refuses the shard
     // a cudaMalloc allocation freed with the model (loader.cu)
     void adopt(void *device_allocation) { pk_allocs_.emplace_back(static_cast<uint8_t *>(device_allocation)); }
 
@@ -108,35 +108,29 @@ class LlamaDecoder {
     // the prompt pass over n_seqs concatenated prompts (host-checked arguments); leaves the final residual rows in pf_.x.  With score, the
     // expansion of the first lm_head chunk is queued behind the last down_proj GEMM.
     cudaError_t prefill_rows(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, bool score = false);
-    cudaError_t enqueue_step(const int *tokpos, cudaStream_t s, bool pdl, bool gemv_only = false);  // raw kernel sequence
+    // after prefill_rows: the last row of each prompt through the final RMSNorm + lm_head GEMV into logits[n_seqs][V], greedy ids into next
+    cudaError_t prompt_logits(int n_seqs, const int *lengths, float *logits, int *next);
+    // the final RMSNorm + lm_head GEMV over rows of x (pitch E) into rows of y (pitch V)
+    W4GemvParams lm_head_gemv(const float *x, float *y) const;
+    // one single-sequence step on device {token, position}: the persistent kernel, or the batched step at batch 1 on slot 0
+    cudaError_t enqueue_step(const int *tokpos, cudaStream_t s, bool pdl);
     // runs body(stream, pdl) through the graph cached in g for `key`: replays it when it is current, otherwise runs body eagerly on the
     // context's stream and captures it for the next call (PDL edges first, plain edges if refused); graphs off: eager only
     cudaError_t run_graphed(CachedGraph &g, const void *key, const std::function<cudaError_t(cudaStream_t, bool)> &body);
-    void build_ops();
     cudaError_t build_persistent(std::string *err);
-    cudaError_t batch_alloc(std::string *err);  // cudaErrorNotSupported (+ *err) for a model the batched step does not cover
-    cudaError_t enqueue_batch(int batch, const int *req, cudaStream_t s, bool pdl);  // raw kernel sequence of one batched step
-    void drop_batch_graphs();
+    // the batched step's buffers and parameters; cudaErrorNotSupported (+ *err) for a model the batched step does not cover
+    cudaError_t batch_alloc(std::string *err);
+    // raw kernel sequence of one batched step on req = device int[batch][3]; lm_head rows into logits[batch][V], greedy ids into next
+    cudaError_t enqueue_batch(int batch, const int *req, float *logits, int *next, cudaStream_t s, bool pdl);
+    void drop_graphs();
 
-    enum OpType { OP_EMBED, OP_GEMV, OP_ATTN, OP_ARGMAX, OP_TP_SIGNAL, OP_TP_ARGMAX_SCATTER, OP_TP_ARGMAX_FINISH };
-    struct StepOp {
-        OpType type;
-        W4GemvParams g;
-        AttnDecodeArgs at;
-        TpSignalArgs sig;
-        TpArgmaxArgs am;
-        TpArgmaxFinishArgs amf;
-    };
-    // tensor parallel state
+    // tensor parallel state (the persistent kernel's hand-off buffers)
     int tp_ = 1;
     bool tp_connected_ = false;
     DevPtr<uint8_t> tp_buf_;             // peer-visible allocation of this rank
-    size_t tp_bytes_ = 0, tp_gather_floats_ = 0;
+    size_t tp_bytes_ = 0;
     uint8_t *tp_peer_[kMaxTP] = {};      // every rank's allocation as mapped into this process
-    int step_index_ = 0;
-    std::vector<StepOp> ops_;
-    W4GemvParams lm_gemv_{};            // the step's final RMSNorm + lm_head GEMV (M = 1), also run after a prompt pass
-    // persistent decode kernel (default; TCE_PERSISTENT=0 selects one kernel per op inside a CUDA graph)
+    // persistent decode kernel (default; TCE_PERSISTENT=0 selects the batched step at batch 1, one kernel per op inside a CUDA graph)
     bool persistent_ = false;
     pk::Args pargs_{};
     std::vector<DevPtr<uint8_t>> pk_allocs_;  // repacked scales|zeros, tensor maps, layer table, counters; adopted loader copies
@@ -148,12 +142,8 @@ class LlamaDecoder {
     tce_llama_weights w_{};
     // device state
     DevPtr<__half> d_kv_;           // [L][2][KVH][max_ctx][hd]
-    DevPtr<float> d_resid_;         // fp32 residual stream [E]
-    DevPtr<__half> d_qkv_;          // [(H+2KVH)*hd]
-    DevPtr<__half> d_attn_;         // [H*hd]
-    DevPtr<__half> d_act_;          // [F] SiLU(gate)*up
     DevPtr<float> d_logits_;        // [V]
-    DevPtr<int> d_tokpos_;          // {token, pos} staged for the host entry point
+    DevPtr<int> d_tokpos_;          // {token, pos, slot = 0}: staged for the host entry point, the request of the kernel-per-op step
     DevPtr<int> d_next_;            // greedy arg-max
     DevPtr<int> d_gen_;             // generate loop: [0] history head, [1] output count, [2] stop flag, then history ring [max_ctx], output list [max_ctx]
     const float *d_cos_ = nullptr, *d_sin_ = nullptr;  // the caller's RoPE tables, or the halves of rope_
@@ -201,8 +191,8 @@ class LlamaDecoder {
     cudaStream_t cap_stream_ = nullptr;
     CachedGraph g_host_;            // H2D(tokpos) + step + argmax + D2H(logits,next)
     CachedGraph g_dev_;             // step on the caller's {token, pos}
-    DevPtr<int> d_tokpos_safe_;     // kernel-per-op path: {token, position} after the device-side range check (+ [2] unused, [3] TP step counter alias)
-    // batched decode state (allocated on first use): the step's buffers hold TCE_LLAMA_MAX_BATCH rows each
+    // batched decode state (allocated on first use; also the kernel-per-op single-sequence step): the step's buffers hold
+    // TCE_LLAMA_MAX_BATCH rows each
     std::vector<DevPtr<__half>> slot_kv_;  // KV-cache slots 1.. ([L][2][KVH][max_ctx][hd] each)
     struct BatchState {
         DevPtr<__half *> slot_table;  // device table of every slot's base, slot 0 = d_kv_
@@ -224,10 +214,14 @@ class LlamaDecoder {
         // [8][max_ctx] output lists; the sampler arguments of each row
         DevPtr<int> gen;
         DevPtr<SampleArgs> sample;
+        // the step's parameters on these buffers: GEMV 4 * layer + {0: q|k|v, 1: o, 2: gate|up, 3: down} (M = 1), then the lm_head;
+        // the attention of each layer (its slot table is read at launch)
+        std::vector<W4GemvParams> gemv_ops;
+        std::vector<AttnBatchArgs> attn_ops;
     };
     std::unique_ptr<BatchState> bs_;  // non-null: every buffer of the batched step exists
     // one graph per batch size: host entry (with / without the logits copy), device entry (for one request pointer), generate loop (one
-    // batched step on bs_->req + the row sampler)
+    // batched step on bs_->req + the row sampler).  Dropped with the single-sequence graphs when the slot table changes.
     CachedGraph g_bhost_[2][TCE_LLAMA_MAX_BATCH + 1];
     CachedGraph g_bdev_[TCE_LLAMA_MAX_BATCH + 1];
     CachedGraph g_bgen_[TCE_LLAMA_MAX_BATCH + 1];

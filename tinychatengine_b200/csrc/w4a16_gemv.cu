@@ -257,21 +257,6 @@ KArgs make_kargs(Ctx *ctx, const W4GemvParams &p, int *total_rows) {
     a.full = (a.NG % kStageGroups == 0) ? 1 : 0;
     a.sl = a.NG;
     a.nsl = 1;
-    a.tp_size = p.tp_size;
-    a.tp_in = p.tp_in;
-    a.tp_flags = p.tp_flags;
-    a.tp_step = p.tp_step;
-    a.tp_k = p.tp_k;
-    a.tp_per_step = p.tp_per_step;
-    a.resid_out = p.resid_out;
-    for (int i = 0; i < kMaxTP; i++) a.tp_out[i] = p.tp_out[i];
-    a.tp_sig_counter = p.tp_sig_counter;
-    for (int i = 0; i < kMaxTP; i++) a.tp_sig_flag[i] = p.tp_sig_flag[i];
-    a.tp_sig_k = p.tp_sig_k;
-    if (p.tp_sig_counter) {  // the sender stamps its flags with the step counter too
-        a.tp_step = p.tp_step;
-        a.tp_per_step = p.tp_per_step;
-    }
     return a;
 }
 
@@ -423,7 +408,6 @@ cudaError_t launch_w4a16_gemv(Ctx *ctx, const W4GemvParams &p) {
     const int cw = consumer_warps(ctx, p);
     if (p.M == 1) return (cw == 16) ? launch_mma<1, 16>(ctx, a, p.pdl) : launch_mma<1, 8>(ctx, a, p.pdl);
     // M = 2..8: one pass over the weights, the activation rows staged one K-slice at a time where the whole rows do not fit
-    if (p.tp_size > 1) return cudaErrorNotSupported;
     a.sl = slice_of(ctx, p);
     if (a.sl == 0) return cudaErrorInvalidConfiguration;
     a.nsl = (a.NG + a.sl - 1) / a.sl;

@@ -61,17 +61,6 @@ struct KArgs {
     // multi-column kernel: the activation columns are staged one K-slice at a time.  A slice is `sl` groups (a multiple of kStageGroups, or NG)
     // and the units are ordered slice-major, u = T*sl*s + rt*len(s) + (g - s*sl): a CTA stages only the slices its range touches
     int sl, nsl;
-    // tensor parallel: see W4GemvParams
-    int tp_size;
-    const float *tp_in;
-    const unsigned *tp_flags;
-    const int *tp_step;
-    int tp_k, tp_per_step;
-    float *resid_out;
-    float *tp_out[kMaxTP];
-    unsigned *tp_sig_counter;     // fused signal (EPI_TP_SCATTER_F32): local arrival counter, peers' flag words, collective index
-    unsigned *tp_sig_flag[kMaxTP];
-    int tp_sig_k;
     // one 2-D tensor map per weight segment: uint32 [rows][IC/8], box = [16 (8 in pair mode) rows][sg*16 words]
     alignas(64) CUtensorMap tmap[3];
 };
@@ -324,11 +313,7 @@ TCE_DEVINL void finish_tile(const KArgs &a, const float (&v)[VPL], int rt, int l
             const int row = idx / NCOLS, col = idx % NCOLS;
             if (idx < kVals && col < a.M) {
                 const size_t o = (size_t)col * a.ldy + (size_t)rt * 16 + row;
-                if (a.epi == EPI_TP_SCATTER_F32) {
-                    // fused collective: the finished outputs go straight into slot `rank` of every rank's gather
-                    // buffer over NVLink (peer stores); the reduction happens in the next kernel's prologue
-                    for (int pr = 0; pr < a.tp_size; pr++) a.tp_out[pr][o] = v[i];
-                } else if (a.epi == EPI_STORE_HALF)
+                if (a.epi == EPI_STORE_HALF)
                     reinterpret_cast<__half *>(a.y)[o] = __float2half(v[i]);
                 else if (a.epi == EPI_STORE_F32)
                     reinterpret_cast<float *>(a.y)[o] = v[i];
@@ -426,21 +411,6 @@ TCE_DEVINL void epilogue(const KArgs &a, const Smem &sm, RedState &es, int cta, 
         u += ge - gb;
         rt++;
         gb = 0;
-    }
-    if (a.epi == EPI_TP_SCATTER_F32 && a.tp_sig_counter) {
-        // fused collective signal: this CTA's peer stores are fenced system-wide, then it checks in; the last CTA of the launch
-        // publishes the step-stamped flag to every rank (release), which the receiving prologue acquires
-        __threadfence_system();
-        __syncwarp();
-        unsigned last = 0;
-        if (lane == 0) last = (atomicAdd(a.tp_sig_counter, 1u) == (unsigned)(ncta - 1)) ? 1u : 0u;
-        last = __shfl_sync(0xffffffffu, last, 0);
-        if (last) {
-            __threadfence_system();
-            if (lane == 0) *a.tp_sig_counter = 0u;
-            const unsigned value = (unsigned)(*a.tp_step) * (unsigned)a.tp_per_step + (unsigned)a.tp_sig_k + 1u;
-            if (lane < a.tp_size) asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(a.tp_sig_flag[lane]), "r"(value) : "memory");
-        }
     }
 }
 
@@ -558,37 +528,6 @@ TCE_DEVINL void stage_activations(const KArgs &a, const Smem &sm, int x_pitch, i
         uint8_t *xcol = sm.xs + (size_t)col * x_pitch;
         float inv = 1.f;
         const float *xsrc = reinterpret_cast<const float *>(a.x);
-        if (a.x_mode == X_RMSNORM_F32 && a.tp_in && col == 0) {
-            // tensor-parallel all-reduce, receive side: wait until every rank's partial for this collective has landed
-            // in the local gather buffer (flags written by the peers' signal kernels), then residual += sum over ranks
-            // in fixed rank order (bit-identical on every rank).  The sum is written to resid_out by every CTA (same
-            // values), each thread re-reads only what it wrote itself.
-            if (ctid < a.tp_size) {
-                const unsigned expect = (unsigned)(*a.tp_step) * (unsigned)a.tp_per_step + (unsigned)a.tp_k + 1u;
-                const long long t0 = clock64();
-                while (true) {
-                    unsigned f;
-                    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(f) : "l"(a.tp_flags + ctid) : "memory");
-                    if (f >= expect) break;
-                    if (clock64() - t0 > 6000000000LL) __trap();
-                }
-            }
-            named_bar_sync(1, kConsumerThreads);
-            for (int ui = ctid; ui < units; ui += kConsumerThreads) {
-                float4 s0 = *reinterpret_cast<const float4 *>(xsrc + ui * 8);
-                float4 s1 = *reinterpret_cast<const float4 *>(xsrc + ui * 8 + 4);
-                for (int pr = 0; pr < a.tp_size; pr++) {
-                    const float *gp = a.tp_in + (size_t)pr * a.IC + ui * 8;
-                    const float4 g0 = *reinterpret_cast<const float4 *>(gp);
-                    const float4 g1 = *reinterpret_cast<const float4 *>(gp + 4);
-                    s0.x += g0.x; s0.y += g0.y; s0.z += g0.z; s0.w += g0.w;
-                    s1.x += g1.x; s1.y += g1.y; s1.z += g1.z; s1.w += g1.w;
-                }
-                *reinterpret_cast<float4 *>(a.resid_out + ui * 8) = s0;
-                *reinterpret_cast<float4 *>(a.resid_out + ui * 8 + 4) = s1;
-            }
-            xsrc = a.resid_out;
-        }
         if (a.x_mode == X_RMSNORM_F32 && col < a.M) {
             const float *xr = xsrc + (size_t)col * a.ldx;
             float ss = 0.f;

@@ -262,7 +262,6 @@ class LlamaModel:
         blob = b"".join(bytes(o.cpu().tolist()) for o in out)
         buf = (C.c_ubyte * len(blob)).from_buffer_copy(blob)
         _lib.check(self.ctx.L.tce_llama_tp_connect(self.h, C.cast(buf, C.c_void_p)), "tce_llama_tp_connect")
-        self.kernels_per_step = self.ctx.L.tce_llama_kernels_per_step(self.h)  # the step's form is only known once the peers are mapped
         dist.barrier(group=group)
 
     def layer_tensors(self, l: int):
@@ -427,7 +426,10 @@ class LlamaModel:
         g = self.geom
         shape, dt = {0: ((g.embed_dim,), torch.float32), 1: (((g.num_heads + 2 * g.num_kv_heads) * g.head_dim,), torch.float16),
                      2: ((g.num_heads * g.head_dim,), torch.float16), 3: ((g.hidden_dim,), torch.float16)}[which]
-        return _tensor_from_ptr(self.ctx.L.tce_llama_debug_buffer(self.h, which), shape, dt, self.ctx.device)
+        ptr = self.ctx.L.tce_llama_debug_buffer(self.h, which)
+        if not ptr:
+            raise _lib.TceError(f"debug buffer {which}: the kernel-per-op step has not run on this model")
+        return _tensor_from_ptr(ptr, shape, dt, self.ctx.device)
 
     def close(self):
         if self.h:

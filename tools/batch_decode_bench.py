@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Batched decode on Llama-3-8B synthetic weights (32 layers, max_ctx 4096, random-filled caches): ms per step and aggregate tok/s at
-B = 1, 2, 4, 8 sequences whose positions average 2048, against the batch-1 persistent step (tce_llama_decode) in the same process.
+B = 1, 2, 4, 8 sequences whose positions average 2048, against the batch-1 persistent step (tce_llama_decode) in the same process, and the
+kernel-per-op batch-1 step (a second model on the same weights, built with TCE_PERSISTENT=0: the batched step at batch 1 on slot 0).
 
     python tools/batch_decode_bench.py --steps 50 --warmup 5 --out result.json
     python tools/batch_decode_bench.py --profile --out launches.json   # GEMV launches per batched step (torch.profiler, no timing)
@@ -70,6 +71,26 @@ def timed(fn, steps, warmup):
     return e0.elapsed_time(e1) / steps
 
 
+def per_op_model(ctx, model, max_ctx):
+    """a model on the same weights whose single-sequence step is one kernel per op, its slot-0 cache a copy of `model`'s"""
+    from tinychatengine_b200.llama import LlamaModel
+
+    old = os.environ.get("TCE_PERSISTENT")
+    os.environ["TCE_PERSISTENT"] = "0"
+    try:
+        m = LlamaModel(ctx, model.geom, max_ctx=max_ctx, weights=model.W)
+    finally:
+        if old is None:
+            del os.environ["TCE_PERSISTENT"]
+        else:
+            os.environ["TCE_PERSISTENT"] = old
+    for l in range(model.geom.num_layers):
+        for which in (0, 1):
+            m.kv_cache(l, which).copy_(model.kv_cache(l, which))
+    torch.cuda.synchronize()
+    return m
+
+
 def measure(args):
     from tinychatengine_b200.llama import kv_bytes_per_token, weight_bytes_per_token
 
@@ -88,6 +109,9 @@ def measure(args):
 
     tp = torch.tensor([321, 2048], dtype=torch.int32, device="cuda")
     row("persistent batch-1 (tce_llama_decode)", 1, [2048], timed(lambda: model.decode(tp), args.steps, args.warmup))
+    per_op = per_op_model(ctx, model, args.max_ctx)
+    row("kernel-per-op batch-1 (tce_llama_decode, TCE_PERSISTENT=0)", 1, [2048], timed(lambda: per_op.decode(tp), args.steps, args.warmup))
+    per_op.close()
     for batch in BATCHES:
         req = requests(g, batch)
         row("batched (tce_llama_decode_batch)", batch, positions(batch), timed(lambda: model.decode_batch(req), args.steps, args.warmup))

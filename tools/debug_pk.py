@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Persistent decode kernel vs the kernel-per-op graph path, buffer by buffer (1-layer models so every intermediate survives the step)."""
+"""Persistent decode kernel vs the kernel-per-op graph path, step by step: greedy token, appended K/V rows and logits (1-layer models)."""
 import os
 import sys
 from pathlib import Path
@@ -20,9 +20,8 @@ def run(g, mode, steps, W, max_ctx):
     tok = 3
     for pos in range(steps):
         nxt = model.decode_host(tok, pos, lg)
-        out.append({"logits": lg.clone(), "resid": model.debug_buffer(0).float().cpu().clone(), "qkv": model.debug_buffer(1).float().cpu().clone(),
-                    "attn": model.debug_buffer(2).float().cpu().clone(), "act": model.debug_buffer(3).float().cpu().clone(), "next": nxt,
-                    "k": model.kv_cache(0, 0)[:, :pos + 1].float().cpu().clone(), "v": model.kv_cache(0, 1)[:, :pos + 1].float().cpu().clone()})
+        out.append({"logits": lg.clone(), "next": nxt, "k": model.kv_cache(0, 0)[:, :pos + 1].float().cpu().clone(),
+                    "v": model.kv_cache(0, 1)[:, :pos + 1].float().cpu().clone()})
         tok = (nxt * 7 + pos) % g.vocab_size
     model.close()
     ctx.close()
@@ -40,7 +39,7 @@ def main():
     b = run(g, "1", steps, W, 256)
     for pos in range(steps):
         msg = [f"pos {pos}: next {a[pos]['next']} / {b[pos]['next']}"]
-        for k in ("qkv", "k", "v", "attn", "act", "resid", "logits"):
+        for k in ("k", "v", "logits"):
             x, y = a[pos][k], b[pos][k]
             d = (x - y).abs().max().item() / max(x.abs().max().item(), 1e-9)
             msg.append(f"{k} {d:.2e}")
