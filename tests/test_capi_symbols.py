@@ -100,6 +100,88 @@ int main() {
     assert r.returncode == 0 and "ok" in r.stdout, r.stdout
 
 
+def test_slice_walk_properties(tmp_path):
+    """The GEMV's unit walk (csrc/kernels.h SliceWalk, which every role of both GEMV kernels walks) compiled for the host.  With one slice it is
+    the tile-major stream-K walk: the same CTA starts and pieces (rt = u / NG, gb = u % NG, up to the end of the tile or of the range).  With
+    several slices the CTA ranges tile [0, T*NG), are monotone and start on (slice, tile) segment boundaries, the segments run slice-major,
+    and locate() places every unit inside its segment."""
+    import subprocess
+
+    src = tmp_path / "walk.cc"
+    src.write_text(r"""
+#include <cuda_runtime.h>
+#include <stdio.h>
+#include "kernels.h"
+using tce::SliceWalk;
+using tce::StreamK;
+static int check_one_slice(int T, int NG, int nc, int aligned, int gran) {
+    const SliceWalk W{T, NG, NG, 1};
+    StreamK sk; sk.U = (long long)T * NG; sk.nc = nc; sk.NG = NG; sk.aligned = aligned; sk.T = T; sk.gran = gran;
+    for (int c = 0; c < nc; c++) {
+        if (W.start(sk, c) != sk.start(c)) return 1;
+        const int uend = W.start(sk, c + 1);
+        for (int u = W.start(sk, c); u < uend;) {
+            int s, rt, gb, seg0;
+            W.locate(u, s, rt, gb, seg0);
+            const int pe = uend < seg0 + W.len(s) ? uend : seg0 + W.len(s);
+            const int rt_end = (u / NG + 1) * NG;
+            if (s != 0 || rt != u / NG || gb != u % NG || pe != (uend < rt_end ? uend : rt_end)) return 2;
+            u = pe;
+        }
+    }
+    return 0;
+}
+static int check_slices(int T, int NG, int sl, int nc) {
+    const int nsl = (NG + sl - 1) / sl;
+    const SliceWalk W{T, NG, sl, nsl};
+    const int U = T * NG;
+    if (nc > T * nsl) nc = T * nsl;
+    StreamK sk; sk.U = U; sk.nc = nc; sk.NG = NG; sk.T = T;
+    // segments run slice-major: segment k = s*T + rt holds len(s) units, starting where segment k-1 ends
+    if (W.seg_unit(0) != 0 || W.seg_unit((long long)T * nsl) != U) return 1;
+    for (long long k = 0; k < (long long)T * nsl; k++)
+        if (W.seg_unit(k + 1) - W.seg_unit(k) != W.len((int)(k / T))) return 2;
+    if (W.start(sk, 0) != 0 || W.start(sk, nc) != U) return 3;
+    for (int c = 0; c < nc; c++) {
+        const int a = W.start(sk, c), b = W.start(sk, c + 1);
+        if (b < a) return 4;
+        int s, rt, gb, seg0;
+        W.locate(a < U ? a : 0, s, rt, gb, seg0);
+        if (nsl > 1 && a < U && seg0 != a) return 5;  // one slice keeps the stream-K cuts (checked above)
+    }
+    for (int u = 0; u < U; u += (U > 100000 ? 7 : 1)) {
+        int s, rt, gb, seg0;
+        W.locate(u, s, rt, gb, seg0);
+        if (s < 0 || s >= nsl || rt < 0 || rt >= T || seg0 != W.seg_unit((long long)s * T + rt)) return 6;
+        if (u < seg0 || u >= seg0 + W.len(s) || gb != s * sl + (u - seg0) || W.slice(u) != s) return 7;
+    }
+    return 0;
+}
+int main() {
+    const int tiles[] = {1, 3, 256, 1792, 8016}, ngs[] = {8, 32, 86, 112}, ncs[] = {1, 7, 132, 264, 528};
+    for (int t : tiles) for (int ng : ngs) for (int nc : ncs) {
+        const long long U = (long long)t * ng;
+        for (int gran : {1, 16}) {
+            if (U % gran) continue;
+            const int n = nc < U / gran ? nc : (int)(U / gran);
+            if (int e = check_one_slice(t, ng, n, 0, gran)) { printf("one slice T=%d NG=%d nc=%d gran=%d -> %d ", t, ng, n, gran, e); return 1; }
+        }
+        if (t >= nc) if (int e = check_one_slice(t, ng, nc, 1, 1)) { printf("one slice aligned T=%d NG=%d nc=%d -> %d ", t, ng, nc, e); return 1; }
+        for (int sl = 16; sl < ng; sl += 16)
+            if (int e = check_slices(t, ng, sl, nc)) { printf("slices T=%d NG=%d sl=%d nc=%d -> %d ", t, ng, sl, nc, e); return 1; }
+        if (int e = check_slices(t, ng, ng, nc)) { printf("slices T=%d NG=%d sl=NG nc=%d -> %d ", t, ng, nc, e); return 1; }
+    }
+    puts("ok");
+    return 0;
+}
+""")
+    exe = tmp_path / "walk"
+    inc = ROOT / "tinychatengine_b200" / "csrc"
+    subprocess.run(["g++", "-std=c++17", "-O2", "-I/usr/local/cuda/include", f"-I{inc}", "-o", str(exe), str(src)], check=True)
+    r = subprocess.run([str(exe)], capture_output=True, text=True)
+    assert r.returncode == 0 and "ok" in r.stdout, r.stdout
+
+
 @pytest.mark.skipif(torch.cuda.is_available(), reason="this checks the no-GPU behaviour")
 def test_no_cpu_fallback(built_lib):
     from tinychatengine_b200 import _lib

@@ -1,5 +1,5 @@
-"""Host-side model of the decode GEMV's arithmetic (tinychatengine_b200/csrc/w4a16_gemv_impl.cuh: emit_unit :441-531, the group combination :687-697 and
-:831-846; shared by the persistent decode kernel): fp16 activations -> 32-bit block fixed point per 128-group -> four balanced base-256 int8 digit planes ->
+"""Host-side model of the decode GEMV's arithmetic (tinychatengine_b200/csrc: emit_unit in w4a16_act_planes.cuh, shared by the persistent decode kernel,
+and the group combination of unit1 and consume_cols in w4a16_gemv_impl.cuh): fp16 activations -> 32-bit block fixed point per 128-group -> four balanced base-256 int8 digit planes ->
 exact integer dot products with the nibbles -> one fp32 FMA per group.  The model restates that arithmetic in numpy with the SAME integer widths and checks,
 without a GPU, the properties DESIGN.md 4.1 claims: the digits reconstruct X, nothing overflows 32 bits at the extreme inputs, and the result stays inside
 the parity contract (<= 1e-2 per element wherever |y| > 1e-3 max|y|, SURVEY.md 8(d) config 1) on the heavy-tailed activations that broke round 1's 15-bit

@@ -182,4 +182,18 @@ TCE_DEVINL float ldg_cg_f32(const float *p) {
     return r;
 }
 
+// ---------------------------------------------------------------- host: TMA descriptors ------------------
+// cuTensorMapEncodeTiled is a pure host-side encoder; it is reached through the runtime's driver entry point so the library does not
+// link libcuda directly.  Looked up once per process; nullptr when the driver does not provide it.
+typedef CUresult (*TmapEncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
+                                 const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+inline TmapEncodeFn tmap_encoder() {
+    static const TmapEncodeFn fn = [] {
+        void *sym = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        return cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &q) == cudaSuccess ? reinterpret_cast<TmapEncodeFn>(sym) : nullptr;
+    }();
+    return fn;
+}
+
 }  // namespace tce

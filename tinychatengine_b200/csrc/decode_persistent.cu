@@ -27,7 +27,7 @@
 
 #include "attention_impl.cuh"
 #include "persistent.h"
-#include "w4a16_gemv_impl.cuh"
+#include "w4a16_act_planes.cuh"
 
 namespace tce {
 namespace pk {
@@ -1227,19 +1227,14 @@ cudaError_t repack_meta(Ctx *ctx, const W4Seg *segs, int nseg, int pair, int IC,
 }
 
 cudaError_t encode_kv_tmap(CUtensorMap *out, const void *kv, long long rows) {
-    typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
-                                 const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-    void *sym = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &q);
-    if (e != cudaSuccess || !sym) return e != cudaSuccess ? e : cudaErrorNotSupported;
+    const TmapEncodeFn fn = tmap_encoder();
+    if (!fn) return cudaErrorNotSupported;
     const cuuint64_t gdim[2] = {128, (cuuint64_t)rows};
     const cuuint64_t gstride[1] = {256};
     const cuuint32_t box[2] = {64, (cuuint32_t)kKvChunk};
     const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = reinterpret_cast<EncodeFn>(sym)(out, CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, const_cast<void *>(kv), gdim, gstride, box, estr,
-                                                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, const_cast<void *>(kv), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 

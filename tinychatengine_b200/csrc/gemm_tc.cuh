@@ -267,22 +267,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wg_kernel(const __grid_const
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
-                             const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-inline EncodeFn encoder() {
-    static EncodeFn fn = nullptr;
-    if (!fn) {
-        void *sym = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &q) == cudaSuccess && sym) fn = reinterpret_cast<EncodeFn>(sym);
-    }
-    return fn;
-}
-
 // [rows][K] K-major operand (fp16 or int8), box {128 B, box_rows}, SWIZZLE_128B
 inline cudaError_t encode_kmajor(CUtensorMap *out, const void *base, bool i8, long long rows, long long K, long long ld_elems, int box_rows) {
-    EncodeFn fn = encoder();
+    const TmapEncodeFn fn = tmap_encoder();
     if (!fn) return cudaErrorNotSupported;
     const int es = i8 ? 1 : 2;
     const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)rows};

@@ -142,4 +142,36 @@ struct StreamK {
     }
 };
 
+// Unit order of the W4A16 GEMV over T row tiles of NG groups, cut into K-slices of `sl` groups (the last slice may be shorter): units are
+// ordered slice-major, u = T*sl*s + rt*len(s) + (g - s*sl), and a (slice, tile) segment is len(s) consecutive units.  With one slice
+// (sl = NG) this is the tile-major stream-K order u = rt*NG + g.  A piece is the part of one segment inside one CTA's range.
+struct SliceWalk {
+    int T, NG, sl, nsl;
+    __host__ __device__ int len(int s) const { return s < nsl - 1 ? sl : NG - s * sl; }
+    __host__ __device__ int slice(int u) const {
+        if (nsl == 1) return 0;
+        const int s = u / (T * sl);
+        return s < nsl - 1 ? s : nsl - 1;
+    }
+    // unit u -> slice s, row tile rt, first group gb of the piece, first unit seg0 of the (slice, tile) segment
+    __host__ __device__ void locate(int u, int &s, int &rt, int &gb, int &seg0) const {
+        s = slice(u);
+        const int base = s * T * sl, L = len(s);
+        rt = (u - base) / L;
+        seg0 = base + rt * L;
+        gb = s * sl + (u - seg0);
+    }
+    // first unit of segment k (k = s * T + rt; the last slice may be shorter)
+    __host__ __device__ int seg_unit(long long k) const {
+        const long long kf = (long long)T * (nsl - 1);
+        return (int)(k <= kf ? k * sl : kf * sl + (k - kf) * (NG - (nsl - 1) * sl));
+    }
+    // first unit of CTA c: one slice keeps the stream-K cuts of `sk`; with several the ranges are cut at segment boundaries, so every
+    // piece is a whole (slice, tile) segment
+    __host__ __device__ int start(const StreamK &sk, int c) const {
+        if (nsl == 1) return (int)sk.start(c);
+        return seg_unit((long long)T * nsl * c / sk.nc);
+    }
+};
+
 }  // namespace tce

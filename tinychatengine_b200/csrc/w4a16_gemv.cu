@@ -1,8 +1,8 @@
-// w4a16_gemv.cu -- stand-alone W4A16 group-128 GEMV launch (batch 1..8 decode) on sm_90a.
+// w4a16_gemv.cu -- stand-alone W4A16 GEMV launch (batch 1..8 decode) on sm_90a.
 //
 // Replaces MatmulOperator::gemv_forward_cuda + gemv_kernel_g128 (reference kernels/cuda/gemv_cuda.cu:140-260).
-// The device-side roles live in w4a16_gemv_impl.cuh (shared with the persistent decode kernel); this file is the
-// kernel wrapper, the independent cross-check kernel and the host-side launch logic.
+// The device-side roles live in w4a16_gemv_impl.cuh; this file is the kernel wrapper, the independent cross-check
+// kernel (also the group-64 path) and the host-side launch logic.
 #include <stdio.h>
 
 #include "w4a16_gemv_impl.cuh"
@@ -17,7 +17,7 @@ template <int NCOLS, int CW>
 __global__ void __launch_bounds__(32 * (kProducerWarps + 1 + CW), (NCOLS == 1 && CW == 8) ? 2 : 1) w4a16_gemv_kernel(const __grid_constant__ KArgs a) {
     extern __shared__ __align__(128) uint8_t smem[];
     using L = Layout<NCOLS, CW>;
-    const int xw = NCOLS == 1 ? a.IC : a.sl * 128;  // activation elements staged per column
+    const int xw = a.sl * 128;  // activation elements staged per column: one K-slice (the whole row when nsl == 1)
     const Smem sm = carve<NCOLS, CW>(smem, a.IC, a.nst, xw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int cta = blockIdx.x, ncta = gridDim.x;
@@ -27,7 +27,7 @@ __global__ void __launch_bounds__(32 * (kProducerWarps + 1 + CW), (NCOLS == 1 &&
         if (lane == 0) dbg_stamp(a, cta, 0);
         init_barriers_warp<CW>(sm, lane);
     } else if (tid == 32) {
-        // the TMA unit's first use of a tensor map costs a descriptor fetch: start it while lane 0 initialises the barriers
+        // the TMA unit's first use of a tensor map costs a descriptor fetch: start it while warp 0 initialises the barriers
         for (int i = 0; i < a.nseg; i++) asm volatile("prefetch.tensormap [%0];" ::"l"(&a.tmap[i]) : "memory");
     }
     // Warp 0 (which initialised the barriers) only signals; the others wait where they first need the barriers: the epilogue warp
@@ -41,52 +41,44 @@ __global__ void __launch_bounds__(32 * (kProducerWarps + 1 + CW), (NCOLS == 1 &&
     }
 
     if (warp < kProducerWarps) {
-        RingState rs;
-        if constexpr (NCOLS == 1)
-            produce(a, sm, rs, cta, ncta, lane, l2_policy_evict_first());
-        else
-            produce_cols(a, sm, rs, cta, ncta, lane, l2_policy_evict_first());
+        produce<NCOLS>(a, sm, cta, ncta, lane, l2_policy_evict_first());
         // this CTA has requested its last byte of weights: a programmatically dependent kernel may become resident
         pdl_launch_dependents();
         return;
     }
     if (warp == kProducerWarps) {
         pdl_wait();  // outputs (and the residual we add into) belong to earlier kernels
-        RedState es;
-        if constexpr (NCOLS == 1)
-            epilogue<NCOLS, CW>(a, sm, es, cta, ncta, lane);
-        else
-            epilogue_cols<NCOLS, CW>(a, sm, es, cta, ncta, lane);
+        epilogue<NCOLS, CW>(a, sm, cta, ncta, lane);
         if (lane == 0) dbg_stamp(a, cta, 5);
         return;
     }
     const int ctid = tid - 32 * (kProducerWarps + 1);
     const int cw = warp - (kProducerWarps + 1);
     pdl_wait();  // activations belong to the previous kernel until here
-    int s0 = 0;
-    if constexpr (NCOLS == 1) {
-        stage_activations<NCOLS, CW>(a, sm, L::x_pitch(a.IC), ctid, cw, lane);
-    } else {
-        if (a.x_mode == X_RMSNORM_F32) rms_partials<NCOLS, CW>(a, sm, ctid, cw, lane);
-        s0 = first_slice(a, cta, ncta);
-        stage_slice<NCOLS, CW>(a, sm, L::x_pitch(xw), s0, ctid, cw, lane);
-    }
+    if (a.x_mode == X_RMSNORM_F32) rms_partials<NCOLS, CW>(a, sm, ctid, cw, lane);
+    const int s0 = first_slice<NCOLS>(a, cta, ncta);
+    stage_slice<NCOLS, CW>(a, sm, L::x_pitch(xw), s0, ctid, cw, lane);
     if (ctid == 0) dbg_stamp(a, cta, 2);
     asm volatile("bar.sync 3, %0;" ::"r"(32 * (kProducerWarps + 1 + CW)) : "memory");
-    RingState rs;
-    RedState cs;
-    if constexpr (NCOLS == 1)
-        consume<NCOLS, CW>(a, sm, rs, cs, L::x_pitch(a.IC), cta, ncta, cw, lane);
-    else
-        consume_cols<NCOLS, CW>(a, sm, rs, cs, L::x_pitch(xw), s0, cta, ncta, ctid, cw, lane);
+    if constexpr (NCOLS == 1) {
+        if (a.full)
+            consume1<CW, true>(a, sm, L::x_pitch(xw), s0, cta, ncta, ctid, cw, lane);
+        else
+            consume1<CW, false>(a, sm, L::x_pitch(xw), s0, cta, ncta, ctid, cw, lane);
+    } else {
+        consume_cols<NCOLS, CW>(a, sm, L::x_pitch(xw), s0, cta, ncta, ctid, cw, lane);
+    }
     if (ctid == 0) dbg_stamp(a, cta, 4);
 }
 
 // ------------------------------------------------------------------------------------------------------
-// Simple cross-check kernel: one warp per output row, 128-bit loads, scalar fp32 math.  Not the product
-// path for performance; kept as an independently-written second implementation ("gemv_impl" = 0) and for
-// the < 16 trailing rows of an OC that is not a multiple of 16.
+// Simple cross-check kernel: one warp per output row, 128-bit loads, scalar fp32 math like the reference.  Not the product
+// path for performance; kept as an independently-written second implementation ("gemv_impl" = 0), for the < 16 trailing
+// rows of an OC that is not a multiple of 16, and as the group-64 GEMV (GS = 64, reference gemv_kernel_g64,
+// kernels/cuda/gemv_cuda.cu:68-123: the same QM_CUDA layout with zeros_w = zeros_width(IC, 64) and one scale / zero point per
+// 64 input channels; QM_CUDA models are quantised with group 128, that slot exists for interface completeness).
 // ------------------------------------------------------------------------------------------------------
+template <int GS>
 __global__ void w4a16_gemv_simple_kernel(const KArgs a, int total_rows) {
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
@@ -109,7 +101,7 @@ __global__ void w4a16_gemv_simple_kernel(const KArgs a, int total_rows) {
         float acc = 0.f;
         for (int c = lane; c < a.IC / 32; c += 32) {  // 32 nibbles per uint4
             const uint4 wv = wrow[c];
-            const int G = c >> 2;
+            const int G = c >> (GS == 128 ? 2 : 1);
             const float sc = __half2float(srow[G]);
             const float z = (float)((zrow[G >> 3] >> ((G & 7) * 4)) & 0xF);
             const uint32_t words[4] = {wv.x, wv.y, wv.z, wv.w};
@@ -135,62 +127,33 @@ __global__ void w4a16_gemv_simple_kernel(const KArgs a, int total_rows) {
     }
 }
 
-// Group size 64 (reference gemv_kernel_g64, kernels/cuda/gemv_cuda.cu:68-123): same QM_CUDA layout with zeros_w = zeros_width(IC, 64) and one
-// scale / zero point per 64 input channels.  One warp per output row, 128-bit loads, fp32 accumulation like the reference; kept simple
-// (QM_CUDA models are quantised with group 128, this slot exists for interface completeness).
-__global__ void w4a16_gemv_g64_kernel(const __half *__restrict__ x, const uint32_t *__restrict__ w, const uint32_t *__restrict__ zeros,
-                                      const __half *__restrict__ scales, __half *__restrict__ y, int M, int IC, int OC, int zeros_w) {
-    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    const int lane = threadIdx.x & 31;
-    if (row >= OC) return;
-    const uint4 *wrow = reinterpret_cast<const uint4 *>(w + (size_t)row * (IC / 8));
-    const uint32_t *zrow = zeros + (size_t)row * zeros_w;
-    const __half *srow = scales + (size_t)row * zeros_w * 8;
-    for (int m = 0; m < M; m++) {
-        const __half *xr = x + (size_t)m * IC;
-        float acc = 0.f;
-        for (int c = lane; c < IC / 32; c += 32) {  // 32 nibbles per uint4: two uint4 per group
-            const uint4 wv = wrow[c];
-            const int G = c >> 1;
-            const float sc = __half2float(srow[G]);
-            const float z = (float)((zrow[G >> 3] >> ((G & 7) * 4)) & 0xF);
-            const uint32_t words[4] = {wv.x, wv.y, wv.z, wv.w};
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-#pragma unroll
-                for (int i = 0; i < 8; i++) {
-                    const float q = (float)((words[j] >> (4 * i)) & 0xF);
-                    acc += (sc * (q - z)) * __half2float(xr[c * 32 + j * 8 + i]);
-                }
-            }
-        }
-        acc = warp_sum(acc);
-        if (lane == 0) y[(size_t)m * OC + row] = __float2half(acc);
-    }
-}
-
 }  // namespace
 
 cudaError_t launch_w4a16_gemv_g64(Ctx *ctx, const __half *x, const uint32_t *w, const uint32_t *zeros, const __half *scales, __half *y, int M, int IC, int OC) {
+    KArgs a = {};
+    a.seg[0].w = w;
+    a.seg[0].zeros = zeros;
+    a.seg[0].scales = scales;
+    a.seg[0].rows = OC;
+    a.nseg = 1;
+    a.IC = IC;
+    a.zeros_w = zeros_width(IC, 64);
+    a.sf_w = a.zeros_w * 8;
+    a.M = M;
+    a.ldx = IC;
+    a.x = x;
+    a.y = y;
+    a.epi = EPI_STORE_HALF;
+    a.ldy = OC;
     const int warps = 8;
-    w4a16_gemv_g64_kernel<<<(OC + warps - 1) / warps, warps * 32, 0, ctx->stream>>>(x, w, zeros, scales, y, M, IC, OC, zeros_width(IC, 64));
+    w4a16_gemv_simple_kernel<64><<<(OC + warps - 1) / warps, warps * 32, 0, ctx->stream>>>(a, OC);
     return cudaGetLastError();
 }
 
 // 2-D tensor map of one packed weight segment: uint32 [rows][IC/8], box = [box_rows][sg*16 words], no swizzle.
-// cuTensorMapEncodeTiled is a pure host-side encoder; it is reached through the runtime's driver entry point so the
-// library does not link libcuda directly.
 cudaError_t encode_w4_tmap(CUtensorMap *out, const void *w, int rows, int IC, int sg, int box_rows) {
-    typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
-                                 const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-    static EncodeFn fn = nullptr;
-    if (!fn) {
-        void *sym = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &q);
-        if (e != cudaSuccess || !sym) return e != cudaSuccess ? e : cudaErrorNotSupported;
-        fn = reinterpret_cast<EncodeFn>(sym);
-    }
+    const TmapEncodeFn fn = tmap_encoder();
+    if (!fn) return cudaErrorNotSupported;
     const cuuint64_t gdim[2] = {(cuuint64_t)(IC / 8), (cuuint64_t)rows};
     const cuuint64_t gstride[1] = {(cuuint64_t)(IC / 2)};
     const cuuint32_t box[2] = {(cuuint32_t)(sg * 16), (cuuint32_t)box_rows};
@@ -203,16 +166,8 @@ cudaError_t encode_w4_tmap(CUtensorMap *out, const void *w, int rows, int IC, in
 // 3-D view [group][row][64 B] of the same matrix: a box {64 B, box_rows, sg groups} lands in shared memory group-major with the rows of a group 64 B apart,
 // so the 16 rows x 64 B of one (tile, group) unit are 1 KiB contiguous and a quarter-warp's LDS.128 covers 128 consecutive bytes (no bank conflicts)
 cudaError_t encode_w4_tmap_units(CUtensorMap *out, const void *w, int rows, int IC, int sg, int box_rows) {
-    typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
-                                 const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-    static EncodeFn fn = nullptr;
-    if (!fn) {
-        void *sym = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &q);
-        if (e != cudaSuccess || !sym) return e != cudaSuccess ? e : cudaErrorNotSupported;
-        fn = reinterpret_cast<EncodeFn>(sym);
-    }
+    const TmapEncodeFn fn = tmap_encoder();
+    if (!fn) return cudaErrorNotSupported;
     const cuuint64_t gdim[3] = {16, (cuuint64_t)rows, (cuuint64_t)(IC / 128)};
     const cuuint64_t gstride[2] = {(cuuint64_t)(IC / 2), 64};
     const cuuint32_t box[3] = {16, (cuuint32_t)box_rows, (cuuint32_t)sg};
@@ -283,7 +238,7 @@ int pick_slice(int IC, int budget) {
 template <int NCOLS, int CW>
 cudaError_t launch_mma(Ctx *ctx, const KArgs &a_in, bool pdl) {
     KArgs a = a_in;
-    const int xw = NCOLS == 1 ? a.IC : a.sl * kW4Group;
+    const int xw = a.sl * kW4Group;
     if (!ring_fit<NCOLS, CW>(a.IC, xw, ctx->smem_optin, kStages)) return cudaErrorInvalidConfiguration;
     static DeviceOnce attr_once;  // per template instantiation
     if (attr_once.pending(ctx->device)) {
@@ -347,7 +302,7 @@ cudaError_t launch_w4a16_gemv_simple(Ctx *ctx, const W4GemvParams &p) {
     int rows;
     KArgs a = make_kargs(ctx, p, &rows);
     const int warps = 8;
-    w4a16_gemv_simple_kernel<<<(rows + warps - 1) / warps, warps * 32, 0, ctx->stream>>>(a, rows);
+    w4a16_gemv_simple_kernel<kW4Group><<<(rows + warps - 1) / warps, warps * 32, 0, ctx->stream>>>(a, rows);
     return cudaGetLastError();
 }
 
