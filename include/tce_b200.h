@@ -205,7 +205,9 @@ TCE_API int tce_sample(tce_ctx *ctx, float *logits_dev, int n_vocab, const int *
                        unsigned long long draw_index, int *token_host, int *cand_ids_host, float *cand_probs_host, int *cand_count_host);
 /* generate loop: decode `first_token` at position pos0, sample, feed the sample back, ... for at most n_predict tokens or until eos_id
  * is drawn or the context is full.  history_host (n_history recent tokens, oldest first) seeds the penalty window.  Only the generated
- * ids (4 bytes each) cross PCIe.  Single GPU (tp_size == 1).                                                                       */
+ * ids (4 bytes each) cross PCIe.  Single GPU (tp_size == 1).  KV rows, in slot 0: the loop decodes rows pos0 .. pos0 + *n_out - 1 (the
+ * last id is not decoded), as tce_llama_generate_batch does, and stops there when it ran out of budget or context.  After an eos_id stop
+ * the steps already queued behind it may also decode the eos id into row pos0 + *n_out (when that is below max_ctx); no row past it.    */
 TCE_API int tce_llama_generate(tce_llama *m, int first_token, int pos0, int n_predict, const tce_sampling *cfg, const int *history_host,
                                int n_history, int eos_id, int *out_tokens_host, int *n_out);
 /* ---- batched decode: up to TCE_LLAMA_MAX_BATCH sequences per step, each in its own KV-cache slot -------------------------------------
@@ -265,6 +267,20 @@ typedef struct tce_gen_request {
  * batch, slot (unreserved or repeated), first_token, pos0, n_predict < 0, n_history outside [0, max_ctx], out_stride below a clamped
  * n_predict or a NULL pointer; TCE_ERR_UNSUPPORTED for temp > 0 without 1 <= top_k <= 1024.                                           */
 TCE_API int tce_llama_generate_batch(tce_llama *m, int batch, const tce_gen_request *reqs, int *out_tokens_host, int out_stride, int *n_out);
+/* KV-cache row copy: rows src_pos .. src_pos + n - 1 of slot src_slot to rows dst_pos_host[i] .. dst_pos_host[i] + n - 1 of slot
+ * dst_slots_host[i], for each of the n_dst destinations, in every layer, K and V, every KV head.  The source rows are read once for all
+ * destinations.  The cache holds keys after RoPE, so a K row that moves by d = dst_pos - src_pos is rotated by d: rotate-half (dim j with
+ * j + 64, as the prompt pass applies it) with c = cos[|d|], s = sign(d) * sin[|d|] from the model's own tables (generated from rope_theta,
+ * the caller's, or the loaded tree's): r_j = x_j c_j - x_{j+64} s_j, r_{j+64} = x_{j+64} c_{j+64} + x_j s_{j+64}, every product and sum
+ * rounded on its own in fp32 (no FMA), then rounded to fp16.  V rows, and K rows with d = 0, are copied bit for bit.  With one destination
+ * in the source slot the ranges may overlap, in either direction: the result is that of copying through a temporary (memmove).  No other
+ * row of any slot changes.  n = 0 does nothing.  Forking a prompt into other slots is d = 0; the context shift of a full slot (keep rows
+ * [0, n_keep), drop the next n_discard, move the rest down) is one copy inside the slot with d = -n_discard.  Asynchronous on the context's
+ * stream, ordered with the decode steps and generate loops; the slot table does not change, so no captured graph is dropped.
+ * TCE_ERR_INVALID, before anything is enqueued, for n_dst outside [1, TCE_LLAMA_MAX_BATCH], n < 0, an unreserved slot, a source or
+ * destination range outside [0, max_ctx), two destinations whose ranges overlap in the same slot, or a destination that overlaps the source
+ * while n_dst > 1; TCE_ERR_UNSUPPORTED with tp_size > 1.                                                                                   */
+TCE_API int tce_llama_kv_copy(tce_llama *m, int src_slot, int src_pos, int n, int n_dst, const int *dst_slots_host, const int *dst_pos_host);
 TCE_API const float *tce_llama_logits(tce_llama *m);          /* device float[vocab] */
 TCE_API void *tce_llama_kv_cache(tce_llama *m, int layer, int which); /* which: 0 K, 1 V; half[KVH][max_ctx][hd] */
 TCE_API int tce_llama_kernels_per_step(tce_llama *m);

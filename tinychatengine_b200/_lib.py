@@ -86,6 +86,7 @@ SIGNATURES = {
     "tce_llama_prefill_batch": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 6),
     "tce_llama_score_batch": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 9),
     "tce_llama_generate_batch": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(GenRequest), C.c_void_p, C.c_int, C.c_void_p]),
+    "tce_llama_kv_copy": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "tce_llama_batch_logits": (C.c_void_p, [C.c_void_p]),
     "tce_llama_logits": (C.c_void_p, [C.c_void_p]),
     "tce_llama_kv_cache": (C.c_void_p, [C.c_void_p, C.c_int, C.c_int]),

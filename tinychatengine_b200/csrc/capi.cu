@@ -559,6 +559,12 @@ int tce_llama_generate_batch(tce_llama *m, int batch, const tce_gen_request *req
     cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->generate_batch(batch, reqs, out_tokens_host, out_stride, n_out, &err);
     return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_generate_batch", err);
 }
+int tce_llama_kv_copy(tce_llama *m, int src_slot, int src_pos, int n, int n_dst, const int *dst_slots_host, const int *dst_pos_host) {
+    if (!m || !dst_slots_host || !dst_pos_host) return fail(TCE_ERR_INVALID, "tce_llama_kv_copy: null argument");
+    std::string err;
+    cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->kv_copy(src_slot, src_pos, n, n_dst, dst_slots_host, dst_pos_host, &err);
+    return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_kv_copy", err);
+}
 const float *tce_llama_batch_logits(tce_llama *m) { return m ? reinterpret_cast<LlamaDecoder *>(m)->batch_logits() : nullptr; }
 const float *tce_llama_logits(tce_llama *m) { return m ? reinterpret_cast<LlamaDecoder *>(m)->logits() : nullptr; }
 void *tce_llama_kv_cache(tce_llama *m, int layer, int which) { return m ? reinterpret_cast<LlamaDecoder *>(m)->kv_cache(layer, which) : nullptr; }

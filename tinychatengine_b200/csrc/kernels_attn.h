@@ -57,6 +57,23 @@ struct AttnPrefillArgs {
     AttnPrefillSeq seq[kMaxPrefillSeqs];
 };
 cudaError_t launch_attn_prefill(Ctx *ctx, const AttnPrefillArgs &a);
+// KV-cache row copy (kv_copy.cu): rows src_pos..src_pos+n-1 of every (layer, K|V, head) slab of slot `src` to rows dst_pos[i].. of the same
+// slab of slot dst[i], for every destination.  K rows are rotated by d = dst_pos[i] - src_pos (rotate-half RoPE with cos[|d|] and
+// sign(d) * sin[|d|], fp32 without contraction, then round to fp16); V rows and K rows with d = 0 are byte copies.  head_dim 128, host-checked
+// arguments: the destinations do not overlap each other, and a destination overlaps the source only when it is the only one (in_place).
+constexpr int kMaxKvCopyDst = 8;
+struct KvCopyArgs {
+    const __half *src;              // slot base, [L][2][KVH][max_ctx][128]
+    __half *dst[kMaxKvCopyDst];     // slot bases
+    int dst_pos[kMaxKvCopyDst];
+    int n_dst, src_pos, n;
+    int num_kv_heads, max_ctx;
+    const float *cos, *sin;         // [max_ctx][128]
+    int in_place;                   // the one destination overlaps the source in its slot: memmove order, one CTA per slab
+    int reverse;                    // with in_place: the rows move up (d > 0), so the tiles run from the last one down
+};
+// n_slabs = L * 2 * KVH; n = 0 launches nothing
+cudaError_t launch_kv_copy(Ctx *ctx, const KvCopyArgs &a, int n_slabs);
 cudaError_t launch_embedding_rows(Ctx *ctx, const __half *table, const int *tokens, float *resid, int n, int E);
 cudaError_t launch_rmsnorm_rows_f32(Ctx *ctx, const float *x, const float *gamma, __half *y, int rows, int dim, float eps);
 

@@ -1100,4 +1100,51 @@ cudaError_t LlamaDecoder::generate_batch(int batch, const tce_gen_request *reqs,
     return cudaSuccess;
 }
 
+// ------------------------------------------------------------------------------------------------ KV-cache row copies
+// Forking a prompt's rows into other slots (d = 0) and shifting a slot's context down past n_keep (one destination, the source slot).  The
+// slot table and slot count stay as they are, so no cached graph is dropped; the launch is stream-ordered with the steps and loops.
+cudaError_t LlamaDecoder::kv_copy(int src_slot, int src_pos, int n, int n_dst, const int *dst_slots, const int *dst_pos, std::string *err) {
+    static_assert(kMaxKvCopyDst == TCE_LLAMA_MAX_BATCH, "one launch covers the destinations of a batch");
+    auto bad = [&](const char *m) {
+        if (err) *err = m;
+        return cudaErrorInvalidValue;
+    };
+    if (tp_ > 1) {
+        if (err) *err = "KV-cache slots are single-GPU (tp_size > 1)";
+        return cudaErrorNotSupported;
+    }
+    const int cap = cfg_.max_ctx;
+    if (n_dst < 1 || n_dst > kMaxKvCopyDst || !dst_slots || !dst_pos) return bad("n_dst outside [1, TCE_LLAMA_MAX_BATCH]");
+    if (n < 0) return bad("n < 0");
+    auto in_range = [&](int pos) { return pos >= 0 && pos <= cap && n <= cap - pos; };  // rows pos..pos+n-1 within [0, max_ctx)
+    if (src_slot < 0 || src_slot >= n_slots()) return bad("source slot not reserved");
+    if (!in_range(src_pos)) return bad("source rows outside [0, max_ctx)");
+    auto overlap = [&](int sa, int pa, int sb, int pb) { return sa == sb && (pa > pb ? pa - pb : pb - pa) < n; };
+    for (int i = 0; i < n_dst; i++) {
+        if (dst_slots[i] < 0 || dst_slots[i] >= n_slots()) return bad("destination slot not reserved");
+        if (!in_range(dst_pos[i])) return bad("destination rows outside [0, max_ctx)");
+        for (int j = 0; j < i; j++)
+            if (overlap(dst_slots[i], dst_pos[i], dst_slots[j], dst_pos[j])) return bad("two destinations overlap in one slot");
+        if (n_dst > 1 && overlap(dst_slots[i], dst_pos[i], src_slot, src_pos)) return bad("a destination overlaps the source (allowed for a single destination only)");
+    }
+    if (n == 0) return cudaSuccess;
+    KvCopyArgs a{};
+    auto base = [&](int slot) { return (__half *)kv_cache_slot(slot, 0, 0); };
+    a.src = base(src_slot);
+    for (int i = 0; i < n_dst; i++) {
+        a.dst[i] = base(dst_slots[i]);
+        a.dst_pos[i] = dst_pos[i];
+    }
+    a.n_dst = n_dst;
+    a.src_pos = src_pos;
+    a.n = n;
+    a.num_kv_heads = cfg_.num_kv_heads;
+    a.max_ctx = cap;
+    a.cos = d_cos_;
+    a.sin = d_sin_;
+    a.in_place = n_dst == 1 && dst_pos[0] != src_pos && overlap(dst_slots[0], dst_pos[0], src_slot, src_pos);
+    a.reverse = a.in_place && dst_pos[0] > src_pos;
+    return launch_kv_copy(ctx_, a, cfg_.num_layers * 2 * cfg_.num_kv_heads);
+}
+
 }  // namespace tce

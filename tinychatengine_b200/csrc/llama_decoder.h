@@ -79,6 +79,9 @@ class LlamaDecoder {
     const float *batch_logits();
     // generate loop of up to TCE_LLAMA_MAX_BATCH sequences: one batched step + one sampler launch (a block per row) per token
     cudaError_t generate_batch(int batch, const tce_gen_request *reqs, int *out_tokens_host, int out_stride, int *n_out, std::string *err);
+    // rows src_pos..src_pos+n-1 of src_slot to rows dst_pos[i].. of dst_slots[i] (every layer, K and V, K re-rotated by the position change):
+    // host-checked, then one launch on the context's stream (tce_llama_kv_copy)
+    cudaError_t kv_copy(int src_slot, int src_pos, int n, int n_dst, const int *dst_slots, const int *dst_pos, std::string *err);
     int kernels_per_step() const { return persistent_ ? 1 : 1 + 5 * cfg_.num_layers + 2; }
     // 0..3: row 0 of the kernel-per-op step's buffers (null until they exist)
     void *debug_buffer(int which) const {

@@ -281,19 +281,69 @@ class LlamaModel:
         return nxt.value
 
     def generate(self, first_token: int, pos0: int, n_predict: int, *, history=(), eos_id: int = -1, top_k=40, top_p=0.95, temp=0.8, repeat_penalty=1.1,
-                 frequency_penalty=0.0, presence_penalty=0.0, repeat_last_n=64, seed=0):
-        """Device generate loop (decode + sample per token, only the ids come back); defaults are the reference's opt_params."""
+                 frequency_penalty=0.0, presence_penalty=0.0, repeat_last_n=64, seed=0, n_keep=None):
+        """Device generate loop (decode + sample per token, only the ids come back); defaults are the reference's opt_params.  n_keep: when
+        the context fills before n_predict ids, shift slot 0 with kv_shift(0, max_ctx, n_keep) and carry on (the reference's opt_params.n_keep);
+        None stops at max_ctx."""
         import numpy as np
 
         cfg = _lib.Sampling(int(top_k), float(top_p), float(temp), float(repeat_penalty), float(frequency_penalty), float(presence_penalty),
                             int(repeat_last_n), int(seed))
-        hist = np.ascontiguousarray(np.asarray(list(history), dtype=np.int32))
-        out = np.zeros(max(1, n_predict), dtype=np.int32)
-        n = C.c_int(0)
-        _lib.check(self.ctx.L.tce_llama_generate(self.h, int(first_token), int(pos0), int(n_predict), C.byref(cfg),
-                                                 hist.ctypes.data_as(C.c_void_p) if hist.size else None, int(hist.size), int(eos_id),
-                                                 out.ctypes.data_as(C.c_void_p), C.byref(n)), "tce_llama_generate")
-        return out[:n.value].tolist()
+
+        def run(first, p0, budget, hist_ids):
+            hist = np.ascontiguousarray(np.asarray(list(hist_ids), dtype=np.int32))
+            out = np.zeros(max(1, budget), dtype=np.int32)
+            n = C.c_int(0)
+            _lib.check(self.ctx.L.tce_llama_generate(self.h, int(first), int(p0), int(budget), C.byref(cfg),
+                                                     hist.ctypes.data_as(C.c_void_p) if hist.size else None, int(hist.size), int(eos_id),
+                                                     out.ctypes.data_as(C.c_void_p), C.byref(n)), "tce_llama_generate")
+            return out[:n.value].tolist()
+
+        self._check_n_keep(n_keep)
+        ids = run(first_token, pos0, n_predict, history)
+        p0, seg = pos0, len(ids)
+        while self._context_full(n_keep, p0, seg, n_predict - (len(ids) - seg), ids, eos_id):
+            p0 = self.kv_shift(0, self.max_ctx, n_keep)
+            more = run(ids[-1], p0, n_predict - len(ids), (list(history) + ids)[-self.max_ctx:])
+            ids += more
+            seg = len(more)
+        return ids
+
+    def _check_n_keep(self, n_keep):
+        if n_keep is not None and not (0 <= n_keep and (self.max_ctx - n_keep) // 2 >= 1):
+            raise ValueError(f"n_keep = {n_keep}: the context shift needs 0 <= n_keep and (max_ctx - n_keep) // 2 >= 1 (max_ctx = {self.max_ctx})")
+
+    def _context_full(self, n_keep, pos0, n_seg, budget, ids, eos_id) -> bool:
+        """A generate call that returned n_seg ids from pos0 with this budget stopped only because the context filled (and n_keep asks to
+        shift and continue)."""
+        return n_keep is not None and n_seg > 0 and pos0 + n_seg == self.max_ctx and n_seg < budget and ids[-1] != eos_id
+
+    def kv_copy(self, src_slot: int, src_pos: int, n: int, dst_slots, dst_pos=None):
+        """Copy KV-cache rows src_pos .. src_pos + n - 1 of src_slot to rows dst_pos[i] .. of dst_slots[i] (up to MAX_BATCH destinations;
+        default: the same positions), every layer, K and V; K rows are re-rotated by the position change (tce_llama_kv_copy).  Asynchronous,
+        ordered with the other calls on the model's stream."""
+        dst_slots = [int(s) for s in dst_slots]
+        dst_pos = [int(src_pos)] * len(dst_slots) if dst_pos is None else [int(p) for p in dst_pos]
+        if len(dst_pos) != len(dst_slots):
+            raise ValueError("kv_copy: one destination position per destination slot")
+        arr = lambda v: (C.c_int * max(1, len(v)))(*v)
+        _lib.check(self.ctx.L.tce_llama_kv_copy(self.h, int(src_slot), int(src_pos), int(n), len(dst_slots), arr(dst_slots), arr(dst_pos)),
+                   "tce_llama_kv_copy")
+
+    def fork(self, src_slot: int, n_rows: int, dst_slots):
+        """Rows 0 .. n_rows - 1 of src_slot (a prompt pass's cache) into each of dst_slots at the same positions."""
+        self.kv_copy(src_slot, 0, n_rows, dst_slots)
+
+    def kv_shift(self, slot: int, n_past: int, n_keep: int, n_discard=None) -> int:
+        """Context shift of a slot holding n_past rows: keep [0, n_keep), drop the next n_discard (default (n_past - n_keep) // 2, the llama.cpp
+        rule) and move [n_keep + n_discard, n_past) down to n_keep, K re-rotated.  Returns the new n_past."""
+        if n_discard is None:
+            n_discard = (n_past - n_keep) // 2
+        if n_discard < 1 or n_keep < 0 or n_keep + n_discard > n_past:
+            raise ValueError(f"kv_shift: n_past = {n_past}, n_keep = {n_keep}, n_discard = {n_discard}: needs n_discard >= 1, n_keep >= 0 and "
+                             "n_keep + n_discard <= n_past")
+        self.kv_copy(slot, n_keep + n_discard, n_past - n_keep - n_discard, [slot], [n_keep])
+        return n_past - n_discard
 
     def prefill(self, tokens, pos0: int = 0, logits_host=None, slot: int = 0) -> int:
         """Prompt processing: all `tokens` (host ints) at positions pos0.. in one pass into KV-cache slot `slot`; returns the greedy next
@@ -378,10 +428,32 @@ class LlamaModel:
             r += m
         return out
 
-    def generate_batch(self, requests) -> list[list[int]]:
+    def generate_batch(self, requests, n_keep=None) -> list[list[int]]:
         """Device generate loop of up to MAX_BATCH sequences (one batched step + one sampler launch per token, only the ids come back).
         Each request is a dict with first_token, pos0, slot, n_predict and optional history, eos_id and the sampling fields of generate(),
-        with the same defaults (the reference's opt_params)."""
+        with the same defaults (the reference's opt_params).  n_keep: a sequence that stops only because its slot filled is shifted with
+        kv_shift(slot, max_ctx, n_keep) and continues in the next call, with the rest of its budget; None stops it at max_ctx."""
+        self._check_n_keep(n_keep)
+        outs = self._generate_batch(requests)
+        if n_keep is None:
+            return outs
+        ids = [list(o) for o in outs]
+        active = list(enumerate(requests))
+        while True:
+            cont = []
+            for (i, r), seg in zip(active, outs):
+                if self._context_full(n_keep, r["pos0"], len(seg), r["n_predict"], ids[i], r.get("eos_id", -1)):
+                    p0 = self.kv_shift(r["slot"], self.max_ctx, n_keep)
+                    hist = (list(requests[i].get("history", ())) + ids[i])[-self.max_ctx:]
+                    cont.append((i, dict(r, first_token=ids[i][-1], pos0=p0, n_predict=r["n_predict"] - len(seg), history=hist)))
+            if not cont:
+                return ids
+            active = cont
+            outs = self._generate_batch([r for _, r in active])
+            for (i, _), seg in zip(active, outs):
+                ids[i] += seg
+
+    def _generate_batch(self, requests) -> list[list[int]]:
         defaults = dict(history=(), eos_id=-1, top_k=40, top_p=0.95, temp=0.8, repeat_penalty=1.1, frequency_penalty=0.0, presence_penalty=0.0,
                         repeat_last_n=64, seed=0)
         n = len(requests)
