@@ -102,7 +102,9 @@ TCE_API int tce_opt_int8_attention(tce_ctx *ctx, const void *q8, const void *k8,
  *   k_cache, v_cache half[KVH][max_ctx][head_dim]  appended in place at *pos
  *   cos, sin float[max_ctx][head_dim]  (rotary_emb/cos_cached layout)
  *   pos   device int: index of the current token == number of tokens already cached
- *   out   half[H*head_dim]                                                                                 */
+ *   out   half[H*head_dim]
+ * The split workspace belongs to the context: the first call, and a call with a larger shape than any before it, allocates it, which
+ * synchronises the device (so such a call cannot run inside a stream capture).                                                */
 TCE_API int tce_attn_decode(tce_ctx *ctx, const void *qkv, void *k_cache, void *v_cache, const float *cos,
                             const float *sin, const int *pos, void *out, float alpha, int num_heads, int num_kv_heads,
                             int head_dim, int max_ctx);

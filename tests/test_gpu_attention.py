@@ -196,3 +196,107 @@ def test_attention_kernels_against_reference_module_fixture(ctx, golden_dir):
     amax = np.abs(ref_core.reshape(T, -1, 32)).max(-1, keepdims=True)
     tol = (amax / 254 * 1.05 + 2e-3 * np.abs(ref_core).max()) * np.ones((1, 1, 32), np.float32)
     assert np.all(np.abs(core - ref_core).reshape(T, -1, 32) <= tol)
+
+
+def _decode_case(H, KVH, past, max_ctx, seed):
+    """Seeded inputs of one tce_attn_decode call and the fp32 GQA oracle's answer: (qkv, K cache, V cache, cos, sin, want)."""
+    from oracle import capi
+
+    rng = np.random.default_rng(seed)
+    cosb, sinb = capi.rope_tables(max_ctx, HD, 500000.0)
+    qkv = rng.standard_normal((H + 2 * KVH) * HD).astype(np.float16)
+    pk = (rng.standard_normal((KVH, past, HD)) * 0.7).astype(np.float16)
+    pv = rng.standard_normal((KVH, past, HD)).astype(np.float16)
+    f = qkv.astype(np.float32)[None]
+    want, _, _ = capi.llama_attention_core(f[:, : H * HD], f[:, H * HD: (H + KVH) * HD], f[:, (H + KVH) * HD:], pk.astype(np.float32) if past else None,
+                                           pv.astype(np.float32) if past else None, capi.causal_mask(1, past), cosb, sinb, 1.0 / np.sqrt(HD), H, KVH, HD)
+    dev = torch.device("cuda", 0)
+    kc = torch.full((KVH, max_ctx, HD), float("nan"), dtype=torch.float16, device=dev)
+    vc = torch.full_like(kc, float("nan"))
+    kc[:, :past] = torch.from_numpy(pk).to(dev)
+    vc[:, :past] = torch.from_numpy(pv).to(dev)
+    return torch.from_numpy(qkv).to(dev), kc, vc, torch.from_numpy(cosb).to(dev), torch.from_numpy(sinb).to(dev), want[0]
+
+
+def _decode(c, case, H, KVH, past, max_ctx):
+    qkv, kc, vc, cosb, sinb, _ = case
+    out = torch.zeros(H * HD, dtype=torch.float16, device=qkv.device)
+    pos = torch.tensor([past], dtype=torch.int32, device=qkv.device)
+    c.attn_decode(qkv, kc, vc, cosb, sinb, pos, out, 1.0 / np.sqrt(HD), H, KVH, HD, max_ctx)
+    torch.cuda.synchronize()
+    return out.cpu()
+
+
+def test_decode_and_opt_attention_interleaved_on_one_context():
+    """tce_opt_int8_attention and a multi-split tce_attn_decode on one context share no memory: each gives the bits it gives on a fresh
+    context, before and after the other."""
+    from tinychatengine_b200.runtime import Context
+
+    H8, hd, past8 = 12, 64, 300
+    rnd = lambda shape, seed: torch.from_numpy(np.random.default_rng(seed).integers(-127, 128, shape, dtype=np.int8)).cuda()
+    q, k, v = rnd((1, H8 * hd), 1), rnd((1, H8 * hd), 2), rnd((1, H8 * hd), 3)
+    pk, pv = rnd((H8, past8, hd), 4), rnd((H8, past8, hd), 5)
+
+    def opt(c):
+        fk = torch.zeros((H8, past8 + 1, hd), dtype=torch.int8, device="cuda")
+        return c.opt_int8_attention(q, k, v, pk, pv, fk, torch.zeros_like(fk), None, 0.0007, 0.011, past8, H8, hd).cpu()
+
+    H, KVH, past, max_ctx = 32, 8, 3000, 4096
+    case = _decode_case(H, KVH, past, max_ctx, 11)
+    fresh = [Context(0) for _ in range(2)]
+    try:
+        opt_fresh, dec_fresh = opt(fresh[0]), _decode(fresh[1], case, H, KVH, past, max_ctx)
+    finally:
+        for c in fresh:
+            c.close()
+    c = Context(0)
+    try:
+        opt1 = opt(c)
+        dec = _decode(c, case, H, KVH, past, max_ctx)
+        opt2 = opt(c)
+    finally:
+        c.close()
+    assert torch.equal(opt1, opt_fresh) and torch.equal(opt2, opt_fresh)
+    assert torch.equal(dec, dec_fresh)
+
+
+def test_decode_workspace_grows():
+    """A short-context call sizes the context's split workspace; a later long-context call on the same context grows it."""
+    from tinychatengine_b200.runtime import Context
+
+    c = Context(0)
+    try:
+        for H, KVH, past, max_ctx in ((8, 2, 100, 256), (32, 8, 4000, 4096)):
+            case = _decode_case(H, KVH, past, max_ctx, past)
+            got, want = _decode(c, case, H, KVH, past, max_ctx).float().numpy(), case[-1]
+            assert np.all(np.isfinite(got))
+            assert np.abs(got - want).max() / max(np.abs(want).max(), 1e-6) <= 3e-3, (H, past)
+    finally:
+        c.close()
+
+
+@pytest.mark.parametrize("H,KVH,hd,max_ctx,chunk,status", [
+    (8, 2, 64, 64, None, -2),      # head_dim 64: TCE_ERR_UNSUPPORTED
+    (6, 4, 128, 64, None, -1),     # H % KVH != 0: TCE_ERR_INVALID
+    (6, 2, 128, 64, None, -3),     # 3 query heads per KV head: no kernel, TCE_ERR_CUDA
+    (128, 128, 128, 1025, 1, -3),  # H x nsplit = 128 x 1025 split records: more than one call takes, TCE_ERR_CUDA
+])
+def test_decode_refusals_write_nothing(H, KVH, hd, max_ctx, chunk, status):
+    from tinychatengine_b200.runtime import Context, _ptr
+
+    c = Context(0)
+    try:
+        if chunk is not None:
+            c.set_option("attn_chunk", chunk)
+        g = torch.Generator(device="cuda").manual_seed(H + max_ctx)
+        rnd = lambda *shape: torch.randn(shape, generator=g, device="cuda").half()
+        qkv, kc, vc, out = rnd((H + 2 * KVH) * hd), rnd(KVH, max_ctx, hd), rnd(KVH, max_ctx, hd), rnd(H * hd)
+        cosb, sinb = torch.ones((max_ctx, hd), device="cuda"), torch.zeros((max_ctx, hd), device="cuda")
+        pos = torch.tensor([max_ctx - 1], dtype=torch.int32, device="cuda")
+        before = [t.clone() for t in (out, kc, vc)]
+        rc = c.L.tce_attn_decode(c.h, _ptr(qkv), _ptr(kc), _ptr(vc), _ptr(cosb), _ptr(sinb), _ptr(pos), _ptr(out), 1.0 / np.sqrt(hd), H, KVH, hd, max_ctx)
+        torch.cuda.synchronize()
+        assert rc == status, c.L.tce_last_error()
+        assert all(torch.equal(a, b) for a, b in zip(before, (out, kc, vc)))
+    finally:
+        c.close()

@@ -8,72 +8,277 @@
 //
 //  * KV cache is [KVH][max_ctx][128] fp16 per layer, appended IN PLACE at `pos` (no ping-pong copy, no V
 //    transpose);
-//  * grid = (KVH, ceil(max_ctx/chunk)): a CTA owns `chunk` cached positions of one KV head and serves the
-//    H/KVH query heads that share it, so each cached byte is read once per token;
-//  * its K and V slabs (contiguous chunk*256 B each) are pulled into shared memory by two TMA bulk copies
-//    issued up front -- the whole cache of the layer is in flight at once, the kernel is HBM-bound;
-//  * fp32 RoPE / scores / softmax statistics / PV accumulation; split results are merged flash-decoding
-//    style by the last CTA of each KV head to arrive (fixed order, deterministic).
-#include "attention_impl.cuh"
-#include "kernels.h"
+//  * grid = (KVH, ceil(max_ctx/chunk), batch): a CTA owns `chunk` cached positions of one KV head of one sequence and
+//    serves the H/KVH query heads that share it, so each cached byte is read once per token;
+//  * its K and V rows are pulled into padded shared rows by 16-byte cp.async copies issued up front -- the whole cache of
+//    the layer is in flight at once, the kernel is HBM-bound;
+//  * the H/KVH query heads are the (up to 8) columns of one MMA tile: scores and P.V run on mma.sync m16n8k16 with fp16
+//    operands (q * alpha, K, P, V) and fp32 accumulation; a scalar version of the two products cost ~6 of the kernel's ~18 us;
+//  * fp32 RoPE / softmax statistics; split results are merged flash-decoding style through global partial records by the
+//    last CTA of each KV head to arrive (fixed order, deterministic).
+// A thread-block-cluster flavour -- one cluster of 8 / 16 CTAs per KV head, partials merged over distributed shared memory --
+// was implemented and measured: 2.2 us per layer SLOWER (cluster co-scheduling + two cluster barriers), so it was removed.
+#include "common.cuh"
+#include "kernels_attn.h"
 
 namespace tce {
 namespace {
 
-using namespace attn;
+constexpr int HD = 128;  // head_dim (every Llama config in llm/include/model.h:71-83)
+constexpr int kAttnThreads = 256;
+constexpr int kPitch = HD + 8;  // halves per K/V/Q row in shared memory: 272-byte rows keep ldmatrix and fragment loads conflict free
 
+int chunk_rows(int chunk) { return chunk > 0 ? chunk : 128; }  // cached positions per CTA; attn_chunk <= 0 selects the default
+
+inline __host__ __device__ int rows16(int chunk) { return (chunk + 15) & ~15; }
+inline __host__ __device__ int p_floats(int chunk) { return rows16(chunk) > HD + 8 ? rows16(chunk) : HD + 8; }
+// shared memory of one CTA; the word after it elects the last split
+inline __host__ __device__ size_t smem_bytes(int nrep, int chunk) {
+    size_t b = (size_t)2 * rows16(chunk) * kPitch * 2;  // K, V slabs (padded rows)
+    b += (size_t)8 * kPitch * 2;                         // q, fp16, 8 head rows (rows >= nrep are zero)
+    b += (size_t)nrep * p_floats(chunk) * 4;             // scores fp32
+    b += (size_t)nrep * rows16(chunk) * 2;               // probabilities fp16
+    b += (size_t)nrep * HD * 4;                          // o
+    b += (size_t)2 * nrep * 16 * 4;                      // stats [2][nrep][16]
+    return (b + 15) & ~(size_t)15;
+}
+
+// one (kv head, split, sequence) work item per CTA
 template <int NREP>
 __global__ void __launch_bounds__(kAttnThreads, 1) attn_decode_kernel(const __grid_constant__ AttnDecodeArgs a) {
+    static_assert(NREP <= 8, "the query heads of one KV head ride in the 8 MMA columns");
     extern __shared__ __align__(128) uint8_t smem[];
-    uint64_t *bar = reinterpret_cast<uint64_t *>(smem + smem_bytes(NREP, a.chunk));
-    int *flag = reinterpret_cast<int *>(bar + 2);
-    const int tid = threadIdx.x;
-    if (tid == 0) {
-        mbar_init(&bar[0], 1);
-        mbar_init(&bar[1], 1);
-        mbar_fence_init();
+    const int chunk = a.chunk;
+    const int R16 = rows16(chunk);
+    __half *sK = reinterpret_cast<__half *>(smem);                       // [R16][kPitch]
+    __half *sV = sK + (size_t)R16 * kPitch;                              // [R16][kPitch]
+    __half *sQ = sV + (size_t)R16 * kPitch;                              // [8][kPitch] rotated * alpha, rows >= NREP zero
+    float *sP = reinterpret_cast<float *>(sQ + 8 * kPitch);              // [NREP][p_floats] scores
+    __half *sPh = reinterpret_cast<__half *>(sP + NREP * p_floats(chunk));  // [NREP][R16] probabilities
+    float *sO = reinterpret_cast<float *>(sPh + NREP * R16);             // [NREP][HD] unnormalised output of this split
+    float *sStat = sO + NREP * HD;                                       // [NREP][16] max | [NREP][16] sum
+    int *flag = reinterpret_cast<int *>(smem + smem_bytes(NREP, chunk));
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
+    const int kvh = blockIdx.x, split = blockIdx.y, seq = blockIdx.z;
+    pdl_launch_dependents();
+    pdl_wait();  // q|k|v (and the request records) come from the previous kernels; the cache was written by earlier steps
+
+    // ---- this sequence's position and K / V slabs: its request's slot, or the caller's cache ----
+    int pos;
+    __half *Kc, *Vc;
+    if (a.req) {
+        const int4 r = reinterpret_cast<const int4 *>(a.req)[seq];  // one load: the position is not left behind the slot-table lookup
+        if (r.w == 0) return;  // refused entry (uniform over the CTA)
+        __half *slot = a.slots[r.z];
+        Kc = slot + a.k_off;
+        Vc = slot + a.v_off;
+        pos = r.y;
+    } else {
+        Kc = a.k_cache;
+        Vc = a.v_cache;
+        pos = *a.pos;
+    }
+    Kc += (size_t)kvh * a.max_ctx * HD;
+    Vc += (size_t)kvh * a.max_ctx * HD;
+    const __half *qkv = a.qkv + (size_t)seq * a.qkv_stride;
+    __half *out = a.out + (size_t)seq * a.out_stride;
+    float *ws = a.ws + (size_t)seq * a.num_heads * a.nsplit_max * (HD + 2);  // [H][nsplit_max][HD + 2]
+    unsigned *counters = a.counters + (size_t)seq * a.num_kv_heads;
+
+    const int T = pos + 1;  // visible positions
+    const int t0 = min(T, split * chunk);
+    if (t0 >= T) return;  // empty split
+    const int t1 = min(T, t0 + chunk);
+    const int nrows = t1 - t0;
+    const bool owns_new = (pos >= t0 && pos < t1);
+    const int ncached = owns_new ? nrows - 1 : nrows;  // rows that already live in the cache
+    const int mtiles = (nrows + 15) >> 4;
+
+    // ---- cached K/V rows -> padded shared rows (16-byte cp.async, whole slab in flight at once) ----
+    for (int e = tid; e < ncached * (HD / 8); e += kAttnThreads) {
+        const int r = e >> 4, c8 = e & 15;
+        cp_async16(sK + (size_t)r * kPitch + c8 * 8, Kc + (size_t)(t0 + r) * HD + c8 * 8);
+        cp_async16(sV + (size_t)r * kPitch + c8 * 8, Vc + (size_t)(t0 + r) * HD + c8 * 8);
+    }
+    // rows of the last 16-row tile beyond nrows: finite zeros (their probabilities are zero, 0 * garbage must not be NaN)
+    for (int e = tid; e < (mtiles * 16 - nrows) * (HD / 8); e += kAttnThreads) {
+        const int r = nrows + (e >> 4), c8 = e & 15;
+        *reinterpret_cast<uint4 *>(sK + (size_t)r * kPitch + c8 * 8) = make_uint4(0, 0, 0, 0);
+        *reinterpret_cast<uint4 *>(sV + (size_t)r * kPitch + c8 * 8) = make_uint4(0, 0, 0, 0);
+    }
+
+    // ---- RoPE (llm/src/ops/RotaryPosEmb.cc:7-69 rotate-half) on the NREP query heads and, if this CTA owns the new position, on
+    //      the new key; fp32 math, tables [max_ctx][HD] fp32; q * alpha is rounded to fp16 for the tensor-core product ----
+    const float *cosr = a.cos + (size_t)pos * HD, *sinr = a.sin + (size_t)pos * HD;
+    const int H = a.num_heads, KVH = a.num_kv_heads;
+    for (int i = tid; i < 8 * HD; i += kAttnThreads) {
+        const int r = i / HD, j = i % HD;
+        float v = 0.f;
+        if (r < NREP) {
+            const __half *q = qkv + (size_t)(kvh * NREP + r) * HD;
+            const float x = __half2float(q[j]);
+            const float xr = (j < HD / 2) ? -__half2float(q[j + HD / 2]) : __half2float(q[j - HD / 2]);
+            v = (x * cosr[j] + xr * sinr[j]) * a.alpha;
+        }
+        sQ[r * kPitch + j] = __float2half(v);
+    }
+    if (owns_new && tid < HD) {
+        const int j = tid;
+        const __half *k = qkv + (size_t)H * HD + (size_t)kvh * HD;
+        const __half *v = qkv + (size_t)(H + KVH) * HD + (size_t)kvh * HD;
+        const float x = __half2float(k[j]);
+        const float xr = (j < HD / 2) ? -__half2float(k[j + HD / 2]) : __half2float(k[j - HD / 2]);
+        const __half kh = __float2half(x * cosr[j] + xr * sinr[j]);
+        sK[(size_t)(nrows - 1) * kPitch + j] = kh;  // row `pos` of the slab; the copies above never touch it
+        sV[(size_t)(nrows - 1) * kPitch + j] = v[j];
+        Kc[(size_t)pos * HD + j] = kh;              // in-place append
+        Vc[(size_t)pos * HD + j] = v[j];
+    }
+    cp_async_wait_all();
+    __syncthreads();
+
+    // ---- scores on the tensor cores: S^T[key][head] = K[key][:] . q[head][:]  (m16n8k16: 16 keys x 8 head columns x 16 dims) ----
+    {
+        uint32_t qb[8][2];  // B operand: q[head = g][dims], all 8 k-steps
+#pragma unroll
+        for (int ks = 0; ks < 8; ks++) {
+            qb[ks][0] = *reinterpret_cast<const uint32_t *>(sQ + g * kPitch + ks * 16 + qd * 2);
+            qb[ks][1] = *reinterpret_cast<const uint32_t *>(sQ + g * kPitch + ks * 16 + 8 + qd * 2);
+        }
+        for (int mt = warp; mt < mtiles; mt += kAttnThreads / 32) {
+            float c[4] = {0.f, 0.f, 0.f, 0.f};
+            const __half *arow = sK + (size_t)(mt * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * kPitch + (lane >> 4) * 8;
+#pragma unroll
+            for (int ks = 0; ks < 8; ks++) {
+                uint32_t a0, a1, a2, a3;
+                ldmatrix_x4(a0, a1, a2, a3, arow + ks * 16);
+                mma_m16n8k16(c, a0, a1, a2, a3, qb[ks][0], qb[ks][1]);
+            }
+            const int key = mt * 16 + g, h0 = qd * 2;  // c0,c1: (key, heads h0, h0+1); c2,c3: (key + 8, ...)
+            if (h0 < NREP) {
+                if (key < nrows) sP[h0 * p_floats(chunk) + key] = c[0];
+                if (key + 8 < nrows) sP[h0 * p_floats(chunk) + key + 8] = c[2];
+            }
+            if (h0 + 1 < NREP) {
+                if (key < nrows) sP[(h0 + 1) * p_floats(chunk) + key] = c[1];
+                if (key + 8 < nrows) sP[(h0 + 1) * p_floats(chunk) + key + 8] = c[3];
+            }
+        }
     }
     __syncthreads();
-    pdl_launch_dependents();
-    pdl_wait();  // qkv of this token comes from the previous kernel; the cache was written by earlier steps
-    uint32_t parity = 0;
-    attn_item<NREP>(a, smem, bar, flag, parity, blockIdx.x, blockIdx.y, tid, *a.pos, [] { __syncthreads(); });
-}
 
-// grid (KVH, nsplit, batch): the work item of the single-sequence kernel on sequence blockIdx.z's rows, slot and position
-template <int NREP>
-__global__ void __launch_bounds__(kAttnThreads, 1) attn_decode_batch_kernel(const __grid_constant__ AttnBatchArgs b) {
-    extern __shared__ __align__(128) uint8_t smem[];
-    uint64_t *bar = reinterpret_cast<uint64_t *>(smem + smem_bytes(NREP, b.base.chunk));
-    int *flag = reinterpret_cast<int *>(bar + 2);
-    const int tid = threadIdx.x, seq = blockIdx.z;
-    if (tid == 0) {
-        mbar_init(&bar[0], 1);
-        mbar_init(&bar[1], 1);
-        mbar_fence_init();
+    // ---- softmax statistics of this split (fp32): m = max, p = exp(s - m) (kept as fp16 for the P.V product), l = sum p ----
+    float m_loc[NREP], l_loc[NREP];
+#pragma unroll
+    for (int r = 0; r < NREP; r++) {
+        float m = -INFINITY;
+        for (int i = tid; i < nrows; i += kAttnThreads) m = fmaxf(m, sP[r * p_floats(chunk) + i]);
+        m = warp_max(m);
+        if (lane == 0) sStat[r * 16 + warp] = m;
     }
     __syncthreads();
-    pdl_launch_dependents();
-    pdl_wait();  // the request records and q|k|v come from the previous kernels of the step
-    const int *r = b.req + 4 * seq;
-    if (r[3] == 0) return;  // refused entry (uniform over the CTA)
-    AttnDecodeArgs a = b.base;
-    a.qkv += (size_t)seq * b.qkv_stride;
-    a.out += (size_t)seq * b.out_stride;
-    __half *slot = b.slots[r[2]];
-    a.k_cache = slot + b.k_off;
-    a.v_cache = slot + b.v_off;
-    a.ws += (size_t)seq * a.num_heads * a.nsplit_max * (HD + 2);
-    a.counters += (size_t)seq * a.num_kv_heads;
-    uint32_t parity = 0;
-    attn_item<NREP>(a, smem, bar, flag, parity, blockIdx.x, blockIdx.y, tid, r[1], [] { __syncthreads(); });
+#pragma unroll
+    for (int r = 0; r < NREP; r++) {
+        float m = sStat[r * 16];
+#pragma unroll
+        for (int w = 1; w < kAttnThreads / 32; w++) m = fmaxf(m, sStat[r * 16 + w]);
+        m_loc[r] = m;
+        float l = 0.f;
+        for (int i = tid; i < mtiles * 16; i += kAttnThreads) {
+            float p = 0.f;
+            if (i < nrows) {
+                p = __expf(sP[r * p_floats(chunk) + i] - m);
+                l += p;
+            }
+            sPh[r * R16 + i] = __float2half(p);
+        }
+        l = warp_sum(l);
+        if (lane == 0) sStat[NREP * 16 + r * 16 + warp] = l;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < NREP; r++) {
+        float l = 0.f;
+#pragma unroll
+        for (int w = 0; w < kAttnThreads / 32; w++) l += sStat[NREP * 16 + r * 16 + w];
+        l_loc[r] = l;
+    }
+
+    // ---- O[head][dim] = sum_key P[head][key] V[key][dim] on the tensor cores: warp w owns dims 16w..16w+15 over all keys ----
+    {
+        float o0[4] = {0.f, 0.f, 0.f, 0.f}, o1[4] = {0.f, 0.f, 0.f, 0.f};
+        const int dbase = warp * 16;
+        for (int kt = 0; kt < mtiles; kt++) {
+            uint32_t a0 = 0u, a2 = 0u;  // A = P: rows = heads (g < NREP valid, rows 8..15 zero), k = 16 keys
+            if (g < NREP) {
+                a0 = *reinterpret_cast<const uint32_t *>(sPh + g * R16 + kt * 16 + qd * 2);
+                a2 = *reinterpret_cast<const uint32_t *>(sPh + g * R16 + kt * 16 + 8 + qd * 2);
+            }
+            uint32_t b0, b1, b2, b3;
+            ldmatrix_x4_t(b0, b1, b2, b3, sV + (size_t)(kt * 16 + (lane & 15)) * kPitch + dbase + (lane >> 4) * 8);
+            mma_m16n8k16(o0, a0, 0u, a2, 0u, b0, b1);
+            mma_m16n8k16(o1, a0, 0u, a2, 0u, b2, b3);
+        }
+        if (g < NREP) {  // c0,c1: (head g, dims 2qd, 2qd+1)
+            sO[g * HD + dbase + qd * 2] = o0[0];
+            sO[g * HD + dbase + qd * 2 + 1] = o0[1];
+            sO[g * HD + dbase + 8 + qd * 2] = o1[0];
+            sO[g * HD + dbase + 8 + qd * 2 + 1] = o1[1];
+        }
+    }
+    __syncthreads();
+
+    // ---- per-split result (unnormalised o, m, l) ----
+    const int nsplit_active = (T + chunk - 1) / chunk;
+    const int wstride = HD + 2;
+    for (int i = tid; i < NREP * HD; i += kAttnThreads) {
+        const int r = i / HD, d = i % HD;
+        const float o = sO[i];
+        const int head = kvh * NREP + r;
+        if (nsplit_active == 1) {
+            out[(size_t)head * HD + d] = __float2half(o / l_loc[r]);
+        } else {
+            float *rec = ws + ((size_t)head * a.nsplit_max + split) * wstride;
+            rec[d] = o;
+            if (d == 0) {
+                rec[HD] = m_loc[r];
+                rec[HD + 1] = l_loc[r];
+            }
+        }
+    }
+    if (nsplit_active == 1) return;
+
+    // ---- merge: the last split of this KV head to arrive combines all of them in split order ----
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) {
+        const unsigned prev = atomicAdd(&counters[kvh], 1u);
+        const int last = (prev == (unsigned)(nsplit_active - 1)) ? 1 : 0;
+        if (last) counters[kvh] = 0;
+        *flag = last;
+    }
+    __syncthreads();
+    if (*flag == 0) return;
+    __threadfence();
+    for (int i = tid; i < NREP * HD; i += kAttnThreads) {
+        const int r = i / HD, d = i % HD;
+        const int head = kvh * NREP + r;
+        const float *base = ws + (size_t)head * a.nsplit_max * wstride;
+        float m = -INFINITY;
+        for (int s = 0; s < nsplit_active; s++) m = fmaxf(m, ldg_cg_f32(base + (size_t)s * wstride + HD));
+        float l = 0.f, o = 0.f;
+        for (int s = 0; s < nsplit_active; s++) {
+            const float w = __expf(ldg_cg_f32(base + (size_t)s * wstride + HD) - m);
+            l += w * ldg_cg_f32(base + (size_t)s * wstride + HD + 1);
+            o += w * ldg_cg_f32(base + (size_t)s * wstride + d);
+        }
+        out[(size_t)head * HD + d] = __float2half(o / l);
+    }
 }
 
-size_t attn_smem_bytes(int nrep, int chunk) { return smem_bytes(nrep, chunk) + 2 * sizeof(uint64_t) + 16; }
-
 template <int NREP>
-cudaError_t launch(Ctx *ctx, const AttnDecodeArgs &a, bool pdl) {
-    const size_t smem = attn_smem_bytes(NREP, a.chunk);
+cudaError_t launch(Ctx *ctx, const AttnDecodeArgs &a, int batch, bool pdl) {
+    const size_t smem = smem_bytes(NREP, a.chunk) + 16;  // + the last-split flag
     static DeviceOnce attr_once;
     if (attr_once.pending(ctx->device)) {
         cudaError_t e = cudaFuncSetAttribute(attn_decode_kernel<NREP>, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->smem_optin);
@@ -82,7 +287,7 @@ cudaError_t launch(Ctx *ctx, const AttnDecodeArgs &a, bool pdl) {
     }
     if ((int)smem > ctx->smem_optin) return cudaErrorInvalidConfiguration;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(a.num_kv_heads, a.nsplit_max);
+    cfg.gridDim = dim3(a.num_kv_heads, a.nsplit_max, batch);
     cfg.blockDim = dim3(kAttnThreads);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = ctx->stream;
@@ -94,70 +299,28 @@ cudaError_t launch(Ctx *ctx, const AttnDecodeArgs &a, bool pdl) {
     return cudaLaunchKernelEx(&cfg, attn_decode_kernel<NREP>, a);
 }
 
-template <int NREP>
-cudaError_t launch_batch(Ctx *ctx, const AttnBatchArgs &b, int batch, bool pdl) {
-    const size_t smem = attn_smem_bytes(NREP, b.base.chunk);
-    static DeviceOnce attr_once;
-    if (attr_once.pending(ctx->device)) {
-        cudaError_t e = cudaFuncSetAttribute(attn_decode_batch_kernel<NREP>, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->smem_optin);
-        if (e != cudaSuccess) return e;
-        attr_once.done(ctx->device);
-    }
-    if ((int)smem > ctx->smem_optin) return cudaErrorInvalidConfiguration;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(b.base.num_kv_heads, b.base.nsplit_max, batch);
-    cfg.blockDim = dim3(kAttnThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, attn_decode_batch_kernel<NREP>, b);
-}
-
 }  // namespace
 
-size_t attn_batch_ws_floats(int num_heads, int max_ctx, int chunk) {
-    if (chunk <= 0) chunk = 128;
+size_t attn_decode_ws_floats(int num_heads, int max_ctx, int chunk) {
+    chunk = chunk_rows(chunk);
     return (size_t)num_heads * ((max_ctx + chunk - 1) / chunk) * (HD + 2);
 }
 
-cudaError_t launch_attn_decode_batch(Ctx *ctx, AttnBatchArgs b, int batch, bool pdl) {
-    AttnDecodeArgs &a = b.base;
+cudaError_t launch_attn_decode(Ctx *ctx, const AttnDecodeArgs &args, int batch, bool pdl) {
+    AttnDecodeArgs a = args;
     if (a.head_dim != HD) return cudaErrorNotSupported;
     if (a.num_heads % a.num_kv_heads || batch < 1) return cudaErrorInvalidValue;
-    if (a.chunk <= 0) a.chunk = 128;
+    a.chunk = chunk_rows(a.chunk);
     a.nsplit_max = (a.max_ctx + a.chunk - 1) / a.chunk;
     // per sequence: its own partial records and split counters, in the caller's workspace
-    if (!a.ws || !a.counters || (size_t)batch * attn_batch_ws_floats(a.num_heads, a.max_ctx, a.chunk) > b.ws_floats ||
-        (size_t)batch * a.num_kv_heads > b.n_counters)
+    if (!a.ws || !a.counters || (size_t)batch * attn_decode_ws_floats(a.num_heads, a.max_ctx, a.chunk) > a.ws_floats ||
+        (size_t)batch * a.num_kv_heads > a.n_counters)
         return cudaErrorInvalidValue;
     switch (a.num_heads / a.num_kv_heads) {
-        case 1: return launch_batch<1>(ctx, b, batch, pdl);
-        case 2: return launch_batch<2>(ctx, b, batch, pdl);
-        case 4: return launch_batch<4>(ctx, b, batch, pdl);
-        case 8: return launch_batch<8>(ctx, b, batch, pdl);
-        default: return cudaErrorNotSupported;
-    }
-}
-
-cudaError_t launch_attn_decode(Ctx *ctx, AttnDecodeArgs a, bool pdl) {
-    if (a.head_dim != HD) return cudaErrorNotSupported;
-    if (a.num_heads % a.num_kv_heads) return cudaErrorInvalidValue;
-    const int nrep = a.num_heads / a.num_kv_heads;
-    if (a.chunk <= 0) a.chunk = 128;
-    a.nsplit_max = (a.max_ctx + a.chunk - 1) / a.chunk;
-    const size_t need = (size_t)a.num_heads * a.nsplit_max * (HD + 2) * sizeof(float);
-    if (need > ctx->attn_ws_bytes || a.num_kv_heads > 1024) return cudaErrorInvalidValue;
-    a.ws = ctx->attn_ws;
-    a.counters = ctx->attn_counters;
-    switch (nrep) {
-        case 1: return launch<1>(ctx, a, pdl);
-        case 2: return launch<2>(ctx, a, pdl);
-        case 4: return launch<4>(ctx, a, pdl);
-        case 8: return launch<8>(ctx, a, pdl);
+        case 1: return launch<1>(ctx, a, batch, pdl);
+        case 2: return launch<2>(ctx, a, batch, pdl);
+        case 4: return launch<4>(ctx, a, batch, pdl);
+        case 8: return launch<8>(ctx, a, batch, pdl);
         default: return cudaErrorNotSupported;
     }
 }

@@ -58,10 +58,6 @@ __global__ void __launch_bounds__(256) rope_kv_append_kernel(const AttnPrefillAr
     }
 }
 
-TCE_DEVINL void ldmatrix_x4_trans(uint32_t &r0, uint32_t &r1, uint32_t &r2, uint32_t &r3, const void *smem_row) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(smem_u32(smem_row)));
-}
-
 __global__ void __launch_bounds__(128) attn_prefill_kernel(const AttnPrefillArgs a) {
     __shared__ __align__(16) __half sK[kKT * kPitch];
     __shared__ __align__(16) __half sV[kKT * kPitch];
@@ -186,7 +182,7 @@ __global__ void __launch_bounds__(128) attn_prefill_kernel(const AttnPrefillArgs
             for (int dp = 0; dp < 8; dp++) {
                 uint32_t b0, b1, b2, b3;
                 const __half *vrow = sV + (ks * 16 + (lane & 15)) * kPitch + dp * 16 + (lane >> 4) * 8;
-                ldmatrix_x4_trans(b0, b1, b2, b3, vrow);
+                ldmatrix_x4_t(b0, b1, b2, b3, vrow);
                 mma_m16n8k16(o[dp * 2], pf[ks][0], pf[ks][1], pf[ks][2], pf[ks][3], b0, b1);
                 mma_m16n8k16(o[dp * 2 + 1], pf[ks][0], pf[ks][1], pf[ks][2], pf[ks][3], b2, b3);
             }

@@ -20,6 +20,10 @@ using namespace tce;
 struct tce_ctx {
     Ctx c;
     int attn_chunk = 128;
+    // tce_attn_decode's split records, then its split arrival counters (zeroed; the last split re-arms them): sized by the first call,
+    // grown when a later call needs more
+    float *attn_ws = nullptr;
+    size_t attn_ws_floats = 0, attn_n_counters = 0;
 };
 
 static thread_local std::string g_err;
@@ -85,14 +89,12 @@ int tce_ctx_create(int device, tce_ctx **out) {
     ctx->attn_chunk = env_int("TCE_ATTN_CHUNK", 256);  // cached rows per CTA
     c.gemv_max_ctas = c.num_sms * 4;
     c.gemv_max_tiles = 32768;
-    c.attn_ws_bytes = (size_t)128 * 1024 * 130 * sizeof(float);  // heads * splits * (128 + 2): 128 heads x 1024 splits
     c.gemv_partial_records = c.gemv_max_ctas * 2 > 16384 ? c.gemv_max_ctas * 2 : 16384;  // 8 MB: e.g. 256 row tiles x 32 K-slices
     cudaError_t ie = cudaMalloc(&c.gemv_partials, (size_t)c.gemv_partial_records * 16 * 8 * sizeof(float));
     if (ie == cudaSuccess) ie = cudaMalloc(&c.gemv_counters, (size_t)c.gemv_max_tiles * sizeof(unsigned));
     if (ie == cudaSuccess) ie = cudaMemset(c.gemv_counters, 0, (size_t)c.gemv_max_tiles * sizeof(unsigned));
-    if (ie == cudaSuccess) ie = cudaMalloc(&c.attn_ws, c.attn_ws_bytes);
-    if (ie == cudaSuccess) ie = cudaMalloc(&c.attn_counters, 1024 * sizeof(unsigned));
-    if (ie == cudaSuccess) ie = cudaMemset(c.attn_counters, 0, 1024 * sizeof(unsigned));
+    if (ie == cudaSuccess) ie = cudaMalloc(&c.opt_seed, 2 * sizeof(float));
+    if (ie == cudaSuccess) ie = cudaMemset(c.opt_seed, 0, 2 * sizeof(float));
     if (ie == cudaSuccess) ie = cudaDeviceSynchronize();
     if (ie != cudaSuccess) {  // a half-built context is released, not leaked (cudaFree(nullptr) is a no-op)
         tce_ctx_destroy(ctx);
@@ -107,8 +109,8 @@ int tce_ctx_destroy(tce_ctx *ctx) {
     cudaSetDevice(ctx->c.device);
     cudaFree(ctx->c.gemv_partials);
     cudaFree(ctx->c.gemv_counters);
-    cudaFree(ctx->c.attn_ws);
-    cudaFree(ctx->c.attn_counters);
+    cudaFree(ctx->c.opt_seed);
+    cudaFree(ctx->attn_ws);
     cudaFree(ctx->c.w16_scratch);
     cudaFree(ctx->c.gemv_dbg_keep);
     delete ctx;
@@ -316,12 +318,32 @@ int tce_opt_int8_attention(tce_ctx *ctx, const void *q8, const void *k8, const v
 }
 
 // ---------------------------------------------------------------------------------------------- attention
+// grows tce_attn_decode's workspace to at least `floats` records and `counters` counters (cudaFree synchronises, so never inside a stream capture)
+static cudaError_t attn_ws_reserve(tce_ctx *ctx, size_t floats, size_t counters) {
+    if (floats <= ctx->attn_ws_floats && counters <= ctx->attn_n_counters) return cudaSuccess;
+    floats = floats > ctx->attn_ws_floats ? floats : ctx->attn_ws_floats;
+    counters = counters > ctx->attn_n_counters ? counters : ctx->attn_n_counters;
+    cudaError_t e = cudaFree(ctx->attn_ws);
+    ctx->attn_ws = nullptr;
+    ctx->attn_ws_floats = ctx->attn_n_counters = 0;
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->attn_ws, (floats + counters) * sizeof(float));
+    if (e == cudaSuccess) e = cudaMemsetAsync(ctx->attn_ws + floats, 0, counters * sizeof(unsigned), ctx->c.stream);
+    if (e != cudaSuccess) return e;
+    ctx->attn_ws_floats = floats;
+    ctx->attn_n_counters = counters;
+    return cudaSuccess;
+}
+
 int tce_attn_decode(tce_ctx *ctx, const void *qkv, void *k_cache, void *v_cache, const float *cosb, const float *sinb, const int *pos,
                     void *out, float alpha, int num_heads, int num_kv_heads, int head_dim, int max_ctx) {
     if (!ctx || !qkv || !k_cache || !v_cache || !cosb || !sinb || !pos || !out) return fail(TCE_ERR_INVALID, "tce_attn_decode: null pointer");
     if (head_dim != 128) return fail(TCE_ERR_UNSUPPORTED, "tce_attn_decode: head_dim %d (only 128)", head_dim);
     if (num_heads < 1 || num_kv_heads < 1 || num_heads % num_kv_heads || max_ctx < 1) return fail(TCE_ERR_INVALID, "tce_attn_decode: bad shape");
+    // one call takes at most 128 heads x 1024 splits of records and 1024 KV heads
+    const size_t floats = attn_decode_ws_floats(num_heads, max_ctx, ctx->attn_chunk);
+    if (floats > (size_t)128 * 1024 * (128 + 2) || num_kv_heads > 1024) return tce_fail_cuda(cudaErrorInvalidValue, "tce_attn_decode");
     CK(cudaSetDevice(ctx->c.device), "cudaSetDevice");
+    CK(attn_ws_reserve(ctx, floats, num_kv_heads), "tce_attn_decode workspace");
     AttnDecodeArgs a = {};
     a.qkv = (const __half *)qkv;
     a.k_cache = (__half *)k_cache;
@@ -336,7 +358,11 @@ int tce_attn_decode(tce_ctx *ctx, const void *qkv, void *k_cache, void *v_cache,
     a.head_dim = head_dim;
     a.max_ctx = max_ctx;
     a.chunk = ctx->attn_chunk;
-    CK(launch_attn_decode(&ctx->c, a, false), "tce_attn_decode");
+    a.ws = ctx->attn_ws;
+    a.ws_floats = ctx->attn_ws_floats;
+    a.counters = reinterpret_cast<unsigned *>(ctx->attn_ws + ctx->attn_ws_floats);
+    a.n_counters = ctx->attn_n_counters;
+    CK(launch_attn_decode(&ctx->c, a, 1, false), "tce_attn_decode");
     return TCE_OK;
 }
 

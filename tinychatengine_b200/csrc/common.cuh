@@ -121,6 +121,18 @@ TCE_DEVINL void named_bar_sync(uint32_t id, uint32_t nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// ---------------------------------------------------------------- cp.async, ldmatrix ----------------------
+TCE_DEVINL void cp_async16(void *dst_smem, const void *src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst_smem)), "l"(src) : "memory");
+}
+TCE_DEVINL void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+TCE_DEVINL void ldmatrix_x4(uint32_t &r0, uint32_t &r1, uint32_t &r2, uint32_t &r3, const void *row) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(smem_u32(row)));
+}
+TCE_DEVINL void ldmatrix_x4_t(uint32_t &r0, uint32_t &r1, uint32_t &r2, uint32_t &r3, const void *row) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(smem_u32(row)));
+}
+
 // ---------------------------------------------------------------- legacy tensor path for skinny shapes ----
 // D(16x8,f32) += A(16x16,f16,row) * B(16x8,f16,col)
 TCE_DEVINL void mma_m16n8k16(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {

@@ -25,7 +25,6 @@
 // All waits are bounded: a protocol bug surfaces as a launch failure within seconds, not as a hung GPU.
 #include <stdio.h>
 
-#include "attention_impl.cuh"
 #include "persistent.h"
 #include "w4a16_act_planes.cuh"
 
@@ -845,7 +844,7 @@ TCE_DEVINL void attention_phase(const Args &a, const LayerDesc &L, const PSmem &
 #pragma unroll
                     for (int ks = 0; ks < 8; ks++) {
                         uint32_t b0, b1, b2, b3;
-                        attn::ldmatrix_x4(b0, b1, b2, b3, kst + kv_off(kb * 16 + lr, 2 * ks + lc));
+                        ldmatrix_x4(b0, b1, b2, b3, kst + kv_off(kb * 16 + lr, 2 * ks + lc));
                         mma_m16n8k16(s0, qa[ks][0], 0u, qa[ks][1], 0u, b0, b1);  // keys 0..7 of the block
                         mma_m16n8k16(s1, qa[ks][0], 0u, qa[ks][1], 0u, b2, b3);  // keys 8..15
                     }
@@ -879,7 +878,7 @@ TCE_DEVINL void attention_phase(const Args &a, const LayerDesc &L, const PSmem &
 #pragma unroll
                     for (int jp = 0; jp < 4; jp++) {
                         uint32_t b0, b1, b2, b3;
-                        attn::ldmatrix_x4_t(b0, b1, b2, b3, vst + kv_off(kb * 16 + lr, 8 * h + 2 * jp + lc));
+                        ldmatrix_x4_t(b0, b1, b2, b3, vst + kv_off(kb * 16 + lr, 8 * h + 2 * jp + lc));
                         mma_m16n8k16(oacc[2 * jp], pa0, 0u, pa2, 0u, b0, b1);
                         mma_m16n8k16(oacc[2 * jp + 1], pa0, 0u, pa2, 0u, b2, b3);
                     }

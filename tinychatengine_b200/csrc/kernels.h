@@ -24,11 +24,9 @@ struct Ctx {
     int gemv_max_tiles = 0;
     unsigned long long *gemv_dbg = nullptr;  // optional phase timestamps (option "gemv_debug")
     unsigned long long *gemv_dbg_keep = nullptr;  // its allocation (kept until the context is destroyed)
-    // flash-decode workspace (partial m, l, o per (head, split))
-    float *attn_ws = nullptr;
-    size_t attn_ws_bytes = 0;
-    unsigned *attn_counters = nullptr;
     unsigned option_gen = 0;       // bumped by every tce_ctx_set_option / set_stream: captured CUDA graphs hold the context by value and are rebuilt
+    // the int8 OPT attention's in-kernel seed hand-off: [0] the seed value of the current call, [1] its epoch flag (zeroed at creation)
+    float *opt_seed = nullptr;
     unsigned attn_seed_epoch = 0;  // calls of the int8 OPT attention so far (tags the in-kernel seed hand-off)
     // tunables (env overridable, see ctx.cu)
     int gemv_impl = 1;      // 0 = simple warp-per-row, 1 = TMA + mma.sync stream-K

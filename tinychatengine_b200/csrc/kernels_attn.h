@@ -6,38 +6,36 @@ struct tce_sampling;  // include/tce_b200.h
 
 namespace tce {
 
+// Decode attention (attention.cu) of `batch` sequences: sequence b is grid.z = b, with its own q|k|v and output rows, KV cache and position,
+// and its own split records and counters in the workspace.
 struct AttnDecodeArgs {
-    const __half *qkv;   // [(H + 2*KVH) * head_dim] projections of the current token (q | k | v), pre-RoPE
-    __half *k_cache;     // [KVH][max_ctx][head_dim]
-    __half *v_cache;     // [KVH][max_ctx][head_dim]
+    const __half *qkv;   // [batch][qkv_stride]: the (H + 2*KVH) * head_dim projections of the current token (q | k | v), pre-RoPE
+    __half *out;         // [batch][out_stride]: H * head_dim
+    int qkv_stride, out_stride;  // elements between the rows of consecutive sequences
     const float *cos;    // [max_ctx][head_dim]  (reference rotary_emb/cos_cached layout)
     const float *sin;    // [max_ctx][head_dim]
-    const int *pos;      // device scalar: index of the token being decoded (= number of cached tokens)
-    __half *out;         // [H * head_dim]
     float alpha;         // qk_bmm alpha (1/sqrt(head_dim))
     int num_heads, num_kv_heads, head_dim, max_ctx;
-    int chunk;           // cached positions per CTA
+    int chunk;           // cached positions per CTA (<= 0: the default)
     int nsplit_max;      // filled by the launcher
-    float *ws;           // filled by the launcher
-    unsigned *counters;  // filled by the launcher
-};
-cudaError_t launch_attn_decode(Ctx *ctx, AttnDecodeArgs a, bool pdl);
-
-// batched decode: sequence b of the batch is grid.z = b, with its own q|k|v / output rows, KV-cache slot and position
-struct AttnBatchArgs {
-    AttnDecodeArgs base;     // qkv / out of sequence 0, RoPE tables, shapes, and the split workspace base.ws / base.counters (k_cache, v_cache and
-                             // pos unused)
-    size_t ws_floats;        // capacity of base.ws: batch * num_heads * nsplit * (head_dim + 2) floats are used
-    size_t n_counters;       // capacity of base.counters (zero-initialised): batch * num_kv_heads are used
-    const int *req;          // device int[batch][4] {token, position, slot, valid} (launch_embedding_batch); valid = 0: the CTA writes nothing
+    float *ws;           // split records: batch * attn_decode_ws_floats(...) are used
+    size_t ws_floats;    // capacity of ws
+    unsigned *counters;  // zero-initialised split arrival counters (the last split re-arms them): batch * num_kv_heads are used
+    size_t n_counters;   // capacity of counters
+    // with a request table (the batched step): each sequence's position and slot
+    const int *req;          // device int[batch][4] {token, position, slot, valid} (launch_embedding_batch), 16-byte aligned; valid = 0: the CTA writes nothing
     __half *const *slots;    // device table of slot bases, each [L][2][KVH][max_ctx][head_dim]
     long long k_off, v_off;  // elements from a slot's base to this layer's K / V slab
-    int qkv_stride, out_stride;  // elements between the rows of consecutive sequences
+    // without one (req == nullptr, batch 1): the cache and position of the one sequence
+    __half *k_cache;     // [KVH][max_ctx][head_dim]
+    __half *v_cache;     // [KVH][max_ctx][head_dim]
+    const int *pos;      // device scalar: index of the token being decoded (= number of cached tokens)
 };
-// returns cudaErrorNotSupported for a head_dim or a query-heads-per-KV-head ratio the kernel does not cover
-cudaError_t launch_attn_decode_batch(Ctx *ctx, AttnBatchArgs b, int batch, bool pdl);
-// floats of split workspace the batched kernel needs per sequence
-size_t attn_batch_ws_floats(int num_heads, int max_ctx, int chunk);
+// returns cudaErrorNotSupported for a head_dim or a query-heads-per-KV-head ratio the kernel does not cover, cudaErrorInvalidValue for a
+// workspace too small for the batch
+cudaError_t launch_attn_decode(Ctx *ctx, const AttnDecodeArgs &a, int batch, bool pdl);
+// floats of split workspace the kernel needs per sequence
+size_t attn_decode_ws_floats(int num_heads, int max_ctx, int chunk);
 
 // prompt processing (sqlen = n > 1): RoPE + KV append for rows pos0..pos0+n-1, causal attention over the cache.  Up to
 // kMaxPrefillSeqs prompts in one launch: their rows are concatenated, and each has its own positions and KV cache.

@@ -695,12 +695,11 @@ cudaError_t LlamaDecoder::batch_alloc(std::string *err) {
     if (bs_) return cudaSuccess;
     const int nrep = cfg_.num_heads / cfg_.num_kv_heads;
     if (nrep != 1 && nrep != 2 && nrep != 4 && nrep != 8) return no("the batched attention kernel takes 1, 2, 4 or 8 query heads per KV head");
-    const int chunk = attn_chunk_ > 0 ? attn_chunk_ : 128;
     const size_t B = TCE_LLAMA_MAX_BATCH, E = cfg_.embed_dim, F = cfg_.hidden_dim, V = cfg_.vocab_size,
                  Q = (size_t)(cfg_.num_heads + 2 * cfg_.num_kv_heads) * cfg_.head_dim, A = (size_t)cfg_.num_heads * cfg_.head_dim;
     // all or nothing: the set is built aside and published whole; a failed allocation frees what this call took
     std::unique_ptr<BatchState> st = std::make_unique<BatchState>();
-    st->attn_ws_floats = B * attn_batch_ws_floats(cfg_.num_heads, cfg_.max_ctx, chunk);
+    st->attn_ws_floats = B * attn_decode_ws_floats(cfg_.num_heads, cfg_.max_ctx, attn_chunk_);
     st->n_counters = B * cfg_.num_kv_heads;
     __half *kv0 = d_kv_.get();
     cudaError_t e = cudaSuccess;
@@ -759,8 +758,7 @@ cudaError_t LlamaDecoder::batch_alloc(std::string *err) {
         gemv({&L.gate, &L.up}, st->resid.get(), (int)E, L.post_norm, st->act.get(), (int)F, EPI_SILU_MUL_HALF);
         gemv({&L.down}, st->act.get(), (int)F, nullptr, st->resid.get(), (int)E, EPI_ADD_F32);
         // RoPE + in-place KV append + attention over the cache of each sequence's slot
-        AttnBatchArgs b{};
-        AttnDecodeArgs &a = b.base;
+        AttnDecodeArgs a{};
         a.qkv = st->qkv.get();
         a.cos = d_cos_;
         a.sin = d_sin_;
@@ -773,14 +771,14 @@ cudaError_t LlamaDecoder::batch_alloc(std::string *err) {
         a.chunk = attn_chunk_;
         a.ws = st->attn_ws.get();
         a.counters = st->attn_counters.get();
-        b.ws_floats = st->attn_ws_floats;
-        b.n_counters = st->n_counters;
-        b.req = st->safe.get();
-        b.k_off = (__half *)kv_cache(l, 0) - kv0;  // this layer's slabs within a slot
-        b.v_off = (__half *)kv_cache(l, 1) - kv0;
-        b.qkv_stride = (int)Q;
-        b.out_stride = (int)A;
-        st->attn_ops.push_back(b);
+        a.ws_floats = st->attn_ws_floats;
+        a.n_counters = st->n_counters;
+        a.req = st->safe.get();
+        a.k_off = (__half *)kv_cache(l, 0) - kv0;  // this layer's slabs within a slot
+        a.v_off = (__half *)kv_cache(l, 1) - kv0;
+        a.qkv_stride = (int)Q;
+        a.out_stride = (int)A;
+        st->attn_ops.push_back(a);
     }
     st->gemv_ops.push_back(lm_head_gemv(st->resid.get(), st->logits.get()));
     bs_ = std::move(st);
@@ -863,9 +861,9 @@ cudaError_t LlamaDecoder::enqueue_batch(int batch, const int *req, float *logits
                                st.safe.get(), false));
     for (int l = 0; l < cfg_.num_layers; l++) {
         DCK(gemv(st.gemv_ops[4 * l]));
-        AttnBatchArgs a = st.attn_ops[l];
+        AttnDecodeArgs a = st.attn_ops[l];
         a.slots = st.slot_table.get();
-        DCK(launch_attn_decode_batch(c, a, batch, pdl));
+        DCK(launch_attn_decode(c, a, batch, pdl));
         for (int i = 1; i < 4; i++) DCK(gemv(st.gemv_ops[4 * l + i]));
     }
     W4GemvParams lm = st.gemv_ops.back();

@@ -220,7 +220,7 @@ class LlamaDecoder {
         // the step's parameters on these buffers: GEMV 4 * layer + {0: q|k|v, 1: o, 2: gate|up, 3: down} (M = 1), then the lm_head;
         // the attention of each layer (its slot table is read at launch)
         std::vector<W4GemvParams> gemv_ops;
-        std::vector<AttnBatchArgs> attn_ops;
+        std::vector<AttnDecodeArgs> attn_ops;
     };
     std::unique_ptr<BatchState> bs_;  // non-null: every buffer of the batched step exists
     // one graph per batch size: host entry (with / without the logits copy), device entry (for one request pointer), generate loop (one

@@ -214,12 +214,8 @@ cudaError_t launch_opt_int8_attention(Ctx *ctx, const OptAttnParams &p) {
         if (e != cudaSuccess) return e;
     }
     // [0] the seed value p[0][0][0] of this call, [1] the epoch flag that says it is there (same-stream ordering makes the reuse safe)
-    float *seed_ws = ctx->attn_ws;
-    unsigned *seed_flag = reinterpret_cast<unsigned *>(ctx->attn_ws) + 1;
-    if (ctx->attn_seed_epoch == 0) {
-        e = cudaMemsetAsync(ctx->attn_ws, 0, 8, ctx->stream);
-        if (e != cudaSuccess) return e;
-    }
+    float *seed_ws = ctx->opt_seed;
+    unsigned *seed_flag = reinterpret_cast<unsigned *>(ctx->opt_seed) + 1;
     const unsigned epoch = ++ctx->attn_seed_epoch;
     const int vec16 = (p.hd % 16 == 0) && (p.final_hs % 16 == 0) && !(((uintptr_t)p.final_k | (uintptr_t)p.final_v) & 15) ? 1 : 0;
     dim3 g2(p.H, p.sqlen);  // block (0, 0) = row (head 0, query 0) is in the first wave: the rows that wait for its seed cannot starve it
