@@ -179,6 +179,7 @@ struct PSmem {
     uint64_t *full, *empty, *red_full, *red_empty;
     uint64_t *rx;       // pair staging: counts the bytes the partner has mirrored into this CTA for the current staging
     int *free_gen;      // pair staging: written by the partner: the number of phases it has finished (its buffers may be overwritten)
+    int2 *red_pos;      // [kCW] each consumer warp's position in the red-buffer ring between GEMV phases (see consume_gemv)
     uint32_t ring_u32, xs_u32, gx_u32, gsum_u32, full_u32, empty_u32, redfull_u32, redempty_u32;
     int nst;
 };
@@ -209,6 +210,7 @@ TCE_DEVINL PSmem carve(uint8_t *raw, const Args &a) {
     s.red_empty = s.red_full + kRedBufs;
     s.rx = s.red_empty + kRedBufs;
     s.free_gen = reinterpret_cast<int *>(s.rx + 1);
+    s.red_pos = reinterpret_cast<int2 *>(s.rx + 2);
     s.ring_u32 = smem_u32(s.ring);
     s.xs_u32 = smem_u32(s.xs);
     s.gx_u32 = smem_u32(s.gx);
@@ -402,8 +404,7 @@ TCE_DEVINL int rot_unit(int u, int units, int cta) {
 }
 
 // fp16 input vector (attention output / SiLU*mul activations) published as {half2, tag} words -> activation planes
-TCE_DEVINL void stage_half(const Args &a, const GemvOp &op, const PSmem &sm, PairCtx &pc, const uint2 *src, uint32_t tag, int cta, int ctid, int lane, int p,
-                           int nphase) {
+TCE_DEVINL void stage_half(const GemvOp &op, const PSmem &sm, PairCtx &pc, const uint2 *src, uint32_t tag, int cta, int ctid, int lane, int p) {
     const int ng_own = own_groups(pc, op.NG);
     const int units = ng_own * 16;  // 8 halfs = 4 words = 32 B per unit; this CTA's groups only (pair mode: every other group)
     if (pc.on) {
@@ -447,7 +448,6 @@ TCE_DEVINL void stage_half(const Args &a, const GemvOp &op, const PSmem &sm, Pai
             }
             __syncwarp();
         }
-        if (ub == 0 && ctid == 0) stamp(a, cta, nphase, p, 4);
 #pragma unroll
         for (int k = 0; k < PRE; k++) {
             if (ub + k * kConsumerThreads >= units) break;  // warp-uniform
@@ -462,7 +462,6 @@ TCE_DEVINL void stage_half(const Args &a, const GemvOp &op, const PSmem &sm, Pai
                 gemv::emit_unit<1>(sm.xs, op.IC, sm.gx, sm.gsum, valid ? ui[k] : 0, valid, v, lane);
         }
     }
-    if (ctid == 0) stamp(a, cta, nphase, p, 5);
     named_bar_sync(1, kConsumerThreads);
     if (pc.on) rx_wait(sm, pc);
 }
@@ -505,7 +504,7 @@ TCE_DEVINL void tp_accumulate(float (&x)[8], const uint2 *slot0, int tp_size, in
 // fp32 residual stream with fused RMSNorm.  Every CTA holds the stream in shared memory; `delta` (o_proj or down_proj outputs of all
 // tensor-parallel ranks, {float, tag} words) is added to it here by every CTA in the same (rank) order.  Returns 1/rms: y = inv * W (x . gamma).
 TCE_DEVINL float stage_rms(const Args &a, const GemvOp &op, const PSmem &sm, PairCtx &pc, const uint2 *delta, uint32_t tag, const float *gamma, int token,
-                           bool first, bool emit, int cta, int ctid, int cw, int lane, int p, int nphase) {
+                           bool first, bool emit, int cta, int ctid, int cw, int lane, int p) {
     const int units = own_groups(pc, op.NG) * 16;  // pair mode: this CTA keeps (and normalises) every other 128-group of the residual stream
     const bool sys = a.tp_size > 1;
     if (pc.on && emit) {
@@ -553,7 +552,6 @@ TCE_DEVINL float stage_rms(const Args &a, const GemvOp &op, const PSmem &sm, Pai
                 } else {
                     tp_accumulate(x, delta + (size_t)ui * 8, a.tp_size, a.E, tag);
                 }
-                if (ui0 == 0 && ctid == 0) stamp(a, cta, nphase, p, 4);
             }
             *reinterpret_cast<float4 *>(sm.resid + (size_t)ui * 8) = make_float4(x[0], x[1], x[2], x[3]);
             *reinterpret_cast<float4 *>(sm.resid + (size_t)ui * 8 + 4) = make_float4(x[4], x[5], x[6], x[7]);
@@ -576,7 +574,6 @@ TCE_DEVINL float stage_rms(const Args &a, const GemvOp &op, const PSmem &sm, Pai
         sm.rms[pc.rank * kCW + cw] = ss;
         if (pc.on) gemv::st_async_b32(pc.r_rms + (uint32_t)(pc.rank * kCW + cw) * 4u, __float_as_uint(ss), pc.dst.bar);
     }
-    if (ctid == 0) stamp(a, cta, nphase, p, 5);
     named_bar_sync(1, kConsumerThreads);
     if (pc.on) rx_wait(sm, pc);
     float tot = 0.f;
@@ -615,7 +612,20 @@ TCE_DEVINL void unit_compute(const UnitRegs &u, float lscale, float &totA, float
 // Warp cw consumes groups cw and cw + 16 of every stage.  Group gi of a stage sits at a fixed place whatever the shape (see GemvOp), so
 // every operand address is a per-lane constant plus the slot base, and the second unit of a warp sits at fixed distances (+16 KiB weights,
 // +4 KiB planes, +512 B scales ...): the inner loop carries almost no address arithmetic (the ALU pipe is what bounds this loop).
-TCE_DEVINL void consume_gemv(const GemvOp &op, const PSmem &sm, Ring &rs, Red &cs, float inv, int cta, int ncta, int cw, int lane) {
+// Stamps of consumer warp 0 (TCE_PK_DEBUG): 4 first stage landed, 5 last stage released, 6 last tile handed to the epilogue.
+// The warp's red-buffer position, its lane id and 1/rms are taken afresh here (shared memory, %laneid, a shuffle of the same value), not
+// carried in registers across the phase loop: held there, they were spilled to local memory (the attention and staging code set the
+// register budget) and reloaded on the path of every tile.
+TCE_DEVINL void consume_gemv(const Args &a, const GemvOp &op, const PSmem &sm, Ring &rs, float inv_in, int cta, int ncta, int cw, int p, int nphase) {
+    int lane;
+    asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
+    const float inv = __shfl_sync(0xffffffffu, inv_in, 0);  // every lane holds the same value
+    Red cs;
+    {
+        const int2 rp = sm.red_pos[cw];
+        cs.rb = rp.x;
+        cs.rphase = (uint32_t)rp.y;
+    }
     const int g = lane >> 2, t = lane & 3;
     int t0, t1;
     partition(op, cta, ncta, t0, t1);
@@ -630,6 +640,10 @@ TCE_DEVINL void consume_gemv(const GemvOp &op, const PSmem &sm, Ring &rs, Red &c
     const uint32_t q_lane = sm.gx_u32 + (uint32_t)cw * 4u;
     const float lscale = (t == 0) ? 65536.f : (t == 1 ? 1.f : 0.f);
     const bool xl = g < 4;  // MMA columns 4..7 are don't-cares
+    if (a.dbg && t1 > t0 && cw == 0 && lane == 0) {  // outside the stage loop: a second wait on the same phase returns at once
+        mbar_wait_u32(sm.full_u32 + (uint32_t)rs.stage * 8u, rs.phase);
+        stamp(a, cta, nphase, p, 4);
+    }
     for (int tile = t0; tile < t1; tile++) {
         float totA = 0.f, totB = 0.f;
         for (int s = 0; s < S; s++) {
@@ -671,6 +685,7 @@ TCE_DEVINL void consume_gemv(const GemvOp &op, const PSmem &sm, Ring &rs, Red &c
             if (lane == 0) mbar_arrive_u32(sm.empty_u32 + (uint32_t)rs.stage * 8u);
             rs.advance(sm.nst);
         }
+        if (tile == t1 - 1 && cw == 0 && lane == 0) stamp(a, cta, nphase, p, 5);
         // ---- hand the tile sums to the epilogue warp ----
         totA += __shfl_xor_sync(0xffffffffu, totA, 1);  // (p3, p2) share of t = 0 + (p1, p0) share of t = 1
         totB += __shfl_xor_sync(0xffffffffu, totB, 1);
@@ -684,6 +699,10 @@ TCE_DEVINL void consume_gemv(const GemvOp &op, const PSmem &sm, Ring &rs, Red &c
         if (lane == 0) mbar_arrive_u32(sm.redfull_u32 + (uint32_t)cs.rb * 8u);
         cs.advance();
     }
+    __syncwarp();  // every lane has read the old position
+    if (lane == 0) sm.red_pos[cw] = make_int2(cs.rb, (int)cs.rphase);
+    __syncwarp();
+    if (cw == 0 && lane == 0) stamp(a, cta, nphase, p, 6);
 }
 
 // ------------------------------------------------------------------------------------------------------------ epilogue warp
@@ -691,13 +710,19 @@ struct EpiState {
     unsigned long long best;  // PE_LOGITS: running arg-max key of this warp
 };
 
+// Stamp (TCE_PK_DEBUG): 7 the last tile's partials are in; the caller stamps 3 after its last publish.
+// The lane id is read here (%laneid), as in consume_gemv: passed in, the lane-derived offsets and predicates were hoisted out of the phase
+// loop, spilled, and reloaded on every tile.
 TCE_DEVINL void epilogue_gemv(const Args &a, const GemvOp &op, const PSmem &sm, Red &es, EpiState &st, uint2 *out_ll, int which, uint32_t tag, int cta, int ncta,
-                              int lane) {
+                              int p, int nphase) {
+    int lane;
+    asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
     int t0, t1;
     partition(op, cta, ncta, t0, t1);
     const bool tp = a.tp_size > 1;
     for (int tile = t0; tile < t1; tile++) {
         mbar_wait_u32(sm.redfull_u32 + (uint32_t)es.rb * 8u, es.rphase);
+        if (tile == t1 - 1 && lane == 0) stamp(a, cta, nphase, p, 7);
         const float *rbuf = sm.red + (size_t)es.rb * kCW * 16;
         // lane l < 16 sums consumer warps 0..7 of row l, lane l + 16 warps 8..15
         float v = 0.f;
@@ -800,12 +825,9 @@ TCE_DEVINL void attention_phase(const Args &a, const LayerDesc &L, const PSmem &
         }
         named_bar_sync(1, kConsumerThreads);
         if (ctid == 0) stamp(a, cta, nphase, p, 4);
-        uint32_t qa[8][2];  // A operand: q[head g][dims], all 8 k-steps (rows 8..15 of the MMA tile are zero)
-#pragma unroll
-        for (int ks = 0; ks < 8; ks++) {
-            qa[ks][0] = *reinterpret_cast<const uint32_t *>(sQ + g * 136 + ks * 16 + t * 2);
-            qa[ks][1] = *reinterpret_cast<const uint32_t *>(sQ + g * 136 + ks * 16 + 8 + t * 2);
-        }
+        // A operand: q[head g][dims] (rows 8..15 of the MMA tile are zero), read from sQ at every k-step: held in registers for the whole
+        // chunk loop, the 16 words pushed the consumers' long-lived state (ring and hand-off positions) into local memory
+        const uint32_t qa_u32 = smem_u32(sQ + g * 136 + t * 2);
         float m_run = -INFINITY, l_run = 0.f;  // of head row g (replicated over t)
         bool have = false;
         float *myO = sO + (size_t)cw * nrep * 128;
@@ -845,8 +867,9 @@ TCE_DEVINL void attention_phase(const Args &a, const LayerDesc &L, const PSmem &
                     for (int ks = 0; ks < 8; ks++) {
                         uint32_t b0, b1, b2, b3;
                         ldmatrix_x4(b0, b1, b2, b3, kst + kv_off(kb * 16 + lr, 2 * ks + lc));
-                        mma_m16n8k16(s0, qa[ks][0], 0u, qa[ks][1], 0u, b0, b1);  // keys 0..7 of the block
-                        mma_m16n8k16(s1, qa[ks][0], 0u, qa[ks][1], 0u, b2, b3);  // keys 8..15
+                        const uint32_t qa0 = lds_u32(qa_u32 + ks * 32u), qa1 = lds_u32(qa_u32 + ks * 32u + 16u);
+                        mma_m16n8k16(s0, qa0, 0u, qa1, 0u, b0, b1);  // keys 0..7 of the block
+                        mma_m16n8k16(s1, qa0, 0u, qa1, 0u, b2, b3);  // keys 8..15
                     }
                 }
                 // thread (g, t): head row g, keys kbase + {2t, 2t+1} (s0) and kbase + 8 + {2t, 2t+1} (s1)
@@ -1037,10 +1060,12 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
     const unsigned epoch = *a.epoch;
     const uint32_t tag_base = epoch * (uint32_t)(2 * nphase + 2) + 1u;  // tag of (phase p, sub-result s) = tag_base + 2p + s: unique over launches, never 0
 
-    // register budget: 20 warps x 96 registers at launch; warpgroup 0 (producer, epilogue, two spare warps) gives most of its share back
-    // and the 16 consumer warps grow to 112 (per scheduler: 32 + 4 x 112 <= 5 x 96 registers per lane)
+    // register budget: 20 warps x 96 registers at launch, and setmaxnreg only moves registers within that pool (per scheduler:
+    // 64 + 4 x 104 = 5 x 96 registers per lane; a split that asks for more never gets them and the kernel stalls).  Warpgroup 0 (loader,
+    // epilogue, two spare warps) keeps 64: at 32 the loader and the epilogue spilled their loop state to local memory, reloaded on the
+    // path of every ring stage and every tile.  The consumer code compiles to the same spills with 112 or 120 as with 104.
     if (warp < kAuxWarps) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 32;" ::: "memory");
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 64;" ::: "memory");
         if (warp >= 2) return;  // warps 2 and 3 only donate their registers
         if (warp == 0) {
             // ================= loader: every byte this CTA needs from HBM, in consumption order =================
@@ -1057,7 +1082,7 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
             if (l < Lyr && k == 1) continue;  // attention publishes its own results
             const int oi = (l == Lyr) ? OPI_LMHEAD : ((k == 0) ? OPI_QKV : (k - 1));
             uint2 *out = (oi == OPI_QKV) ? a.qkv_ll : (oi == OPI_GATEUP ? a.act_ll : (oi == OPI_O ? a.delta_ll[0] : a.delta_ll[1]));
-            epilogue_gemv(a, a.op[oi], sm, es, st, out, (oi == OPI_DOWN) ? 1 : 0, tag_base + 2u * (uint32_t)p, cta, ncta, lane);
+            epilogue_gemv(a, a.op[oi], sm, es, st, out, (oi == OPI_DOWN) ? 1 : 0, tag_base + 2u * (uint32_t)p, cta, ncta, p, nphase);
             if (lane == 0) stamp(a, cta, nphase, p, 3);
         }
         unsigned long long key = st.best;
@@ -1073,13 +1098,14 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
         if (lane == 0) red_release_gpu(a.done);
         return;
     }
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 112;" ::: "memory");
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 104;" ::: "memory");
 
     // ================= consumers =================
     const int ctid = tid - 32 * kAuxWarps;
     const int cw = warp - kAuxWarps;
     Ring rs;
-    Red cs;
+    if (lane == 0) sm.red_pos[cw] = make_int2(0, 0);
+    __syncwarp();
     if (ctid < 256) sm.rope[ctid] = (ctid < 128) ? a.cos[(size_t)pos * 128 + ctid] : a.sin[(size_t)pos * 128 + ctid - 128];  // visible after the first phase's barrier
 #pragma unroll 1
     for (int p = 0; p < nphase; p++) {
@@ -1107,17 +1133,17 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
         }
         float inv = 1.f;
         if (oi == OPI_O) {
-            if (stage) stage_half(a, op, sm, pc, a.attn_ll, tag_in, cta, ctid, lane, p, nphase);
+            if (stage) stage_half(op, sm, pc, a.attn_ll, tag_in, cta, ctid, lane, p);
         } else if (oi == OPI_DOWN) {
-            if (stage) stage_half(a, op, sm, pc, a.act_ll, tag_in, cta, ctid, lane, p, nphase);
+            if (stage) stage_half(op, sm, pc, a.act_ll, tag_in, cta, ctid, lane, p);
         } else {
             // the residual copy of this CTA must see every o_proj / down_proj output, whether or not the CTA owns tiles of this phase
             const float *gamma = (oi == OPI_LMHEAD) ? a.final_norm : (oi == OPI_QKV ? a.layers[l].input_norm : a.layers[l].post_norm);
             const uint2 *delta = (oi == OPI_GATEUP) ? a.delta_ll[0] : a.delta_ll[1];
-            inv = stage_rms(a, op, sm, pc, delta, tag_in, gamma, token, p == 0, stage, cta, ctid, cw, lane, p, nphase);
+            inv = stage_rms(a, op, sm, pc, delta, tag_in, gamma, token, p == 0, stage, cta, ctid, cw, lane, p);
         }
         if (ctid == 0) stamp(a, cta, nphase, p, 1);
-        if (work) consume_gemv(op, sm, rs, cs, inv, cta, ncta, cw, lane);
+        if (work) consume_gemv(a, op, sm, rs, inv, cta, ncta, cw, p, nphase);
         if (ctid == 0) stamp(a, cta, nphase, p, 2);
         named_bar_sync(1, kConsumerThreads);  // every warp is done with the planes before the next phase overwrites them
         if (pc.on && ctid == 0 && p + 1 < nphase) st_cluster_u32(pc.r_free, (uint32_t)(p + 1));  // (not after the last phase: the partner may be gone)
@@ -1202,7 +1228,8 @@ int attn_nsplit_max(int ncta, int KVH, int max_ctx) {
 }
 
 static size_t fixed_bytes(int xs_bytes, int max_ng, int E) {
-    return (size_t)xs_bytes + (size_t)E * 4 + (size_t)max_ng * 12 + (size_t)kRedBufs * kCW * 16 * 4 + 32 * 4 + 256 * 4 + (size_t)(2 * kMaxStages + 2 * kRedBufs) * 8 + 16 + 1024;
+    return (size_t)xs_bytes + (size_t)E * 4 + (size_t)max_ng * 12 + (size_t)kRedBufs * kCW * 16 * 4 + 32 * 4 + 256 * 4 + (size_t)(2 * kMaxStages + 2 * kRedBufs) * 8 + 16 +
+           (size_t)kCW * 8 + 1024;
 }
 int pick_stages(int smem_optin, int xs_bytes, int max_ng, int E) {
     const long long avail = (long long)smem_optin - (long long)fixed_bytes(xs_bytes, max_ng, E);

@@ -101,6 +101,35 @@ def main():
         summ[names[k]] = m
         print(f"{names[k]:8s} phase {m['phase_us']:6.2f} us (HBM floor {m['hbm_floor_us']:5.2f})  barrier {m['barrier_us']:5.2f}  stage {m['stage_us']:5.2f}  "
               f"consume {m['consume_us']:6.2f}  tail {m['tail_us']:5.2f}  skew {m['skew_us']:5.2f}  hop {m['hop_us']:5.2f}  etail {m['etail_us']:5.2f}  -> {m['GBps']:7.0f} GB/s")
+    # GEMV sub-steps of consumer warp 0 (slots 4..6) and of the epilogue warp (7, then 3), since the CTA's input was staged (slot 1).
+    # Means over the CTAs that own tiles and over the layers: the timer ticks far coarser than one ring stage, a mean over thousands of
+    # intervals that start at unrelated moments still resolves it.  per_stage: (last stage released - first stage landed) / stages: slot 4
+    # is stamped when the first stage has landed, before it is computed, and slot 5 after the last one is released, so the interval holds
+    # the compute of every stage and, where a tile is one stage (q|k|v, o_proj, gate|up), the hand-offs of all tiles but the last.  With
+    # the stages already in shared memory (q|k|v and o_proj: at most 3 per CTA, loaded while the previous phases ran) it is the
+    # consumer-only cost of a ring stage.
+    tick = np.gcd.reduce(np.unique(raw[raw > 0] - raw[raw > 0].min()).astype(np.int64))
+    ops = {0: (E, (H + 2 * KVH) * hd // 16), 2: (H * hd, E // 16), 3: (E, 2 * F // 16), 4: (F, E // 16)}  # IC, 16-row tiles
+    sub = {}
+    for k, (ic, ntiles) in ops.items():
+        S = (ic // 128 + 31) // 32
+        nst = np.array([(ntiles * (c + 1)) // ncta - (ntiles * c) // ncta for c in range(ncta)]) * S
+        rows = {"first_landed": [], "last_released": [], "handed": [], "epi_last_in": [], "published": [], "per_stage": []}
+        for p in range(k, nphase - 1, 5):
+            base = T[:, p, 1]
+            for nm, slot in (("first_landed", 4), ("last_released", 5), ("handed", 6), ("epi_last_in", 7), ("published", 3)):
+                rows[nm].append(T[:, p, slot] - base)
+            ok = nst > 0
+            rows["per_stage"].append((T[ok, p, 5] - T[ok, p, 4]) / nst[ok])
+        m = {nm: float(np.nanmean(np.concatenate(v))) for nm, v in rows.items()}
+        m["stages_per_cta"] = f"{nst.min()}-{nst.max()}"
+        sub[names[k]] = m
+    print(f"GEMV sub-steps since staged (means, us; timer tick {tick} ns):")
+    for nm, m in sub.items():
+        print(f"  {nm:8s} stages/CTA {m['stages_per_cta']:6s} first landed {m['first_landed']:5.2f}  last released {m['last_released']:5.2f}  "
+              f"handed {m['handed']:5.2f}  epilogue has last {m['epi_last_in']:5.2f}  published {m['published']:5.2f}  -> {1e3 * m['per_stage']:6.0f} ns/stage")
+    summ["gemv_substeps"] = sub
+    summ["timer_tick_ns"] = int(tick)
     lm = nphase - 1
     prev_done = np.nanmax(T[:, lm - 1, 3])
     print(f"lm_head  phase {np.nanmax(T[:, lm, 3]) - prev_done:6.2f} us")
