@@ -116,6 +116,14 @@ TCE_API int tce_attn_decode(tce_ctx *ctx, const void *qkv, void *k_cache, void *
 TCE_API int tce_attn_prefill(tce_ctx *ctx, void *qkv, void *k_cache, void *v_cache, const float *cos, const float *sin, void *out, float alpha,
                              int n, int pos0, int num_heads, int num_kv_heads, int head_dim, int max_ctx);
 
+/* Same module for n <= 8 consecutive tokens of ONE sequence (the span step's attention): qkv half[n][(H + 2*KVH)*head_dim] holds the
+ * projections of the tokens at positions pos0..pos0+n-1 (pre-RoPE, not modified); rotated k and v are appended to the caches at those rows,
+ * out half[n][H*head_dim] receives causal attention over cache rows 0..pos0+i for token i.  A CTA reads each cached row of its context split
+ * once for all n * H/KVH query rows.  The split is the context's "attn_chunk", lowered to the largest multiple of 16 whose CTA fits shared
+ * memory.  Workspace as tce_attn_decode.  head_dim == 128; 1 <= n <= 8, 0 <= pos0 <= max_ctx - n.                                      */
+TCE_API int tce_attn_span(tce_ctx *ctx, const void *qkv, void *k_cache, void *v_cache, const float *cos, const float *sin, void *out, float alpha,
+                          int n, int pos0, int num_heads, int num_kv_heads, int head_dim, int max_ctx);
+
 /* ---- small ops either side of the path -------------------------------------------------------------------
  * LlamaRMSNorm_cuda::forward (llm/src/ops/cuda/LlamaRMSNorm.cu:96-115): half in/out, fp32 gamma             */
 TCE_API int tce_rmsnorm_f16(tce_ctx *ctx, const void *x, const float *gamma, void *y, int rows, int dim, float eps);
@@ -269,6 +277,42 @@ typedef struct tce_gen_request {
  * batch, slot (unreserved or repeated), first_token, pos0, n_predict < 0, n_history outside [0, max_ctx], out_stride below a clamped
  * n_predict or a NULL pointer; TCE_ERR_UNSUPPORTED for temp > 0 without 1 <= top_k <= 1024.                                           */
 TCE_API int tce_llama_generate_batch(tce_llama *m, int batch, const tce_gen_request *reqs, int *out_tokens_host, int out_stride, int *n_out);
+/* ---- span step and greedy speculative decoding -------------------------------------------------------------------------------------------
+ * Span step: tokens_host[0..n) at positions pos0 .. pos0 + n - 1 of ONE slot in one pass over the weights (the batched step's GEMVs at
+ * M = n, then a causal multi-query attention that reads the slot's context once for all n rows).  logits_host float[n][vocab] (row i: the
+ * logits after tokens_host[i]) and next_tokens int[n] (greedy) may be NULL.  Writes KV rows pos0 .. pos0 + n - 1 of the slot and no other
+ * row of any slot.  TCE_ERR_INVALID, before anything is enqueued, for n outside [1, TCE_LLAMA_MAX_BATCH], pos0 < 0, pos0 + n > max_ctx, an
+ * unreserved slot or a token outside [0, vocab); TCE_ERR_UNSUPPORTED with tp_size > 1, or when no context split of the span attention
+ * fits the device's shared memory at this model's query heads per KV head (never on an H100 up to 8).  Returns after the copies.         */
+TCE_API int tce_llama_decode_span_host(tce_llama *m, int slot, int pos0, int n, const int *tokens_host, float *logits_host, int *next_tokens);
+typedef struct tce_lookup {
+    int max_draft;            /* 0..7 drafts per step; 0 = the plain greedy loop */
+    int ngram_min, ngram_max; /* 1 <= ngram_min <= ngram_max */
+} tce_lookup;
+typedef struct tce_lookup_stats {
+    int steps;    /* passes over the weights */
+    int drafted;  /* draft tokens verified */
+    int accepted; /* emitted ids that were drafts */
+} tce_lookup_stats;
+/* Greedy generation on slot 0 with prompt-lookup drafts: the ids tce_llama_generate gives at temp <= 0 (penalties over the last
+ * repeat_last_n ids of history + ids, then arg-max, lowest id on ties), up to rounding, in fewer passes over the weights.
+ * Drafter, before each step: S = corpus ++ history ++ [first_token] ++ ids so far, d = min(max_draft, n_predict - |ids| - 1,
+ * max_ctx - pos - 1) where pos is the position of S's last token.  For n = ngram_max down to ngram_min: take the last n tokens of S and
+ * find their most recent earlier occurrence S[p .. p + n) with p + n < |S| (at least one token after it); the draft is S[p + n ..
+ * min(p + n + d, |S|)).  The first n that matches wins; none (or d <= 0): no draft.
+ * Step: without a draft, the single-sequence decode step; with d drafts, the span step on [last id, drafts] at M = d + 1.  Row j is then
+ * sampled with the penalty window the one-token loop would have had after emitting drafts 0 .. j-1; drafts are accepted while row j's id
+ * equals draft j, and the step emits the accepted drafts plus the id of the first rejected row (of row d when all were accepted), cut at
+ * eos_id (inclusive) and at n_predict (clamped to max_ctx - pos0).  The host reads each step's ids back to draft the next one.
+ * KV rows of slot 0: rows pos0 .. pos0 + *n_out - 1 hold first_token and ids[0 .. *n_out - 2] (the last id is not decoded); rows
+ * pos0 + *n_out .. min(max_ctx, pos0 + *n_out + max_draft) - 1 may hold rows of rejected drafts; no other row of any slot changes.
+ * stats may be NULL.  TCE_ERR_INVALID, before anything is enqueued, for a bad first_token or pos0, n_predict < 0, n_history outside
+ * [0, max_ctx], n_corpus < 0, a NULL array with a non-zero count, NULL n_out (or out_tokens with n_predict > 0), max_draft outside [0, 7],
+ * ngram_min < 1 or ngram_min > ngram_max; TCE_ERR_UNSUPPORTED for temp > 0, tp_size > 1, or max_draft > 0 on a model the span step
+ * refuses as unsupported.                                                                                                              */
+TCE_API int tce_llama_generate_lookup(tce_llama *m, int first_token, int pos0, int n_predict, const tce_sampling *cfg, const int *history_host,
+                                      int n_history, const int *corpus_host, int n_corpus, const tce_lookup *lk, int eos_id, int *out_tokens_host,
+                                      int *n_out, tce_lookup_stats *stats);
 /* KV-cache row copy: rows src_pos .. src_pos + n - 1 of slot src_slot to rows dst_pos_host[i] .. dst_pos_host[i] + n - 1 of slot
  * dst_slots_host[i], for each of the n_dst destinations, in every layer, K and V, every KV head.  The source rows are read once for all
  * destinations.  The cache holds keys after RoPE, so a K row that moves by d = dst_pos - src_pos is rotated by d: rotate-half (dim j with

@@ -43,6 +43,16 @@ class GenRequest(C.Structure):
                 ("history", C.POINTER(C.c_int)), ("n_history", C.c_int), ("sampling", Sampling)]
 
 
+class Lookup(C.Structure):
+    """tce_lookup (include/tce_b200.h): the prompt-lookup drafter of tce_llama_generate_lookup."""
+    _fields_ = [("max_draft", C.c_int), ("ngram_min", C.c_int), ("ngram_max", C.c_int)]
+
+
+class LookupStats(C.Structure):
+    """tce_lookup_stats (include/tce_b200.h)."""
+    _fields_ = [("steps", C.c_int), ("drafted", C.c_int), ("accepted", C.c_int)]
+
+
 # every symbol include/tce_b200.h declares (tests/test_capi_symbols.py checks header <-> library <-> this table)
 SIGNATURES = {
     "tce_version": (C.c_int, []),
@@ -64,6 +74,7 @@ SIGNATURES = {
     "tce_opt_int8_attention": (C.c_int, [C.c_void_p] * 6 + [C.c_longlong] + [C.c_void_p] * 2 + [C.c_longlong, C.c_void_p, C.c_float, C.c_float] + [C.c_int] * 4 + [C.c_void_p]),
     "tce_attn_prefill": (C.c_int, [C.c_void_p] * 7 + [C.c_float] + [C.c_int] * 6),
     "tce_attn_decode": (C.c_int, [C.c_void_p] * 8 + [C.c_float] + [C.c_int] * 4),
+    "tce_attn_span": (C.c_int, [C.c_void_p] * 7 + [C.c_float] + [C.c_int] * 6),
     "tce_rmsnorm_f16": (C.c_int, [C.c_void_p] * 4 + [C.c_int, C.c_int, C.c_float]),
     "tce_argmax_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "tce_layernorm_q": (C.c_int, [C.c_void_p] * 5 + [C.c_int, C.c_int]),
@@ -87,6 +98,9 @@ SIGNATURES = {
     "tce_llama_score_batch": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 9),
     "tce_llama_generate_batch": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(GenRequest), C.c_void_p, C.c_int, C.c_void_p]),
     "tce_llama_kv_copy": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "tce_llama_decode_span_host": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tce_llama_generate_lookup": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                                            C.POINTER(Lookup), C.c_int, C.c_void_p, C.POINTER(C.c_int), C.POINTER(LookupStats)]),
     "tce_llama_batch_logits": (C.c_void_p, [C.c_void_p]),
     "tce_llama_logits": (C.c_void_p, [C.c_void_p]),
     "tce_llama_kv_cache": (C.c_void_p, [C.c_void_p, C.c_int, C.c_int]),

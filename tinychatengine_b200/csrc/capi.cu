@@ -366,6 +366,42 @@ int tce_attn_decode(tce_ctx *ctx, const void *qkv, void *k_cache, void *v_cache,
     return TCE_OK;
 }
 
+int tce_attn_span(tce_ctx *ctx, const void *qkv, void *k_cache, void *v_cache, const float *cosb, const float *sinb, void *out, float alpha, int n, int pos0,
+                  int num_heads, int num_kv_heads, int head_dim, int max_ctx) {
+    if (!ctx || !qkv || !k_cache || !v_cache || !cosb || !sinb || !out) return fail(TCE_ERR_INVALID, "tce_attn_span: null pointer");
+    if (head_dim != 128) return fail(TCE_ERR_UNSUPPORTED, "tce_attn_span: head_dim %d (only 128)", head_dim);
+    if (num_heads < 1 || num_kv_heads < 1 || num_heads % num_kv_heads || max_ctx < 1 || n < 1 || n > kMaxSpan || pos0 < 0 || pos0 > max_ctx - n)
+        return fail(TCE_ERR_INVALID, "tce_attn_span: bad shape n=%d pos0=%d max_ctx=%d", n, pos0, max_ctx);
+    const int chunk = attn_span_chunk(num_heads, num_kv_heads, ctx->attn_chunk, ctx->c.smem_optin);
+    if (!chunk) return fail(TCE_ERR_UNSUPPORTED, "tce_attn_span: no split fits shared memory at %d query heads per KV head", num_heads / num_kv_heads);
+    const size_t floats = (size_t)n * attn_decode_ws_floats(num_heads, max_ctx, chunk);
+    if (floats > (size_t)kMaxSpan * 128 * 1024 * (128 + 2) || num_kv_heads > 1024) return tce_fail_cuda(cudaErrorInvalidValue, "tce_attn_span");
+    CK(cudaSetDevice(ctx->c.device), "cudaSetDevice");
+    CK(attn_ws_reserve(ctx, floats, num_kv_heads), "tce_attn_span workspace");
+    AttnDecodeArgs a = {};
+    a.qkv = (const __half *)qkv;
+    a.k_cache = (__half *)k_cache;
+    a.v_cache = (__half *)v_cache;
+    a.cos = cosb;
+    a.sin = sinb;
+    a.span_pos0 = pos0;
+    a.out = (__half *)out;
+    a.alpha = alpha;
+    a.num_heads = num_heads;
+    a.num_kv_heads = num_kv_heads;
+    a.head_dim = head_dim;
+    a.max_ctx = max_ctx;
+    a.qkv_stride = (num_heads + 2 * num_kv_heads) * head_dim;
+    a.out_stride = num_heads * head_dim;
+    a.chunk = chunk;
+    a.ws = ctx->attn_ws;
+    a.ws_floats = ctx->attn_ws_floats;
+    a.counters = reinterpret_cast<unsigned *>(ctx->attn_ws + ctx->attn_ws_floats);
+    a.n_counters = ctx->attn_n_counters;
+    CK(launch_attn_span(&ctx->c, a, n, false), "tce_attn_span");
+    return TCE_OK;
+}
+
 int tce_attn_prefill(tce_ctx *ctx, void *qkv, void *k_cache, void *v_cache, const float *cosb, const float *sinb, void *out, float alpha, int n, int pos0,
                      int num_heads, int num_kv_heads, int head_dim, int max_ctx) {
     if (!ctx || !qkv || !k_cache || !v_cache || !cosb || !sinb || !out) return fail(TCE_ERR_INVALID, "tce_attn_prefill: null pointer");
@@ -590,6 +626,21 @@ int tce_llama_kv_copy(tce_llama *m, int src_slot, int src_pos, int n, int n_dst,
     std::string err;
     cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->kv_copy(src_slot, src_pos, n, n_dst, dst_slots_host, dst_pos_host, &err);
     return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_kv_copy", err);
+}
+int tce_llama_decode_span_host(tce_llama *m, int slot, int pos0, int n, const int *tokens_host, float *logits_host, int *next_tokens) {
+    if (!m || !tokens_host) return fail(TCE_ERR_INVALID, "tce_llama_decode_span_host: null argument");
+    std::string err;
+    cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->decode_span_host(slot, pos0, n, tokens_host, logits_host, next_tokens, &err);
+    return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_decode_span_host", err);
+}
+int tce_llama_generate_lookup(tce_llama *m, int first_token, int pos0, int n_predict, const tce_sampling *cfg, const int *history_host, int n_history,
+                              const int *corpus_host, int n_corpus, const tce_lookup *lk, int eos_id, int *out_tokens_host, int *n_out,
+                              tce_lookup_stats *stats) {
+    if (!m || !cfg || !lk || !n_out) return fail(TCE_ERR_INVALID, "tce_llama_generate_lookup: null argument");
+    std::string err;
+    cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->generate_lookup(first_token, pos0, n_predict, *cfg, history_host, n_history, corpus_host, n_corpus,
+                                                                         *lk, eos_id, out_tokens_host, n_out, stats, &err);
+    return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_generate_lookup", err);
 }
 const float *tce_llama_batch_logits(tce_llama *m) { return m ? reinterpret_cast<LlamaDecoder *>(m)->batch_logits() : nullptr; }
 const float *tce_llama_logits(tce_llama *m) { return m ? reinterpret_cast<LlamaDecoder *>(m)->logits() : nullptr; }

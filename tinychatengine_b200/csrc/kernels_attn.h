@@ -30,12 +30,22 @@ struct AttnDecodeArgs {
     __half *k_cache;     // [KVH][max_ctx][head_dim]
     __half *v_cache;     // [KVH][max_ctx][head_dim]
     const int *pos;      // device scalar: index of the token being decoded (= number of cached tokens)
+    int span_pos0;       // span attention without a request table: the position of row 0
 };
 // returns cudaErrorNotSupported for a head_dim or a query-heads-per-KV-head ratio the kernel does not cover, cudaErrorInvalidValue for a
 // workspace too small for the batch
 cudaError_t launch_attn_decode(Ctx *ctx, const AttnDecodeArgs &a, int batch, bool pdl);
 // floats of split workspace the kernel needs per sequence
 size_t attn_decode_ws_floats(int num_heads, int max_ctx, int chunk);
+// Span attention (attention.cu): rows 0..n-1 of qkv / out are tokens at positions pos0..pos0+n-1 of ONE sequence, given by the request table
+// (a.req rows 0..n-1 {token, pos0 + i, slot, valid}, host-checked: one slot, consecutive positions) or, without one, by k_cache / v_cache
+// and span_pos0.  Rotates and appends the n new K / V rows, then causal multi-query attention: row i sees cache rows 0..pos0+i.  Uses
+// n * attn_decode_ws_floats(H, max_ctx, chunk) floats of split records and KVH counters; a.chunk must be at most attn_span_chunk(...).
+constexpr int kMaxSpan = 8;
+cudaError_t launch_attn_span(Ctx *ctx, const AttnDecodeArgs &a, int n, bool pdl);
+// the largest multiple of 16 rows <= chunk (<= 0: the default) whose span CTA, at n = kMaxSpan, fits smem_optin bytes of shared memory;
+// 0 when none does.  At 8 query heads per KV head the 256-row default does not fit an H100's 227 KiB: the span runs 224-row splits.
+int attn_span_chunk(int num_heads, int num_kv_heads, int chunk, int smem_optin);
 
 // prompt processing (sqlen = n > 1): RoPE + KV append for rows pos0..pos0+n-1, causal attention over the cache.  Up to
 // kMaxPrefillSeqs prompts in one launch: their rows are concatenated, and each has its own positions and KV cache.
@@ -114,6 +124,19 @@ bool sampling_supported(float temp, int top_k, int n_vocab);
 cudaError_t launch_sample(Ctx *ctx, const SampleArgs &a, cudaStream_t stream);
 // rows_dev = device SampleArgs[rows]: row b is sampled by block b (the generate loop of the batched step; host-checked arguments)
 cudaError_t launch_sample_rows(const SampleArgs *rows_dev, int rows, cudaStream_t stream);
+// greedy acceptance of a speculative step (sampling.cu): rows = 1 + drafts logits rows at pitch ld, verified in one launch (a block per row)
+constexpr int kMaxDrafts = 7;
+struct AcceptArgs {
+    SampleArgs chain;          // the greedy chain (penalties, temp <= 0); logits = row 0; hist / hist_head / hist_cap = the history ring
+    size_t ld;                 // floats between logits rows
+    int rows;                  // 1 + number of drafts
+    int drafts[kMaxDrafts];    // draft j is verified by row j
+    int eos_id, budget;        // stop id (-1: none); ids the step may emit (>= 1)
+    int *greedy;               // device int[kMaxDrafts + 1] scratch
+    unsigned *arrive;          // device counter, zero between launches
+    int *result;               // device int[3 + kMaxDrafts + 1]: {emitted, stop (eos emitted), drafts among them, ids...}
+};
+cudaError_t launch_accept(const AcceptArgs &a, cudaStream_t stream);
 // standalone RMSNorm fp16 -> fp16 with fp32 gamma (reference LlamaRMSNorm_cuda, ops/cuda/LlamaRMSNorm.cu:68-115)
 cudaError_t launch_rmsnorm_f16(Ctx *ctx, const __half *x, const float *gamma, __half *y, int rows, int dim, float eps);
 // LayerNormQ::forward (llm/src/ops/LayerNormQ.cc:12-52), bit-exact (serial fp32 sums in the reference's order)

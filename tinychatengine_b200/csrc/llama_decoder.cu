@@ -683,6 +683,8 @@ void LlamaDecoder::drop_graphs() {
         g_bhost_[1][b].reset();
         g_bdev_[b].reset();
         g_bgen_[b].reset();
+        g_span_[0][b].reset();
+        g_span_[1][b].reset();
     }
 }
 
@@ -699,7 +701,13 @@ cudaError_t LlamaDecoder::batch_alloc(std::string *err) {
                  Q = (size_t)(cfg_.num_heads + 2 * cfg_.num_kv_heads) * cfg_.head_dim, A = (size_t)cfg_.num_heads * cfg_.head_dim;
     // all or nothing: the set is built aside and published whole; a failed allocation frees what this call took
     std::unique_ptr<BatchState> st = std::make_unique<BatchState>();
+    // the span step's attention runs the largest split that fits shared memory at 8 rows, and n <= 8 rows use the records of n sequences
+    st->span_chunk = attn_span_chunk(cfg_.num_heads, cfg_.num_kv_heads, attn_chunk_, ctx_->smem_optin);
     st->attn_ws_floats = B * attn_decode_ws_floats(cfg_.num_heads, cfg_.max_ctx, attn_chunk_);
+    if (st->span_chunk) {
+        const size_t span_ws = (size_t)kMaxSpan * attn_decode_ws_floats(cfg_.num_heads, cfg_.max_ctx, st->span_chunk);
+        st->attn_ws_floats = span_ws > st->attn_ws_floats ? span_ws : st->attn_ws_floats;
+    }
     st->n_counters = B * cfg_.num_kv_heads;
     __half *kv0 = d_kv_.get();
     cudaError_t e = cudaSuccess;
@@ -839,7 +847,7 @@ cudaError_t LlamaDecoder::reserve_slots(int n, std::string *err) {
     return cudaSuccess;
 }
 
-cudaError_t LlamaDecoder::enqueue_batch(int batch, const int *req, float *logits, int *next, cudaStream_t s, bool pdl) {
+cudaError_t LlamaDecoder::enqueue_batch(int batch, const int *req, float *logits, int *next, cudaStream_t s, bool pdl, bool span) {
     const BatchState &st = *bs_;
     // the K-sliced GEMVs' fix-up records are grown on the context itself (the launches below see a copy of it); a no-op after the first step
     long long records = 0;
@@ -863,7 +871,8 @@ cudaError_t LlamaDecoder::enqueue_batch(int batch, const int *req, float *logits
         DCK(gemv(st.gemv_ops[4 * l]));
         AttnDecodeArgs a = st.attn_ops[l];
         a.slots = st.slot_table.get();
-        DCK(launch_attn_decode(c, a, batch, pdl));
+        if (span) a.chunk = st.span_chunk;
+        DCK(span ? launch_attn_span(c, a, batch, pdl) : launch_attn_decode(c, a, batch, pdl));
         for (int i = 1; i < 4; i++) DCK(gemv(st.gemv_ops[4 * l + i]));
     }
     W4GemvParams lm = st.gemv_ops.back();
@@ -893,17 +902,170 @@ cudaError_t LlamaDecoder::decode_batch_host(int batch, const int *tokens, const 
         h_req[3 * b + 1] = positions[b];
         h_req[3 * b + 2] = slots[b];
     }
+    return host_rows(g_bhost_[logits_host ? 1 : 0][batch], batch, false, logits_host, next_tokens);
+}
+
+cudaError_t LlamaDecoder::host_rows(CachedGraph &g, int rows, bool span, float *logits_host, int *next_tokens) {
     const int want = logits_host ? 1 : 0;
-    const size_t lbytes = (size_t)batch * cfg_.vocab_size * sizeof(float);
-    DCK(run_graphed(g_bhost_[want][batch], nullptr, [&](cudaStream_t st, bool pdl) {
-        DCK(cudaMemcpyAsync(bs_->req.get(), h_req, (size_t)batch * 3 * sizeof(int), cudaMemcpyHostToDevice, st));
-        DCK(enqueue_batch(batch, bs_->req.get(), bs_->logits.get(), bs_->next.get(), st, pdl));
+    const size_t lbytes = (size_t)rows * cfg_.vocab_size * sizeof(float);
+    DCK(run_graphed(g, nullptr, [&](cudaStream_t st, bool pdl) {
+        DCK(cudaMemcpyAsync(bs_->req.get(), bs_->h_req.get(), (size_t)rows * 3 * sizeof(int), cudaMemcpyHostToDevice, st));
+        DCK(enqueue_batch(rows, bs_->req.get(), bs_->logits.get(), bs_->next.get(), st, pdl, span));
         if (want) DCK(cudaMemcpyAsync(bs_->h_logits.get(), bs_->logits.get(), lbytes, cudaMemcpyDeviceToHost, st));
-        return cudaMemcpyAsync(bs_->h_next.get(), bs_->next.get(), (size_t)batch * sizeof(int), cudaMemcpyDeviceToHost, st);
+        return cudaMemcpyAsync(bs_->h_next.get(), bs_->next.get(), (size_t)rows * sizeof(int), cudaMemcpyDeviceToHost, st);
     }));
     DCK(cudaStreamSynchronize(ctx_->stream));
     if (logits_host) memcpy(logits_host, bs_->h_logits.get(), lbytes);
-    if (next_tokens) memcpy(next_tokens, bs_->h_next.get(), (size_t)batch * sizeof(int));
+    if (next_tokens) memcpy(next_tokens, bs_->h_next.get(), (size_t)rows * sizeof(int));
+    return cudaSuccess;
+}
+
+// ------------------------------------------------------------------------------------------------ span step
+// n consecutive tokens of one slot in one pass over the weights: the batched step's chain at M = n with every row in the same slot, and the
+// span attention (append of the n new K / V rows, then causal multi-query attention) in place of the per-sequence attention.
+bool LlamaDecoder::span_ok(int slot, int pos0, int n, const int *tokens) const {
+    if (n < 1 || n > kMaxSpan || !tokens || slot < 0 || slot >= n_slots() || pos0 < 0 || pos0 > cfg_.max_ctx - n) return false;
+    for (int i = 0; i < n; i++)
+        if (tokens[i] < 0 || tokens[i] >= cfg_.vocab_size) return false;
+    return true;
+}
+
+cudaError_t LlamaDecoder::span_supported(std::string *err) const {
+    if (bs_->span_chunk > 0) return cudaSuccess;
+    if (err) *err = "the span attention's CTA does not fit this device's shared memory at this head ratio";
+    return cudaErrorNotSupported;
+}
+
+void LlamaDecoder::stage_span(int slot, int pos0, int n, const int *tokens) {
+    int *h_req = bs_->h_req.get();
+    for (int i = 0; i < n; i++) {
+        h_req[3 * i] = tokens[i];
+        h_req[3 * i + 1] = pos0 + i;
+        h_req[3 * i + 2] = slot;
+    }
+}
+
+cudaError_t LlamaDecoder::decode_span_host(int slot, int pos0, int n, const int *tokens, float *logits_host, int *next_tokens, std::string *err) {
+    if (tp_ > 1) return batch_alloc(err);  // not supported, with its message
+    if (!span_ok(slot, pos0, n, tokens)) return cudaErrorInvalidValue;
+    DCK(batch_alloc(err));
+    DCK(span_supported(err));
+    stage_span(slot, pos0, n, tokens);
+    return host_rows(g_span_[logits_host ? 1 : 0][n], n, true, logits_host, next_tokens);
+}
+
+// ------------------------------------------------------------------------------------------------ greedy speculative loop
+// Prompt-lookup drafter (the rule stated at tce_llama_generate_lookup): the tokens that followed the most recent earlier occurrence of the
+// longest suffix of S (ngram_max down to ngram_min) that has one.
+static_assert(kMaxSpan == TCE_LLAMA_MAX_BATCH && kMaxDrafts + 1 == kMaxSpan, "a span is one batched step's rows: the last token plus the drafts");
+static int lookup_draft(const std::vector<int> &S, const tce_lookup &lk, int d, int *out) {
+    const int len = (int)S.size();
+    if (d <= 0) return 0;
+    for (int ng = lk.ngram_max; ng >= lk.ngram_min; ng--) {
+        if (ng + 1 > len) continue;
+        const int *suf = S.data() + len - ng;
+        for (int p = len - ng - 1; p >= 0; p--) {
+            if (memcmp(S.data() + p, suf, (size_t)ng * sizeof(int))) continue;
+            const int avail = len - (p + ng), m = avail < d ? avail : d;
+            for (int i = 0; i < m; i++) out[i] = S[p + ng + i];
+            return m;
+        }
+    }
+    return 0;
+}
+
+cudaError_t LlamaDecoder::generate_lookup(int first_token, int pos0, int n_predict, const tce_sampling &sc, const int *history, int n_history, const int *corpus,
+                                          int n_corpus, const tce_lookup &lk, int eos_id, int *out_tokens, int *n_out, tce_lookup_stats *stats,
+                                          std::string *err) {
+    if (tp_ > 1) return batch_alloc(err);  // not supported, with its message
+    if (sc.temp > 0.f) {
+        if (err) *err = "speculative decoding is greedy only (temp <= 0)";
+        return cudaErrorNotSupported;
+    }
+    const int cap = cfg_.max_ctx;
+    if (first_token < 0 || first_token >= cfg_.vocab_size || pos0 < 0 || pos0 >= cap || n_predict < 0 || n_history < 0 || n_history > cap ||
+        n_corpus < 0 || (n_history > 0 && !history) || (n_corpus > 0 && !corpus) || !n_out || (n_predict > 0 && !out_tokens) || lk.max_draft < 0 ||
+        lk.max_draft > kMaxDrafts || lk.ngram_min < 1 || lk.ngram_min > lk.ngram_max)
+        return cudaErrorInvalidValue;
+    if (n_predict > cap - pos0) n_predict = cap - pos0;
+    DCK(batch_alloc(err));
+    if (lk.max_draft > 0) DCK(span_supported(err));
+    cudaStream_t s = ctx_->stream;
+    // [0] arrival counter, [1] history head, [4..15) step result, [16..24) greedy ids, then the history ring [max_ctx]
+    if (!d_spec_) DCK(dev_alloc(d_spec_, (size_t)(24 + cap)));
+    if (!h_spec_) DCK(host_alloc(h_spec_, 16));
+    int *ring = d_spec_.get() + 24;
+    DCK(cudaMemsetAsync(d_spec_.get(), 0, 24 * sizeof(int), s));
+    if (n_history > 0) DCK(cudaMemcpyAsync(ring, history, (size_t)n_history * sizeof(int), cudaMemcpyHostToDevice, s));
+    const int head0 = n_history;
+    DCK(cudaMemcpyAsync(d_spec_.get() + 1, &head0, sizeof(int), cudaMemcpyHostToDevice, s));
+    DCK(cudaStreamSynchronize(s));  // head0 and the caller's arrays are read by now
+    AcceptArgs acc{};
+    acc.chain = sample_args(sc, nullptr, cfg_.vocab_size);
+    acc.chain.hist = ring;
+    acc.chain.hist_head = d_spec_.get() + 1;
+    acc.chain.hist_cap = cap;
+    acc.eos_id = eos_id;
+    acc.ld = (size_t)cfg_.vocab_size;
+    acc.greedy = d_spec_.get() + 16;
+    acc.arrive = reinterpret_cast<unsigned *>(d_spec_.get());
+    acc.result = d_spec_.get() + 4;
+    std::vector<int> S;
+    S.reserve((size_t)n_corpus + n_history + 1 + n_predict);
+    S.insert(S.end(), corpus, corpus + n_corpus);
+    S.insert(S.end(), history, history + n_history);
+    S.push_back(first_token);
+    tce_lookup_stats st{0, 0, 0};
+    int n = 0, pos = pos0, last = first_token;
+    int *res = h_spec_.get();
+    while (n < n_predict) {
+        const int left = n_predict - n;
+        int lim = lk.max_draft;
+        if (lim > left - 1) lim = left - 1;
+        if (lim > cap - pos - 1) lim = cap - pos - 1;
+        const int d = lookup_draft(S, lk, lim, acc.drafts);
+        acc.rows = d + 1;
+        acc.budget = left;
+        if (d == 0) {
+            // the single-sequence step (the persistent kernel where it applies), as tce_llama_generate runs it
+            int *h = h_tokpos_.get();
+            h[0] = last;
+            h[1] = pos;
+            h[2] = 0;
+            DCK(cudaMemcpyAsync(d_tokpos_.get(), h, 3 * sizeof(int), cudaMemcpyHostToDevice, s));
+            DCK(run_graphed(g_dev_, d_tokpos_.get(), [&](cudaStream_t gs, bool pdl) { return enqueue_step(d_tokpos_.get(), gs, pdl); }));
+            acc.chain.logits = d_logits_.get();
+        } else {
+            int toks[kMaxSpan];
+            toks[0] = last;
+            for (int i = 0; i < d; i++) toks[i + 1] = acc.drafts[i];
+            stage_span(0, pos, d + 1, toks);
+            DCK(run_graphed(g_span_[0][d + 1], nullptr, [&](cudaStream_t gs, bool pdl) {
+                DCK(cudaMemcpyAsync(bs_->req.get(), bs_->h_req.get(), (size_t)(d + 1) * 3 * sizeof(int), cudaMemcpyHostToDevice, gs));
+                DCK(enqueue_batch(d + 1, bs_->req.get(), bs_->logits.get(), bs_->next.get(), gs, pdl, true));
+                return cudaMemcpyAsync(bs_->h_next.get(), bs_->next.get(), (size_t)(d + 1) * sizeof(int), cudaMemcpyDeviceToHost, gs);
+            }));
+            acc.chain.logits = bs_->logits.get();
+        }
+        DCK(launch_accept(acc, s));
+        // the host drafts the next step from these ids: one small read-back per step
+        DCK(cudaMemcpyAsync(res, acc.result, 11 * sizeof(int), cudaMemcpyDeviceToHost, s));
+        DCK(cudaStreamSynchronize(s));
+        const int emitted = res[0];
+        st.steps++;
+        st.drafted += d;
+        st.accepted += res[2];
+        for (int i = 0; i < emitted; i++) {
+            out_tokens[n + i] = res[3 + i];
+            S.push_back(res[3 + i]);
+        }
+        n += emitted;
+        pos += emitted;
+        last = res[3 + emitted - 1];
+        if (res[1]) break;
+    }
+    *n_out = n;
+    if (stats) *stats = st;
     return cudaSuccess;
 }
 

@@ -77,6 +77,11 @@ class LlamaDecoder {
     cudaError_t decode_batch_host(int batch, const int *tokens, const int *positions, const int *slots, float *logits_host, int *next_tokens,
                                   std::string *err);
     const float *batch_logits();
+    // span step: tokens[0..n) at positions pos0..pos0+n-1 of one slot in one pass (tce_llama_decode_span_host)
+    cudaError_t decode_span_host(int slot, int pos0, int n, const int *tokens, float *logits_host, int *next_tokens, std::string *err);
+    // greedy speculative loop on slot 0 with prompt-lookup drafts verified by the span step (tce_llama_generate_lookup)
+    cudaError_t generate_lookup(int first_token, int pos0, int n_predict, const tce_sampling &sc, const int *history, int n_history, const int *corpus,
+                                int n_corpus, const tce_lookup &lk, int eos_id, int *out_tokens, int *n_out, tce_lookup_stats *stats, std::string *err);
     // generate loop of up to TCE_LLAMA_MAX_BATCH sequences: one batched step + one sampler launch (a block per row) per token
     cudaError_t generate_batch(int batch, const tce_gen_request *reqs, int *out_tokens_host, int out_stride, int *n_out, std::string *err);
     // rows src_pos..src_pos+n-1 of src_slot to rows dst_pos[i].. of dst_slots[i] (every layer, K and V, K re-rotated by the position change):
@@ -124,7 +129,13 @@ class LlamaDecoder {
     // the batched step's buffers and parameters; cudaErrorNotSupported (+ *err) for a model the batched step does not cover
     cudaError_t batch_alloc(std::string *err);
     // raw kernel sequence of one batched step on req = device int[batch][3]; lm_head rows into logits[batch][V], greedy ids into next
-    cudaError_t enqueue_batch(int batch, const int *req, float *logits, int *next, cudaStream_t s, bool pdl);
+    // span: the rows are consecutive tokens of one slot (launch_attn_span instead of the per-sequence attention)
+    cudaError_t enqueue_batch(int batch, const int *req, float *logits, int *next, cudaStream_t s, bool pdl, bool span = false);
+    // one step of `rows` staged requests (bs_->h_req) through graph g, logits / greedy ids copied back
+    cudaError_t host_rows(CachedGraph &g, int rows, bool span, float *logits_host, int *next_tokens);
+    bool span_ok(int slot, int pos0, int n, const int *tokens) const;
+    cudaError_t span_supported(std::string *err) const;  // cudaErrorNotSupported (+ *err) when no span split fits shared memory
+    void stage_span(int slot, int pos0, int n, const int *tokens);  // the n requests of a span into bs_->h_req
     void drop_graphs();
 
     // tensor parallel state (the persistent kernel's hand-off buffers)
@@ -209,6 +220,7 @@ class LlamaDecoder {
         DevPtr<int> next;             // [8] greedy arg-max
         DevPtr<float> attn_ws;        // attention split records of 8 sequences at this model's max_ctx
         size_t attn_ws_floats = 0;
+        int span_chunk = 0;           // cached rows per CTA of the span attention (attn_span_chunk), 0: the span step is not supported
         DevPtr<unsigned> attn_counters;  // [8][KVH] split arrival counters
         size_t n_counters = 0;
         HostPtr<int> h_req, h_next;
@@ -228,6 +240,10 @@ class LlamaDecoder {
     CachedGraph g_bhost_[2][TCE_LLAMA_MAX_BATCH + 1];
     CachedGraph g_bdev_[TCE_LLAMA_MAX_BATCH + 1];
     CachedGraph g_bgen_[TCE_LLAMA_MAX_BATCH + 1];
+    CachedGraph g_span_[2][TCE_LLAMA_MAX_BATCH + 1];  // span step per n, with / without the logits copy
+    // speculative loop: device {counter, step result, greedy ids, history ring [max_ctx]} and the pinned read-back of one step's result
+    DevPtr<int> d_spec_;
+    HostPtr<int> h_spec_;
     bool use_graphs_ = true;
     bool atomic_residual_ = true;  // o_proj/down_proj partial tiles use RED.ADD (TCE_DETERMINISTIC=1 turns it off)
 };

@@ -64,22 +64,23 @@ TCE_DEVINL unsigned block_flag_scan(bool flag, unsigned *warp_tot, unsigned &tot
     return before + __popc(bal & ((1u << lane) - 1u));
 }
 
-// the whole chain for one sequence, on one kSampleThreads-thread block
-TCE_DEVINL void sample_one(const SampleArgs &a, SampleShared &sh) {
+// penalties + selection of the chain for one sequence, on one kSampleThreads-thread block; returns the id on thread 0 (sh.result, sh.size
+// and sh.p hold it for every thread after the call).  The window is the last W tokens of a sequence of `head` entries: entries below
+// ring_head come from the history ring, entries from ring_head on from `tail` (the acceptance kernel's drafts; tail = nullptr: head ==
+// ring_head).
+TCE_DEVINL int sample_chain(const SampleArgs &a, SampleShared &sh, int head, int ring_head, const int *tail) {
     const int tid = threadIdx.x;
-    if (a.stop && *a.stop) return;  // the sequence has ended (EOS drawn earlier): leave every buffer as it is
     float *logits = a.logits;
     const int V = a.n_vocab;
 
     // ---- window of recent tokens: the last `W` entries of the history ring (zeros before the first real token, as the reference's
     // last_n_tokens vector of n_ctx zeros, LLaMAGenerate.cu:43-44, 137-141) ----
     const int cap = a.hist_cap;
-    const int head = a.hist_head ? *a.hist_head : 0;  // entries written so far
     int W = a.repeat_last_n < 0 ? cap : (a.repeat_last_n < cap ? a.repeat_last_n : cap);
     if (!a.hist) W = 0;
     auto window = [&](int j) -> int {  // j-th entry of the window, oldest first
         const int logical = head - W + j;  // index into the unbounded sequence; negative = initial zero
-        return logical < 0 ? 0 : a.hist[logical % cap];
+        return logical < 0 ? 0 : (logical >= ring_head ? tail[logical - ring_head] : a.hist[logical % cap]);
     };
     const bool pen = W > 0 && (a.repeat_penalty != 1.0f || a.frequency_penalty != 0.0f || a.presence_penalty != 0.0f);
     if (pen) {
@@ -250,6 +251,20 @@ TCE_DEVINL void sample_one(const SampleArgs &a, SampleShared &sh) {
         }
         sh.result = result;
         sh.size = size;
+    }
+    __syncthreads();
+    return sh.result;
+}
+
+// the whole chain for one sequence, then the publishing of its id
+TCE_DEVINL void sample_one(const SampleArgs &a, SampleShared &sh) {
+    const int tid = threadIdx.x;
+    if (a.stop && *a.stop) return;  // the sequence has ended (EOS drawn earlier): leave every buffer as it is
+    const int cap = a.hist_cap;
+    const int head = a.hist_head ? *a.hist_head : 0;  // entries written so far
+    const int result = sample_chain(a, sh, head, head, nullptr);
+    auto cand_id = [&](int i) -> int { return (int)(0xFFFFFFFFu - (uint32_t)(sh.cand[i] & 0xFFFFFFFFull)); };
+    if (tid == 0) {
         // ---- publish: the token, the next decode step's {token, position}, the history ring, the output list, the stop flag ----
         if (a.out_token) *a.out_token = result;
         if (a.tokpos) {
@@ -298,7 +313,59 @@ __global__ void __launch_bounds__(kSampleThreads, 1) sample_rows_kernel(const Sa
     sample_one(rows[blockIdx.x], sh);
 }
 
+// Acceptance of a speculative step: block j runs the greedy chain on logits row j with the window the one-token loop would have had after
+// emitting drafts 0..j-1 (the ring, then drafts[<j]).  The last block to finish accepts drafts while row j's id equals draft j, emits them
+// plus the id of the first row whose draft was rejected (of the last row when none was), cut at eos_id (inclusive) and at the budget, and
+// appends the emitted ids to the history ring.
+__global__ void __launch_bounds__(kSampleThreads, 1) accept_kernel(const __grid_constant__ AcceptArgs a) {
+    __shared__ SampleShared sh;
+    __shared__ int drafts[kMaxDrafts];
+    __shared__ int is_last;
+    const int tid = threadIdx.x, j = blockIdx.x;
+    if (tid < kMaxDrafts) drafts[tid] = a.drafts[tid];
+    const int ring_head = *a.chain.hist_head;
+    __syncthreads();
+    SampleArgs s = a.chain;
+    s.logits += (size_t)j * a.ld;
+    const int id = sample_chain(s, sh, ring_head + j, ring_head, drafts);
+    if (tid == 0) {
+        a.greedy[j] = id;
+        __threadfence();
+        const unsigned prev = atomicAdd(a.arrive, 1u);
+        is_last = prev == (unsigned)(a.rows - 1);
+    }
+    __syncthreads();
+    if (!is_last || tid != 0) return;
+    __threadfence();
+    *a.arrive = 0u;  // re-armed for the next step
+    const volatile int *greedy = a.greedy;
+    int k = 0;
+    while (k < a.rows - 1 && greedy[k] == drafts[k]) k++;
+    int n = 0, stop = 0;
+    const int cap = a.chain.hist_cap;
+    for (int i = 0; i <= k && n < a.budget; i++) {
+        const int t = i < k ? drafts[i] : greedy[k];
+        a.result[3 + n] = t;
+        a.chain.hist[(ring_head + n) % cap] = t;
+        n++;
+        if (t == a.eos_id) {
+            stop = 1;
+            break;
+        }
+    }
+    *a.chain.hist_head = ring_head + n;
+    a.result[0] = n;
+    a.result[1] = stop;
+    a.result[2] = k < n ? k : n;  // emitted ids that were drafts
+}
+
 }  // namespace
+
+cudaError_t launch_accept(const AcceptArgs &a, cudaStream_t stream) {
+    if (a.rows < 1 || a.rows > kMaxDrafts + 1 || !a.chain.logits || !a.chain.hist || !a.chain.hist_head || a.chain.temp > 0.f) return cudaErrorInvalidValue;
+    accept_kernel<<<a.rows, kSampleThreads, 0, stream>>>(a);
+    return cudaGetLastError();
+}
 
 cudaError_t launch_sample_rows(const SampleArgs *rows_dev, int rows, cudaStream_t stream) {
     if (!rows_dev || rows < 1) return cudaErrorInvalidValue;

@@ -377,6 +377,36 @@ class LlamaModel:
         _lib.check(self.ctx.L.tce_llama_decode_batch_host(self.h, n, arr(tokens), arr(positions), arr(slots), p, nxt), "tce_llama_decode_batch_host")
         return list(nxt[:n])
 
+    def decode_span(self, tokens, pos0: int, slot: int = 0, logits_host=None) -> list[int]:
+        """Span step: up to MAX_BATCH consecutive tokens (host ints) at positions pos0.. of one slot in one pass over the weights; fills
+        logits_host (float32 [len(tokens), vocab], may be None; row i = the logits after tokens[i]) and returns the greedy ids of every row."""
+        n = len(tokens)
+        arr = (C.c_int * max(1, n))(*[int(t) for t in tokens])
+        nxt = (C.c_int * max(1, n))()
+        p = None if logits_host is None else C.c_void_p(logits_host.data_ptr())
+        _lib.check(self.ctx.L.tce_llama_decode_span_host(self.h, int(slot), int(pos0), n, arr, p, nxt), "tce_llama_decode_span_host")
+        return list(nxt[:n])
+
+    def generate_lookup(self, first_token: int, pos0: int, n_predict: int, *, history=(), corpus=(), max_draft=7, ngram=(1, 3), eos_id: int = -1,
+                        repeat_penalty=1.1, frequency_penalty=0.0, presence_penalty=0.0, repeat_last_n=64):
+        """Greedy generation on slot 0 with prompt-lookup drafts verified by the span step (tce_llama_generate_lookup): the ids of
+        generate(temp=0) with the same penalties, in fewer passes over the weights when the continuation repeats corpus / history / earlier
+        output.  Returns (ids, {"steps", "drafted", "accepted"})."""
+        import numpy as np
+
+        cfg = _lib.Sampling(40, 0.95, 0.0, float(repeat_penalty), float(frequency_penalty), float(presence_penalty), int(repeat_last_n), 0)
+        lk = _lib.Lookup(int(max_draft), int(ngram[0]), int(ngram[1]))
+        hist = np.ascontiguousarray(np.asarray(list(history), dtype=np.int32))
+        corp = np.ascontiguousarray(np.asarray(list(corpus), dtype=np.int32))
+        out = np.zeros(max(1, int(n_predict)), dtype=np.int32)
+        n = C.c_int(0)
+        st = _lib.LookupStats()
+        ptr = lambda a: a.ctypes.data_as(C.c_void_p) if a.size else None
+        _lib.check(self.ctx.L.tce_llama_generate_lookup(self.h, int(first_token), int(pos0), int(n_predict), C.byref(cfg), ptr(hist), int(hist.size),
+                                                        ptr(corp), int(corp.size), C.byref(lk), int(eos_id), out.ctypes.data_as(C.c_void_p),
+                                                        C.byref(n), C.byref(st)), "tce_llama_generate_lookup")
+        return out[:n.value].tolist(), {"steps": st.steps, "drafted": st.drafted, "accepted": st.accepted}
+
     def prefill_batch(self, prompts, slots, pos0s=None, logits_host=None) -> list[int]:
         """Prompt processing of up to MAX_BATCH prompts (lists of host ints) in one pass over the weights, prompt s into KV-cache slot
         slots[s] at positions pos0s[s].. (default 0); fills logits_host (float32 [n_prompts, vocab], may be None) with the logits of each

@@ -107,6 +107,11 @@ class Context:
                                           hd, max_ctx), "tce_attn_decode")
         return out
 
+    def attn_span(self, qkv, k_cache, v_cache, cos, sin, out, alpha, n, pos0, H, KVH, hd, max_ctx):
+        _lib.check(self.L.tce_attn_span(self.h, _ptr(qkv), _ptr(k_cache), _ptr(v_cache), _ptr(cos), _ptr(sin), _ptr(out), alpha, n, pos0, H, KVH, hd,
+                                        max_ctx), "tce_attn_span")
+        return out
+
     def attn_prefill(self, qkv, k_cache, v_cache, cos, sin, out, alpha, n, pos0, H, KVH, hd, max_ctx):
         _lib.check(self.L.tce_attn_prefill(self.h, _ptr(qkv), _ptr(k_cache), _ptr(v_cache), _ptr(cos), _ptr(sin), _ptr(out), alpha, n, pos0, H, KVH, hd,
                                            max_ctx), "tce_attn_prefill")
