@@ -313,6 +313,37 @@ typedef struct tce_lookup_stats {
 TCE_API int tce_llama_generate_lookup(tce_llama *m, int first_token, int pos0, int n_predict, const tce_sampling *cfg, const int *history_host,
                                       int n_history, const int *corpus_host, int n_corpus, const tce_lookup *lk, int eos_id, int *out_tokens_host,
                                       int *n_out, tce_lookup_stats *stats);
+/* ---- speculative sampling (any temp) --------------------------------------------------------------------------------------------------
+ * Acceptance rule of one step (speculative sampling, Leviathan et al. 2023 / Chen et al. 2023, with a one-hot draft distribution).  Inputs:
+ * the penalty sequence so far (h entries), d drafts x_0 .. x_{d-1}, and d + 1 logits rows, row j = the logits after [last, x_0 .. x_{j-1}].
+ * For each row j:
+ *   1. the chain of tce_sample (penalties over the last repeat_last_n entries of sequence ++ x_{<j}, top-k, top-p, temperature, softmax)
+ *      gives candidates c_j with probabilities p_j;
+ *   2. q_j = p_j[i*] when j < d and x_j = c_j[i*], else 0 (x_j cut by top-k / top-p; the last row: q_d = 0);
+ *   3. u_j = the uniform of draw index h + j (the one tce_llama_generate uses for its (h + j)-th id), and a_j = the uniform of the same
+ *      index in the stream of seed ^ TCE_SPEC_ACCEPT_STREAM;
+ *   4. r_j: with q_j = 0 the plain inverse-CDF draw with u_j (bit for bit tce_sample's); otherwise, with S = the sum of p_j[i] over i != i*
+ *      (candidate order, fp32) and t = u_j * S (one fp32 multiply), the first i != i* whose running sum over i != i* exceeds t (the last
+ *      i != i* if none).  S = 0: the row counts as accepted.
+ * k = the first j < d whose draft is not accepted (a_j < q_j is false), d if every draft is.  The step emits x_0 .. x_{k-1}, then r_k, cut
+ * at eos_id (inclusive) and at the budget; accepted = min(k, emitted).  At temp <= 0 this is the greedy rule: q_j = 1 exactly when x_j is
+ * the arg-max, and r_k is the arg-max.  Without drafts it is the plain sampled step.                                                     */
+#define TCE_SPEC_ACCEPT_STREAM 0xD1B54A32D192ED03ull
+/* The rule alone, on a caller's logits: logits_dev float[rows][ld] (row j: n_vocab floats, penalised IN PLACE), 1 <= rows <= 8,
+ * drafts_host int[rows - 1] (may be NULL when rows == 1), window_host = the penalty sequence, oldest first (may be NULL/0; entries before it
+ * read as 0), draw_index = h.  ids_host int[rows] receives the emitted ids, *n_out their count, *n_accepted the drafts among them, *stop 1
+ * when eos_id was emitted; q_host float[rows] (may be NULL) receives q_0 .. q_{rows-1}.  TCE_ERR_INVALID for a bad argument, budget < 1 or
+ * ld < n_vocab; TCE_ERR_UNSUPPORTED for temp > 0 without 1 <= top_k <= 1024 when n_vocab > 1024.  Synchronous.                          */
+TCE_API int tce_spec_accept(tce_ctx *ctx, float *logits_dev, int rows, long long ld, int n_vocab, const int *drafts_host, const int *window_host,
+                            int n_window, const tce_sampling *cfg, unsigned long long draw_index, int eos_id, int budget, int *ids_host, int *n_out,
+                            int *n_accepted, int *stop, float *q_host);
+/* tce_llama_generate_lookup at any temp: the same arguments, drafter, steps, stop rules, KV rows, stats and refusals, except that temp > 0
+ * is accepted (it needs 1 <= top_k <= 1024 when vocab > 1024, TCE_ERR_UNSUPPORTED otherwise), and each step applies the rule above with
+ * h = n_history + ids so far.  The emitted ids have the distribution of tce_llama_generate's with the same fields, but are not its ids,
+ * except at max_draft = 0 or temp <= 0, where they are.                                                                                  */
+TCE_API int tce_llama_sample_lookup(tce_llama *m, int first_token, int pos0, int n_predict, const tce_sampling *cfg, const int *history_host,
+                                    int n_history, const int *corpus_host, int n_corpus, const tce_lookup *lk, int eos_id, int *out_tokens_host,
+                                    int *n_out, tce_lookup_stats *stats);
 /* KV-cache row copy: rows src_pos .. src_pos + n - 1 of slot src_slot to rows dst_pos_host[i] .. dst_pos_host[i] + n - 1 of slot
  * dst_slots_host[i], for each of the n_dst destinations, in every layer, K and V, every KV head.  The source rows are read once for all
  * destinations.  The cache holds keys after RoPE, so a K row that moves by d = dst_pos - src_pos is rotated by d: rotate-half (dim j with

@@ -101,6 +101,10 @@ SIGNATURES = {
     "tce_llama_decode_span_host": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "tce_llama_generate_lookup": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_int, C.c_void_p, C.c_int,
                                             C.POINTER(Lookup), C.c_int, C.c_void_p, C.POINTER(C.c_int), C.POINTER(LookupStats)]),
+    "tce_llama_sample_lookup": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(Sampling), C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                                          C.POINTER(Lookup), C.c_int, C.c_void_p, C.POINTER(C.c_int), C.POINTER(LookupStats)]),
+    "tce_spec_accept": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(Sampling),
+                                  C.c_ulonglong, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]),
     "tce_llama_batch_logits": (C.c_void_p, [C.c_void_p]),
     "tce_llama_logits": (C.c_void_p, [C.c_void_p]),
     "tce_llama_kv_cache": (C.c_void_p, [C.c_void_p, C.c_int, C.c_int]),

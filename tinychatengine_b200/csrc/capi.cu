@@ -633,14 +633,73 @@ int tce_llama_decode_span_host(tce_llama *m, int slot, int pos0, int n, const in
     cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->decode_span_host(slot, pos0, n, tokens_host, logits_host, next_tokens, &err);
     return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_decode_span_host", err);
 }
-int tce_llama_generate_lookup(tce_llama *m, int first_token, int pos0, int n_predict, const tce_sampling *cfg, const int *history_host, int n_history,
-                              const int *corpus_host, int n_corpus, const tce_lookup *lk, int eos_id, int *out_tokens_host, int *n_out,
-                              tce_lookup_stats *stats) {
-    if (!m || !cfg || !lk || !n_out) return fail(TCE_ERR_INVALID, "tce_llama_generate_lookup: null argument");
+static int lookup_loop(const char *what, tce_llama *m, int first_token, int pos0, int n_predict, const tce_sampling *cfg, const int *history_host,
+                       int n_history, const int *corpus_host, int n_corpus, const tce_lookup *lk, int eos_id, int *out_tokens_host, int *n_out,
+                       tce_lookup_stats *stats) {
+    if (!m || !cfg || !lk || !n_out) return fail(TCE_ERR_INVALID, "%s: null argument", what);
     std::string err;
     cudaError_t e = reinterpret_cast<LlamaDecoder *>(m)->generate_lookup(first_token, pos0, n_predict, *cfg, history_host, n_history, corpus_host, n_corpus,
                                                                          *lk, eos_id, out_tokens_host, n_out, stats, &err);
-    return e == cudaSuccess ? TCE_OK : batch_fail(e, "tce_llama_generate_lookup", err);
+    return e == cudaSuccess ? TCE_OK : batch_fail(e, what, err);
+}
+int tce_llama_generate_lookup(tce_llama *m, int first_token, int pos0, int n_predict, const tce_sampling *cfg, const int *history_host, int n_history,
+                              const int *corpus_host, int n_corpus, const tce_lookup *lk, int eos_id, int *out_tokens_host, int *n_out,
+                              tce_lookup_stats *stats) {
+    if (cfg && cfg->temp > 0.f) return fail(TCE_ERR_UNSUPPORTED, "tce_llama_generate_lookup: greedy only (temp <= 0); tce_llama_sample_lookup samples");
+    return lookup_loop("tce_llama_generate_lookup", m, first_token, pos0, n_predict, cfg, history_host, n_history, corpus_host, n_corpus, lk, eos_id,
+                       out_tokens_host, n_out, stats);
+}
+int tce_llama_sample_lookup(tce_llama *m, int first_token, int pos0, int n_predict, const tce_sampling *cfg, const int *history_host, int n_history,
+                            const int *corpus_host, int n_corpus, const tce_lookup *lk, int eos_id, int *out_tokens_host, int *n_out,
+                            tce_lookup_stats *stats) {
+    return lookup_loop("tce_llama_sample_lookup", m, first_token, pos0, n_predict, cfg, history_host, n_history, corpus_host, n_corpus, lk, eos_id,
+                       out_tokens_host, n_out, stats);
+}
+int tce_spec_accept(tce_ctx *ctx, float *logits_dev, int rows, long long ld, int n_vocab, const int *drafts_host, const int *window_host, int n_window,
+                    const tce_sampling *cfg, unsigned long long draw_index, int eos_id, int budget, int *ids_host, int *n_out, int *n_accepted, int *stop,
+                    float *q_host) {
+    if (!ctx || !logits_dev || !cfg || !ids_host || !n_out || !n_accepted || !stop || rows < 1 || rows > kMaxDrafts + 1 || n_vocab < 1 ||
+        ld < n_vocab || (rows > 1 && !drafts_host) || n_window < 0 || (n_window > 0 && !window_host) || budget < 1)
+        return fail(TCE_ERR_INVALID, "tce_spec_accept: bad argument");
+    if (!sampling_supported(cfg->temp, cfg->top_k, n_vocab)) return fail(TCE_ERR_UNSUPPORTED, "tce_spec_accept: temp > 0 needs 1 <= top_k <= 1024");
+    CK(cudaSetDevice(ctx->c.device), "cudaSetDevice");
+    AcceptArgs a{};
+    a.chain = sample_args(*cfg, logits_dev, n_vocab);
+    // the penalty window of row j is the last repeat_last_n entries (n_window when < 0) of zeros ++ window ++ drafts[<j]: a ring that holds
+    // all of them, and the emitted ids, never wraps
+    if (a.chain.repeat_last_n < 0) a.chain.repeat_last_n = n_window;
+    const int cap = (n_window > a.chain.repeat_last_n ? n_window : a.chain.repeat_last_n) + rows;
+    int *scratch = nullptr;  // [0] arrival counter, [1] ring head, [4..15) result, [16..24) r, [24..32) q, then the ring
+    CK(cudaMalloc((void **)&scratch, (32 + (size_t)cap) * sizeof(int)), "tce_spec_accept: scratch");
+    cudaStream_t s = ctx->c.stream;
+    cudaError_t e = cudaMemsetAsync(scratch, 0, 32 * sizeof(int), s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(scratch + 1, &n_window, sizeof(int), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && n_window > 0) e = cudaMemcpyAsync(scratch + 32, window_host, (size_t)n_window * sizeof(int), cudaMemcpyHostToDevice, s);
+    a.chain.draw_index = draw_index - (unsigned long long)n_window;  // row j draws with index draw_index + j
+    a.chain.hist = scratch + 32;
+    a.chain.hist_head = scratch + 1;
+    a.chain.hist_cap = cap;
+    a.ld = (size_t)ld;
+    a.rows = rows;
+    for (int i = 0; i < rows - 1; i++) a.drafts[i] = drafts_host[i];
+    a.eos_id = eos_id;
+    a.budget = budget;
+    a.arrive = reinterpret_cast<unsigned *>(scratch);
+    a.result = scratch + 4;
+    a.repl = scratch + 16;
+    a.q = reinterpret_cast<float *>(scratch + 24);
+    if (e == cudaSuccess) e = launch_accept(a, s);
+    int out[32];
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out, scratch, sizeof(out), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    cudaFree(scratch);
+    if (e != cudaSuccess) return fail(TCE_ERR_CUDA, "tce_spec_accept: %s", cudaGetErrorString(e));
+    *n_out = out[4];
+    *stop = out[5];
+    *n_accepted = out[6];
+    for (int i = 0; i < out[4]; i++) ids_host[i] = out[7 + i];
+    if (q_host) memcpy(q_host, out + 24, (size_t)rows * sizeof(float));
+    return TCE_OK;
 }
 const float *tce_llama_batch_logits(tce_llama *m) { return m ? reinterpret_cast<LlamaDecoder *>(m)->batch_logits() : nullptr; }
 const float *tce_llama_logits(tce_llama *m) { return m ? reinterpret_cast<LlamaDecoder *>(m)->logits() : nullptr; }

@@ -124,18 +124,22 @@ bool sampling_supported(float temp, int top_k, int n_vocab);
 cudaError_t launch_sample(Ctx *ctx, const SampleArgs &a, cudaStream_t stream);
 // rows_dev = device SampleArgs[rows]: row b is sampled by block b (the generate loop of the batched step; host-checked arguments)
 cudaError_t launch_sample_rows(const SampleArgs *rows_dev, int rows, cudaStream_t stream);
-// greedy acceptance of a speculative step (sampling.cu): rows = 1 + drafts logits rows at pitch ld, verified in one launch (a block per row)
+// acceptance of a speculative step (sampling.cu, the rule of tce_spec_accept): rows = 1 + drafts logits rows at pitch ld, verified in one
+// launch (a block per row)
 constexpr int kMaxDrafts = 7;
 struct AcceptArgs {
-    SampleArgs chain;          // the greedy chain (penalties, temp <= 0); logits = row 0; hist / hist_head / hist_cap = the history ring
+    SampleArgs chain;          // the chain (any temp); logits = row 0; hist / hist_head / hist_cap = the history ring; row j draws with
+                               // index draw_index + *hist_head + j
     size_t ld;                 // floats between logits rows
     int rows;                  // 1 + number of drafts
     int drafts[kMaxDrafts];    // draft j is verified by row j
     int eos_id, budget;        // stop id (-1: none); ids the step may emit (>= 1)
-    int *greedy;               // device int[kMaxDrafts + 1] scratch
+    int *repl;                 // device int[kMaxDrafts + 1] scratch: r_j
+    float *q;                  // device float[kMaxDrafts + 1]: q_j, the probability of draft j under row j's chain (0 for the last row)
     unsigned *arrive;          // device counter, zero between launches
     int *result;               // device int[3 + kMaxDrafts + 1]: {emitted, stop (eos emitted), drafts among them, ids...}
 };
+// cudaErrorNotSupported where sampling_supported refuses the chain
 cudaError_t launch_accept(const AcceptArgs &a, cudaStream_t stream);
 // standalone RMSNorm fp16 -> fp16 with fp32 gamma (reference LlamaRMSNorm_cuda, ops/cuda/LlamaRMSNorm.cu:68-115)
 cudaError_t launch_rmsnorm_f16(Ctx *ctx, const __half *x, const float *gamma, __half *y, int rows, int dim, float eps);

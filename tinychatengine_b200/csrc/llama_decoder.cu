@@ -954,7 +954,7 @@ cudaError_t LlamaDecoder::decode_span_host(int slot, int pos0, int n, const int 
     return host_rows(g_span_[logits_host ? 1 : 0][n], n, true, logits_host, next_tokens);
 }
 
-// ------------------------------------------------------------------------------------------------ greedy speculative loop
+// ------------------------------------------------------------------------------------------------ speculative loop
 // Prompt-lookup drafter (the rule stated at tce_llama_generate_lookup): the tokens that followed the most recent earlier occurrence of the
 // longest suffix of S (ngram_max down to ngram_min) that has one.
 static_assert(kMaxSpan == TCE_LLAMA_MAX_BATCH && kMaxDrafts + 1 == kMaxSpan, "a span is one batched step's rows: the last token plus the drafts");
@@ -978,24 +978,25 @@ cudaError_t LlamaDecoder::generate_lookup(int first_token, int pos0, int n_predi
                                           int n_corpus, const tce_lookup &lk, int eos_id, int *out_tokens, int *n_out, tce_lookup_stats *stats,
                                           std::string *err) {
     if (tp_ > 1) return batch_alloc(err);  // not supported, with its message
-    if (sc.temp > 0.f) {
-        if (err) *err = "speculative decoding is greedy only (temp <= 0)";
-        return cudaErrorNotSupported;
-    }
     const int cap = cfg_.max_ctx;
     if (first_token < 0 || first_token >= cfg_.vocab_size || pos0 < 0 || pos0 >= cap || n_predict < 0 || n_history < 0 || n_history > cap ||
         n_corpus < 0 || (n_history > 0 && !history) || (n_corpus > 0 && !corpus) || !n_out || (n_predict > 0 && !out_tokens) || lk.max_draft < 0 ||
         lk.max_draft > kMaxDrafts || lk.ngram_min < 1 || lk.ngram_min > lk.ngram_max)
         return cudaErrorInvalidValue;
+    if (!sampling_supported(sc.temp, sc.top_k, cfg_.vocab_size)) {
+        if (err) *err = "temp > 0 needs 1 <= top_k <= 1024";
+        return cudaErrorNotSupported;
+    }
     if (n_predict > cap - pos0) n_predict = cap - pos0;
     DCK(batch_alloc(err));
     if (lk.max_draft > 0) DCK(span_supported(err));
     cudaStream_t s = ctx_->stream;
-    // [0] arrival counter, [1] history head, [4..15) step result, [16..24) greedy ids, then the history ring [max_ctx]
-    if (!d_spec_) DCK(dev_alloc(d_spec_, (size_t)(24 + cap)));
+    // [0] arrival counter, [1] history head, [4..15) step result, [16..24) replacement ids, [24..32) draft probabilities, then the history
+    // ring [max_ctx]
+    if (!d_spec_) DCK(dev_alloc(d_spec_, (size_t)(32 + cap)));
     if (!h_spec_) DCK(host_alloc(h_spec_, 16));
-    int *ring = d_spec_.get() + 24;
-    DCK(cudaMemsetAsync(d_spec_.get(), 0, 24 * sizeof(int), s));
+    int *ring = d_spec_.get() + 32;
+    DCK(cudaMemsetAsync(d_spec_.get(), 0, 32 * sizeof(int), s));
     if (n_history > 0) DCK(cudaMemcpyAsync(ring, history, (size_t)n_history * sizeof(int), cudaMemcpyHostToDevice, s));
     const int head0 = n_history;
     DCK(cudaMemcpyAsync(d_spec_.get() + 1, &head0, sizeof(int), cudaMemcpyHostToDevice, s));
@@ -1007,7 +1008,8 @@ cudaError_t LlamaDecoder::generate_lookup(int first_token, int pos0, int n_predi
     acc.chain.hist_cap = cap;
     acc.eos_id = eos_id;
     acc.ld = (size_t)cfg_.vocab_size;
-    acc.greedy = d_spec_.get() + 16;
+    acc.repl = d_spec_.get() + 16;
+    acc.q = reinterpret_cast<float *>(d_spec_.get() + 24);
     acc.arrive = reinterpret_cast<unsigned *>(d_spec_.get());
     acc.result = d_spec_.get() + 4;
     std::vector<int> S;

@@ -79,7 +79,8 @@ class LlamaDecoder {
     const float *batch_logits();
     // span step: tokens[0..n) at positions pos0..pos0+n-1 of one slot in one pass (tce_llama_decode_span_host)
     cudaError_t decode_span_host(int slot, int pos0, int n, const int *tokens, float *logits_host, int *next_tokens, std::string *err);
-    // greedy speculative loop on slot 0 with prompt-lookup drafts verified by the span step (tce_llama_generate_lookup)
+    // speculative loop on slot 0 with prompt-lookup drafts verified by the span step and the acceptance rule of tce_spec_accept
+    // (tce_llama_sample_lookup; tce_llama_generate_lookup at temp <= 0)
     cudaError_t generate_lookup(int first_token, int pos0, int n_predict, const tce_sampling &sc, const int *history, int n_history, const int *corpus,
                                 int n_corpus, const tce_lookup &lk, int eos_id, int *out_tokens, int *n_out, tce_lookup_stats *stats, std::string *err);
     // generate loop of up to TCE_LLAMA_MAX_BATCH sequences: one batched step + one sampler launch (a block per row) per token

@@ -45,6 +45,7 @@ struct SampleShared {
     unsigned warp_tot[2][32];
     unsigned prefix, need, base_gt, base_eq;
     int result, size;
+    float q;  // probability of the excluded id (0: none, or not a candidate)
 };
 
 // block-wide exclusive scan of one flag per thread over a chunk; returns this thread's offset, `total` = chunk total
@@ -68,7 +69,10 @@ TCE_DEVINL unsigned block_flag_scan(bool flag, unsigned *warp_tot, unsigned &tot
 // and sh.p hold it for every thread after the call).  The window is the last W tokens of a sequence of `head` entries: entries below
 // ring_head come from the history ring, entries from ring_head on from `tail` (the acceptance kernel's drafts; tail = nullptr: head ==
 // ring_head).
-TCE_DEVINL int sample_chain(const SampleArgs &a, SampleShared &sh, int head, int ring_head, const int *tail) {
+// excl >= 0 (a draft): sh.q = its probability p[i*] when it is a candidate, else 0.  With q = 0 the id is the plain draw.  With q > 0 it
+// is the replacement draw of speculative sampling: the same uniform u scaled to S = the sum of p[i] over i != i* (candidate order, fp32),
+// and the first i != i* whose running sum over i != i* exceeds u * S (the last i != i* if none); -1 when S = 0 (nothing to replace with).
+TCE_DEVINL int sample_chain(const SampleArgs &a, SampleShared &sh, int head, int ring_head, const int *tail, int excl = -1) {
     const int tid = threadIdx.x;
     float *logits = a.logits;
     const int V = a.n_vocab;
@@ -206,6 +210,7 @@ TCE_DEVINL int sample_chain(const SampleArgs &a, SampleShared &sh, int head, int
     if (tid == 0) {
         int size = K;
         int result;
+        float u = 0.f;
         if (greedy) {
             result = cand_id(0);  // the largest logit, lowest id among equals (std::max_element keeps the first)
             size = 1;
@@ -238,7 +243,7 @@ TCE_DEVINL int sample_chain(const SampleArgs &a, SampleShared &sh, int head, int
                 cum = __fadd_rn(cum, sh.p[i]);
             }
             for (int i = 0; i < size; i++) sh.p[i] = __fdiv_rn(sh.p[i], cum);
-            const float u = uniform01(a.seed, a.draw_index + (a.hist_head ? (unsigned long long)head : 0ull));
+            u = uniform01(a.seed, a.draw_index + (a.hist_head ? (unsigned long long)head : 0ull));
             float run = 0.f;
             result = cand_id(size - 1);
             for (int i = 0; i < size; i++) {
@@ -249,8 +254,36 @@ TCE_DEVINL int sample_chain(const SampleArgs &a, SampleShared &sh, int head, int
                 }
             }
         }
+        float q = 0.f;
+        int ex = -1;
+        if (excl >= 0) {
+            for (int i = 0; i < size; i++) {
+                if (cand_id(i) == excl) {
+                    ex = i;
+                    q = sh.p[i];
+                    break;
+                }
+            }
+        }
+        if (q > 0.f) {  // greedy: the arg-max is the only candidate, so S = 0
+            float S = 0.f;
+            for (int i = 0; i < size; i++)
+                if (i != ex) S = __fadd_rn(S, sh.p[i]);
+            result = -1;
+            if (S > 0.f) {
+                const float t = __fmul_rn(u, S);
+                float run = 0.f;
+                for (int i = 0; i < size; i++) {
+                    if (i == ex) continue;
+                    run = __fadd_rn(run, sh.p[i]);
+                    result = cand_id(i);
+                    if (t < run) break;
+                }
+            }
+        }
         sh.result = result;
         sh.size = size;
+        sh.q = q;
     }
     __syncthreads();
     return sh.result;
@@ -313,10 +346,11 @@ __global__ void __launch_bounds__(kSampleThreads, 1) sample_rows_kernel(const Sa
     sample_one(rows[blockIdx.x], sh);
 }
 
-// Acceptance of a speculative step: block j runs the greedy chain on logits row j with the window the one-token loop would have had after
-// emitting drafts 0..j-1 (the ring, then drafts[<j]).  The last block to finish accepts drafts while row j's id equals draft j, emits them
-// plus the id of the first row whose draft was rejected (of the last row when none was), cut at eos_id (inclusive) and at the budget, and
-// appends the emitted ids to the history ring.
+// Acceptance of a speculative step (the rule stated at tce_spec_accept): block j runs the chain on logits row j with the window the
+// one-token loop would have had after emitting drafts 0..j-1 (the ring, then drafts[<j]) and draft j (none for the last row) as the
+// excluded id, and publishes {q_j, r_j}.  The last block to finish accepts drafts while a_j < q_j (or r_j = -1: no other candidate), emits
+// them plus r_k of the first row k not accepted (of the last row when every draft was), cut at eos_id (inclusive) and at the budget, and
+// appends the emitted ids to the history ring.  At temp <= 0, q_j is 1 when draft j is the arg-max and 0 otherwise: the greedy rule.
 __global__ void __launch_bounds__(kSampleThreads, 1) accept_kernel(const __grid_constant__ AcceptArgs a) {
     __shared__ SampleShared sh;
     __shared__ int drafts[kMaxDrafts];
@@ -327,9 +361,10 @@ __global__ void __launch_bounds__(kSampleThreads, 1) accept_kernel(const __grid_
     __syncthreads();
     SampleArgs s = a.chain;
     s.logits += (size_t)j * a.ld;
-    const int id = sample_chain(s, sh, ring_head + j, ring_head, drafts);
+    const int r = sample_chain(s, sh, ring_head + j, ring_head, drafts, j < a.rows - 1 ? drafts[j] : -1);
     if (tid == 0) {
-        a.greedy[j] = id;
+        a.repl[j] = r;
+        a.q[j] = sh.q;
         __threadfence();
         const unsigned prev = atomicAdd(a.arrive, 1u);
         is_last = prev == (unsigned)(a.rows - 1);
@@ -338,13 +373,16 @@ __global__ void __launch_bounds__(kSampleThreads, 1) accept_kernel(const __grid_
     if (!is_last || tid != 0) return;
     __threadfence();
     *a.arrive = 0u;  // re-armed for the next step
-    const volatile int *greedy = a.greedy;
+    const volatile int *repl = a.repl;
+    const volatile float *q = a.q;
+    // row j's acceptance uniform has the index of its draw uniform, u_j, in the second counter stream
+    const unsigned long long idx0 = a.chain.draw_index + (unsigned long long)ring_head;
     int k = 0;
-    while (k < a.rows - 1 && greedy[k] == drafts[k]) k++;
+    while (k < a.rows - 1 && (repl[k] < 0 || uniform01(a.chain.seed ^ TCE_SPEC_ACCEPT_STREAM, idx0 + k) < q[k])) k++;
     int n = 0, stop = 0;
     const int cap = a.chain.hist_cap;
     for (int i = 0; i <= k && n < a.budget; i++) {
-        const int t = i < k ? drafts[i] : greedy[k];
+        const int t = i < k ? drafts[i] : repl[k];
         a.result[3 + n] = t;
         a.chain.hist[(ring_head + n) % cap] = t;
         n++;
@@ -362,7 +400,10 @@ __global__ void __launch_bounds__(kSampleThreads, 1) accept_kernel(const __grid_
 }  // namespace
 
 cudaError_t launch_accept(const AcceptArgs &a, cudaStream_t stream) {
-    if (a.rows < 1 || a.rows > kMaxDrafts + 1 || !a.chain.logits || !a.chain.hist || !a.chain.hist_head || a.chain.temp > 0.f) return cudaErrorInvalidValue;
+    if (a.rows < 1 || a.rows > kMaxDrafts + 1 || !a.chain.logits || !a.chain.hist || !a.chain.hist_head || a.chain.hist_cap < 1 || !a.repl || !a.q ||
+        !a.arrive || !a.result)
+        return cudaErrorInvalidValue;
+    if (!sampling_supported(a.chain.temp, a.chain.top_k, a.chain.n_vocab)) return cudaErrorNotSupported;
     accept_kernel<<<a.rows, kSampleThreads, 0, stream>>>(a);
     return cudaGetLastError();
 }

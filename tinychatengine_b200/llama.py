@@ -388,13 +388,21 @@ class LlamaModel:
         return list(nxt[:n])
 
     def generate_lookup(self, first_token: int, pos0: int, n_predict: int, *, history=(), corpus=(), max_draft=7, ngram=(1, 3), eos_id: int = -1,
-                        repeat_penalty=1.1, frequency_penalty=0.0, presence_penalty=0.0, repeat_last_n=64):
-        """Greedy generation on slot 0 with prompt-lookup drafts verified by the span step (tce_llama_generate_lookup): the ids of
-        generate(temp=0) with the same penalties, in fewer passes over the weights when the continuation repeats corpus / history / earlier
-        output.  Returns (ids, {"steps", "drafted", "accepted"})."""
+                        repeat_penalty=1.1, frequency_penalty=0.0, presence_penalty=0.0, repeat_last_n=64, temp=0.0, top_k=40, top_p=0.95, seed=0):
+        """Generation on slot 0 with prompt-lookup drafts verified by the span step, in fewer passes over the weights when the continuation
+        repeats corpus / history / earlier output.  temp <= 0 (tce_llama_generate_lookup): the ids of generate(temp=0) with the same penalties.
+        temp > 0 (tce_llama_sample_lookup): drafts are accepted by speculative sampling, so the ids have the distribution of
+        generate(temp=temp, ...) with the same fields, and at max_draft = 0 they are its ids for the same seed.
+        Returns (ids, {"steps", "drafted", "accepted"})."""
         import numpy as np
 
-        cfg = _lib.Sampling(40, 0.95, 0.0, float(repeat_penalty), float(frequency_penalty), float(presence_penalty), int(repeat_last_n), 0)
+        if temp > 0:
+            cfg = _lib.Sampling(int(top_k), float(top_p), float(temp), float(repeat_penalty), float(frequency_penalty), float(presence_penalty),
+                                int(repeat_last_n), int(seed))
+            fn, name = self.ctx.L.tce_llama_sample_lookup, "tce_llama_sample_lookup"
+        else:
+            cfg = _lib.Sampling(40, 0.95, 0.0, float(repeat_penalty), float(frequency_penalty), float(presence_penalty), int(repeat_last_n), 0)
+            fn, name = self.ctx.L.tce_llama_generate_lookup, "tce_llama_generate_lookup"
         lk = _lib.Lookup(int(max_draft), int(ngram[0]), int(ngram[1]))
         hist = np.ascontiguousarray(np.asarray(list(history), dtype=np.int32))
         corp = np.ascontiguousarray(np.asarray(list(corpus), dtype=np.int32))
@@ -402,9 +410,8 @@ class LlamaModel:
         n = C.c_int(0)
         st = _lib.LookupStats()
         ptr = lambda a: a.ctypes.data_as(C.c_void_p) if a.size else None
-        _lib.check(self.ctx.L.tce_llama_generate_lookup(self.h, int(first_token), int(pos0), int(n_predict), C.byref(cfg), ptr(hist), int(hist.size),
-                                                        ptr(corp), int(corp.size), C.byref(lk), int(eos_id), out.ctypes.data_as(C.c_void_p),
-                                                        C.byref(n), C.byref(st)), "tce_llama_generate_lookup")
+        _lib.check(fn(self.h, int(first_token), int(pos0), int(n_predict), C.byref(cfg), ptr(hist), int(hist.size), ptr(corp), int(corp.size), C.byref(lk),
+                      int(eos_id), out.ctypes.data_as(C.c_void_p), C.byref(n), C.byref(st)), name)
         return out[:n.value].tolist(), {"steps": st.steps, "drafted": st.drafted, "accepted": st.accepted}
 
     def prefill_batch(self, prompts, slots, pos0s=None, logits_host=None) -> list[int]:

@@ -157,6 +157,29 @@ class Context:
             return tok.value, ids[:cnt.value].copy(), probs[:cnt.value].copy()
         return tok.value
 
+    def spec_accept(self, logits, drafts=(), window=(), *, top_k=40, top_p=0.95, temp=0.8, repeat_penalty=1.1, frequency_penalty=0.0,
+                    presence_penalty=0.0, repeat_last_n=64, seed=0, draw_index=0, eos_id=-1, budget=None):
+        """The acceptance rule of one speculative step (tce_spec_accept) on `logits` (float32 CUDA tensor [len(drafts) + 1, V], penalised in
+        place).  Returns (ids, accepted, stop, q)."""
+        import ctypes as C
+
+        import numpy as np
+
+        rows = len(drafts) + 1
+        assert logits.dim() == 2 and logits.shape[0] == rows and logits.stride(1) == 1
+        cfg = _lib.Sampling(int(top_k), float(top_p), float(temp), float(repeat_penalty), float(frequency_penalty), float(presence_penalty),
+                            int(repeat_last_n), int(seed))
+        dr = np.ascontiguousarray(np.asarray(list(drafts), dtype=np.int32))
+        win = np.ascontiguousarray(np.asarray(list(window), dtype=np.int32))
+        ids = np.zeros(rows, dtype=np.int32)
+        q = np.zeros(rows, dtype=np.float32)
+        n, acc, stop = C.c_int(0), C.c_int(0), C.c_int(0)
+        ptr = lambda a: a.ctypes.data_as(C.c_void_p) if a.size else None
+        _lib.check(self.L.tce_spec_accept(self.h, _ptr(logits), rows, logits.stride(0), logits.shape[1], ptr(dr), ptr(win), int(win.size), C.byref(cfg),
+                                          int(draw_index), int(eos_id), int(rows if budget is None else budget), ptr(ids), C.byref(n), C.byref(acc),
+                                          C.byref(stop), ptr(q)), "tce_spec_accept")
+        return ids[:n.value].tolist(), acc.value, stop.value, q
+
     def argmax_f32(self, x, out=None):
         if out is None:
             out = torch.empty((1,), dtype=torch.int32, device=x.device)
