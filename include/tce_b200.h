@@ -215,9 +215,10 @@ TCE_API int tce_sample(tce_ctx *ctx, float *logits_dev, int n_vocab, const int *
                        unsigned long long draw_index, int *token_host, int *cand_ids_host, float *cand_probs_host, int *cand_count_host);
 /* generate loop: decode `first_token` at position pos0, sample, feed the sample back, ... for at most n_predict tokens or until eos_id
  * is drawn or the context is full.  history_host (n_history recent tokens, oldest first) seeds the penalty window.  Only the generated
- * ids (4 bytes each) cross PCIe.  Single GPU (tp_size == 1).  KV rows, in slot 0: the loop decodes rows pos0 .. pos0 + *n_out - 1 (the
- * last id is not decoded), as tce_llama_generate_batch does, and stops there when it ran out of budget or context.  After an eos_id stop
- * the steps already queued behind it may also decode the eos id into row pos0 + *n_out (when that is below max_ctx); no row past it.    */
+ * ids (4 bytes each) cross PCIe.  Single GPU (tp_size == 1).  It is the loop of tce_llama_generate_batch on one sequence in slot 0, with
+ * the single-sequence step: on return slot 0 holds exactly *n_out new rows, at pos0 .. pos0 + *n_out - 1 (the last id is not decoded),
+ * whether it stopped at eos_id, at n_predict or at max_ctx.  TCE_ERR_INVALID, before anything is enqueued, for a bad first_token or pos0,
+ * n_predict < 0, n_history outside [0, max_ctx], a NULL history with n_history > 0, or a NULL output.                                 */
 TCE_API int tce_llama_generate(tce_llama *m, int first_token, int pos0, int n_predict, const tce_sampling *cfg, const int *history_host,
                                int n_history, int eos_id, int *out_tokens_host, int *n_out);
 /* ---- batched decode: up to TCE_LLAMA_MAX_BATCH sequences per step, each in its own KV-cache slot -------------------------------------

@@ -1,5 +1,5 @@
 """Cached CUDA graphs against eager execution: every entry point that replays a graph (decode_host, decode, decode_batch_host, decode_batch,
-generate_batch) gives bit-identical logits, greedy ids and KV rows to the same model built with TCE_NO_GRAPH=1, across the first call of a
+generate, generate_batch) gives bit-identical logits, greedy ids and KV rows to the same model built with TCE_NO_GRAPH=1, across the first call of a
 key (eager run + capture), replays, a new request tensor, an option change, batch-size changes and slot growth."""
 import pytest
 import torch
@@ -137,6 +137,21 @@ def test_batched_graphs_match_eager(monkeypatch):
         return out, 5
 
     _assert_same(monkeypatch, script)
+
+
+@pytest.mark.parametrize("persistent", ["1", "0"])
+def test_generate_graphs_match_eager(monkeypatch, persistent):
+    def script(ctx, model):
+        out = [model.generate(11, 0, 20, seed=1, top_k=20)]  # first token eager + capture, then replays
+        out.append(model.generate(12, 20, 24, temp=0.0))  # the cached graph from the first call
+        ctx.set_option("use_pdl", 0)  # an option change makes the graph stale
+        out.append(model.generate(13, 44, 18, seed=3, top_k=40, top_p=0.9))
+        model.reserve_slots(3)  # a new slot table drops it
+        out.append(model.generate(14, 62, 17, seed=4))
+        out.append(model.generate(15, 79, 16, seed=5, temp=0.0))
+        return out, 1
+
+    _assert_same(monkeypatch, script, persistent)
 
 
 def test_generate_batch_graphs_match_eager(monkeypatch):

@@ -132,3 +132,52 @@ def test_generate_loop_matches_stepwise(ctx):
     assert greedy == chain
     for m in (model, model2, model3):
         m.close()
+
+
+@pytest.mark.parametrize("persistent", ["1", "0"])
+def test_generate_kv_rows(ctx, monkeypatch, persistent):
+    """After a budget stop, an eos_id stop and a max_ctx stop, slot 0 holds exactly rows pos0 .. pos0 + n_out - 1 new and every other row
+    is byte-identical; a call refused for a NULL history writes nothing."""
+    import ctypes as C
+
+    from tinychatengine_b200 import _lib
+    from tinychatengine_b200.llama import GEOMETRIES, LlamaModel
+
+    monkeypatch.setenv("TCE_PERSISTENT", persistent)
+    monkeypatch.setenv("TCE_DETERMINISTIC", "1")
+    g = GEOMETRIES["tiny-gqa"]
+    model = LlamaModel(ctx, g, max_ctx=128, seed=3)
+    gen = torch.Generator(device="cuda")
+    gen.manual_seed(5)
+    caches = [model.kv_cache(l, w) for l in range(g.num_layers) for w in (0, 1)]
+    for c in caches:
+        c.copy_((torch.randn(c.shape, device="cuda", generator=gen) * 0.5).to(torch.float16))
+    orig = [c.cpu().clone() for c in caches]
+
+    def run(pos0, n_predict, **kw):
+        for c, o in zip(caches, orig):
+            c.copy_(o.cuda())
+        out = model.generate(7, pos0, n_predict, **kw)
+        for c, o in zip(caches, orig):
+            a, b = o.clone(), c.cpu().clone()
+            assert not torch.equal(a[:, pos0:pos0 + len(out)], b[:, pos0:pos0 + len(out)])
+            a[:, pos0:pos0 + len(out)] = 0
+            b[:, pos0:pos0 + len(out)] = 0
+            assert torch.equal(a, b)
+        return out
+
+    ref = run(10, 30, seed=9, top_k=20)  # budget stop
+    assert len(ref) == 30
+    eos = ref[4]
+    assert run(10, 30, seed=9, top_k=20, eos_id=eos) == ref[:ref.index(eos) + 1]  # eos stop, with steps queued behind it
+    assert len(run(120, 30, seed=9, top_k=20)) == 8  # max_ctx stop
+    for c, o in zip(caches, orig):
+        c.copy_(o.cuda())
+    cfg = _lib.Sampling(40, 0.95, 0.8, 1.1, 0.0, 0.0, 64, 0)
+    out, n = (C.c_int * 8)(*[-7] * 8), C.c_int(-1)
+    assert ctx.L.tce_llama_generate(model.h, 7, 0, 8, C.byref(cfg), None, 2, -1, out, C.byref(n)) == -1  # n_history > 0, history NULL
+    torch.cuda.synchronize()
+    assert n.value == -1 and list(out) == [-7] * 8
+    for c, o in zip(caches, orig):
+        assert torch.equal(c.cpu(), o)
+    model.close()

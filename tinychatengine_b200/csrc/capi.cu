@@ -520,6 +520,7 @@ int tce_sample(tce_ctx *ctx, float *logits_dev, int n_vocab, const int *window_h
                int *token_host, int *cand_ids_host, float *cand_probs_host, int *cand_count_host) {
     if (!ctx || !logits_dev || !cfg || !token_host || n_vocab < 1 || n_window < 0 || (n_window > 0 && !window_host))
         return fail(TCE_ERR_INVALID, "tce_sample: bad argument");
+    if (!sampling_supported(cfg->temp, cfg->top_k, n_vocab)) return fail(TCE_ERR_UNSUPPORTED, "tce_sample: temp > 0 needs 1 <= top_k <= 1024");
     CK(cudaSetDevice(ctx->c.device), "cudaSetDevice");
     const bool want_cand = cand_ids_host && cand_probs_host && cand_count_host;
     const int kcap = 1024;
@@ -548,7 +549,7 @@ int tce_sample(tce_ctx *ctx, float *logits_dev, int n_vocab, const int *window_h
     int *head = scratch + 1;
     a.hist_head = n_window > 0 ? head : nullptr;
     if (n_window > 0) a.draw_index = draw_index - (unsigned long long)n_window;
-    if (e == cudaSuccess) e = launch_sample(&ctx->c, a, s);
+    if (e == cudaSuccess) e = launch_sample(a, s);
     int out[4] = {0, 0, 0, 0};
     if (e == cudaSuccess) e = cudaMemcpyAsync(out, scratch, sizeof(out), cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
@@ -557,7 +558,6 @@ int tce_sample(tce_ctx *ctx, float *logits_dev, int n_vocab, const int *window_h
         if (e == cudaSuccess) e = cudaMemcpy(cand_probs_host, cprob, (size_t)out[2] * sizeof(float), cudaMemcpyDeviceToHost);
     }
     cudaFree(scratch);
-    if (e == cudaErrorNotSupported) return fail(TCE_ERR_UNSUPPORTED, "tce_sample: temp > 0 needs 1 <= top_k <= 1024");
     if (e != cudaSuccess) return fail(TCE_ERR_CUDA, "tce_sample: %s", cudaGetErrorString(e));
     *token_host = out[0];
     if (want_cand) *cand_count_host = out[2];

@@ -119,10 +119,11 @@ struct SampleArgs {
 };
 // the sampler arguments of one chain: the fields of tce_sampling, draw index 0, no history, outputs or limits
 SampleArgs sample_args(const tce_sampling &sc, float *logits, int n_vocab);
-// temp > 0 over a vocabulary of more than 1024 ids needs 1 <= top_k <= 1024 (launch_sample returns cudaErrorNotSupported otherwise)
+// temp > 0 over a vocabulary of more than 1024 ids needs 1 <= top_k <= 1024
 bool sampling_supported(float temp, int top_k, int n_vocab);
-cudaError_t launch_sample(Ctx *ctx, const SampleArgs &a, cudaStream_t stream);
-// rows_dev = device SampleArgs[rows]: row b is sampled by block b (the generate loop of the batched step; host-checked arguments)
+// one row (tce_sample, the single-sequence generate loop); rows_dev = device SampleArgs[rows]: row b is sampled by block b (the batched
+// generate loop).  Host-checked arguments, including sampling_supported.
+cudaError_t launch_sample(const SampleArgs &a, cudaStream_t stream);
 cudaError_t launch_sample_rows(const SampleArgs *rows_dev, int rows, cudaStream_t stream);
 // acceptance of a speculative step (sampling.cu, the rule of tce_spec_accept): rows = 1 + drafts logits rows at pitch ld, verified in one
 // launch (a block per row)

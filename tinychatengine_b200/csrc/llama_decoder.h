@@ -1,8 +1,10 @@
 // llama_decoder.h -- host-side runner of the fused Llama decode step (one CUDA graph per token).
 #pragma once
 #include <functional>
+#include <map>
 #include <memory>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "../../include/tce_b200.h"
@@ -49,6 +51,26 @@ struct CachedGraph {
     }
 };
 
+// the request and read-back buffers of a decode step of up to `rows` rows
+struct StepIO {
+    int V = 0;
+    HostPtr<int> h_req;       // [rows][3] {token, position, slot} staged for the host entry points
+    DevPtr<int> req;          // [rows][3]
+    DevPtr<float> logits;     // [rows][V]
+    DevPtr<int> next;         // [rows] greedy arg-max
+    HostPtr<float> h_logits;  // [rows][V]
+    HostPtr<int> h_next;      // [rows]
+    cudaError_t alloc(int rows, int V);  // zeroed requests and logits
+    void stage(int slot, int pos0, int n, const int *tokens);  // h_req rows 0..n-1 = {tokens[i], pos0 + i, slot}
+    // what a host round trip copies back: nothing, the greedy ids, or the logits and then the ids
+    enum ReadBack { kNone, kIds, kLogitsIds };
+    static ReadBack wanted(const float *logits_host) { return logits_host ? kLogitsIds : kIds; }
+    // D2H of the first n rows' logits and / or greedy ids
+    cudaError_t read_back(int n, ReadBack r, cudaStream_t s);
+    // synchronise s, then copy the read-back out (either pointer may be null)
+    cudaError_t copy_out(int n, float *logits_host, int *next_host, cudaStream_t s) const;
+};
+
 class LlamaDecoder {
    public:
     static LlamaDecoder *create(Ctx *ctx, int attn_chunk, const tce_llama_config &cfg, const tce_llama_weights &w, std::string *err);
@@ -66,7 +88,7 @@ class LlamaDecoder {
     // epilogue (tce_llama_score_batch)
     cudaError_t score_batch(int n_seqs, const int *tokens_host, const int *lengths, const int *pos0s, const int *slots, const int *targets_host,
                             float *logprobs_host, int *greedy_host, float *greedy_logprobs_host, float *logits_dev, std::string *err);
-    const float *logits() const { return d_logits_.get(); }
+    const float *logits() const { return io1_.logits.get(); }
     void *kv_cache(int layer, int which) const { return kv_cache_slot(0, layer, which); }
     // batched decode: up to TCE_LLAMA_MAX_BATCH sequences per step, each in its own KV-cache slot (slot 0 = d_kv_)
     bool tensor_parallel() const { return tp_ > 1; }
@@ -121,23 +143,34 @@ class LlamaDecoder {
     cudaError_t prompt_logits(int n_seqs, const int *lengths, float *logits, int *next);
     // the final RMSNorm + lm_head GEMV over rows of x (pitch E) into rows of y (pitch V)
     W4GemvParams lm_head_gemv(const float *x, float *y) const;
+    // the decode steps: single = one sequence on slot 0 (the persistent kernel, or the batched step at batch 1), batch = the batched step,
+    // span = the batched step over consecutive tokens of one slot
+    enum class Step { single, batch, span };
+    // the buffers of a kind's step: io1_ for single, bs_->io for the others
+    StepIO &io(Step k) { return k == Step::single ? io1_ : bs_->io; }
+    // allocates what a kind's step needs (batch_alloc unless it runs on the persistent kernel); cudaErrorNotSupported (+ *err) where it
+    // does not run
+    cudaError_t step_ready(Step k, std::string *err);
+    // one step of `rows` requests at device req, logits and greedy ids into io(k)
+    cudaError_t enqueue(Step k, int rows, const int *req, cudaStream_t s, bool pdl);
     // one single-sequence step on device {token, position}: the persistent kernel, or the batched step at batch 1 on slot 0
     cudaError_t enqueue_step(const int *tokpos, cudaStream_t s, bool pdl);
     // runs body(stream, pdl) through the graph cached in g for `key`: replays it when it is current, otherwise runs body eagerly on the
     // context's stream and captures it for the next call (PDL edges first, plain edges if refused); graphs off: eager only
     cudaError_t run_graphed(CachedGraph &g, const void *key, const std::function<cudaError_t(cudaStream_t, bool)> &body);
+    // the first half of a host round trip: the `rows` requests staged in io(k).h_req through the host-entry graph {H2D, step, the D2H
+    // copies of r}; io(k).copy_out is the second half
+    cudaError_t run_host(Step k, int rows, StepIO::ReadBack r);
     cudaError_t build_persistent(std::string *err);
     // the batched step's buffers and parameters; cudaErrorNotSupported (+ *err) for a model the batched step does not cover
     cudaError_t batch_alloc(std::string *err);
     // raw kernel sequence of one batched step on req = device int[batch][3]; lm_head rows into logits[batch][V], greedy ids into next
     // span: the rows are consecutive tokens of one slot (launch_attn_span instead of the per-sequence attention)
     cudaError_t enqueue_batch(int batch, const int *req, float *logits, int *next, cudaStream_t s, bool pdl, bool span = false);
-    // one step of `rows` staged requests (bs_->h_req) through graph g, logits / greedy ids copied back
-    cudaError_t host_rows(CachedGraph &g, int rows, bool span, float *logits_host, int *next_tokens);
+    // the generate loop of `rows` requests on kind k (single: one request on slot 0), checked before anything is enqueued
+    cudaError_t generate_rows(Step k, int rows, const tce_gen_request *reqs, int *out_tokens_host, int out_stride, int *n_out, std::string *err);
     bool span_ok(int slot, int pos0, int n, const int *tokens) const;
     cudaError_t span_supported(std::string *err) const;  // cudaErrorNotSupported (+ *err) when no span split fits shared memory
-    void stage_span(int slot, int pos0, int n, const int *tokens);  // the n requests of a span into bs_->h_req
-    void drop_graphs();
 
     // tensor parallel state (the persistent kernel's hand-off buffers)
     int tp_ = 1;
@@ -157,10 +190,7 @@ class LlamaDecoder {
     tce_llama_weights w_{};
     // device state
     DevPtr<__half> d_kv_;           // [L][2][KVH][max_ctx][hd]
-    DevPtr<float> d_logits_;        // [V]
-    DevPtr<int> d_tokpos_;          // {token, pos, slot = 0}: staged for the host entry point, the request of the kernel-per-op step
-    DevPtr<int> d_next_;            // greedy arg-max
-    DevPtr<int> d_gen_;             // generate loop: [0] history head, [1] output count, [2] stop flag, then history ring [max_ctx], output list [max_ctx]
+    StepIO io1_;                    // the single-sequence step's request {token, pos, slot = 0}, logits and greedy id
     const float *d_cos_ = nullptr, *d_sin_ = nullptr;  // the caller's RoPE tables, or the halves of rope_
     DevPtr<float> rope_;            // [2][max_ctx][hd] cos | sin, when the caller gives none
     // prompt-processing activations, [cap] rows each (allocated on first use)
@@ -198,14 +228,11 @@ class LlamaDecoder {
         DevPtr<float> out;          // [3][n]
     } sc_;
     cudaError_t score_reserve(int n);
-    // pinned host staging for the end-to-end entry point
-    HostPtr<int> h_tokpos_;
-    HostPtr<float> h_logits_;
-    HostPtr<int> h_next_;
-    // graphs
+    // graphs: one per (entry, kind, rows, read-back).  The host entry replays run_host's work, the device entry a step on the
+    // caller's request pointer (its key), the loop entry a step and the row sampler.  All are dropped when the slot table changes.
+    enum Entry { kHost, kDevice, kLoop };
+    std::map<std::tuple<Entry, Step, int, StepIO::ReadBack>, CachedGraph> graphs_;
     cudaStream_t cap_stream_ = nullptr;
-    CachedGraph g_host_;            // H2D(tokpos) + step + argmax + D2H(logits,next)
-    CachedGraph g_dev_;             // step on the caller's {token, pos}
     // batched decode state (allocated on first use; also the kernel-per-op single-sequence step): the step's buffers hold
     // TCE_LLAMA_MAX_BATCH rows each
     std::vector<DevPtr<__half>> slot_kv_;  // KV-cache slots 1.. ([L][2][KVH][max_ctx][hd] each)
@@ -215,33 +242,27 @@ class LlamaDecoder {
         DevPtr<__half> qkv;           // [8][(H+2KVH)*hd]
         DevPtr<__half> attn;          // [8][H*hd]
         DevPtr<__half> act;           // [8][F]
-        DevPtr<float> logits;         // [8][V]
-        DevPtr<int> req;              // [8][3] {token, position, slot} staged for the host entry point
+        StepIO io;                    // 8 rows
         DevPtr<int> safe;             // [8][4] {token, position, slot, valid} after the device-side range check
-        DevPtr<int> next;             // [8] greedy arg-max
         DevPtr<float> attn_ws;        // attention split records of 8 sequences at this model's max_ctx
         size_t attn_ws_floats = 0;
         int span_chunk = 0;           // cached rows per CTA of the span attention (attn_span_chunk), 0: the span step is not supported
         DevPtr<unsigned> attn_counters;  // [8][KVH] split arrival counters
         size_t n_counters = 0;
-        HostPtr<int> h_req, h_next;
-        HostPtr<float> h_logits;
-        // batched generate loop: [8][4] control words {history head, output count, stop flag, unused}, then [8][max_ctx] history rings and
-        // [8][max_ctx] output lists; the sampler arguments of each row
-        DevPtr<int> gen;
-        DevPtr<SampleArgs> sample;
         // the step's parameters on these buffers: GEMV 4 * layer + {0: q|k|v, 1: o, 2: gate|up, 3: down} (M = 1), then the lm_head;
         // the attention of each layer (its slot table is read at launch)
         std::vector<W4GemvParams> gemv_ops;
         std::vector<AttnDecodeArgs> attn_ops;
     };
     std::unique_ptr<BatchState> bs_;  // non-null: every buffer of the batched step exists
-    // one graph per batch size: host entry (with / without the logits copy), device entry (for one request pointer), generate loop (one
-    // batched step on bs_->req + the row sampler).  Dropped with the single-sequence graphs when the slot table changes.
-    CachedGraph g_bhost_[2][TCE_LLAMA_MAX_BATCH + 1];
-    CachedGraph g_bdev_[TCE_LLAMA_MAX_BATCH + 1];
-    CachedGraph g_bgen_[TCE_LLAMA_MAX_BATCH + 1];
-    CachedGraph g_span_[2][TCE_LLAMA_MAX_BATCH + 1];  // span step per n, with / without the logits copy
+    // both generate loops (allocated whole on the first call of either, never reallocated: captured graphs hold these pointers): [8][4]
+    // control words {history head, output count, stop flag, unused}, then [8][max_ctx] history rings and [8][max_ctx] output lists; the
+    // sampler arguments of each row
+    struct LoopState {
+        DevPtr<int> words;
+        DevPtr<SampleArgs> sample;
+    };
+    std::unique_ptr<LoopState> loop_;
     // speculative loop: device {counter, step result, greedy ids, history ring [max_ctx]} and the pinned read-back of one step's result
     DevPtr<int> d_spec_;
     HostPtr<int> h_spec_;

@@ -335,6 +335,8 @@ TCE_DEVINL void sample_one(const SampleArgs &a, SampleShared &sh) {
     }
 }
 
+// one row with its arguments as a kernel parameter (tce_sample, the single-sequence generate loop): the chain reads them from the constant
+// bank, where sample_rows_kernel holds its row's in registers and runs the chain slower
 __global__ void __launch_bounds__(kSampleThreads, 1) sample_kernel(SampleArgs a) {
     __shared__ SampleShared sh;
     sample_one(a, sh);
@@ -408,6 +410,11 @@ cudaError_t launch_accept(const AcceptArgs &a, cudaStream_t stream) {
     return cudaGetLastError();
 }
 
+cudaError_t launch_sample(const SampleArgs &a, cudaStream_t stream) {
+    sample_kernel<<<1, kSampleThreads, 0, stream>>>(a);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_sample_rows(const SampleArgs *rows_dev, int rows, cudaStream_t stream) {
     if (!rows_dev || rows < 1) return cudaErrorInvalidValue;
     sample_rows_kernel<<<rows, kSampleThreads, 0, stream>>>(rows_dev);
@@ -431,13 +438,5 @@ SampleArgs sample_args(const tce_sampling &sc, float *logits, int n_vocab) {
 }
 
 bool sampling_supported(float temp, int top_k, int n_vocab) { return !(temp > 0.f && (top_k <= 0 || top_k > kMaxK) && n_vocab > kMaxK); }
-
-cudaError_t launch_sample(Ctx *ctx, const SampleArgs &a, cudaStream_t stream) {
-    if (!a.logits || a.n_vocab < 1) return cudaErrorInvalidValue;
-    if (!sampling_supported(a.temp, a.top_k, a.n_vocab)) return cudaErrorNotSupported;
-    (void)ctx;
-    sample_kernel<<<1, kSampleThreads, 0, stream>>>(a);
-    return cudaGetLastError();
-}
 
 }  // namespace tce
