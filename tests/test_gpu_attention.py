@@ -275,6 +275,32 @@ def test_decode_workspace_grows():
         c.close()
 
 
+@pytest.mark.parametrize("chunk", [64, 256])
+@pytest.mark.parametrize("H,KVH", [(32, 8), (8, 8)])
+def test_span_of_one_row_is_the_decode_call(H, KVH, chunk):
+    """tce_attn_span at n = 1 and tce_attn_decode on the same inputs give the same output and K / V cache bits: in one split, on the last row
+    of a split, on the first row of the next one, and over many splits."""
+    from tinychatengine_b200.runtime import Context
+
+    max_ctx = 4096
+    bits = lambda t: t.view(torch.int16)  # the unwritten cache rows are NaN
+    c = Context(0)
+    try:
+        c.set_option("attn_chunk", chunk)
+        for past in (0, 37, chunk - 1, chunk, 3000):
+            case = _decode_case(H, KVH, past, max_ctx, 7 * past + H)
+            qkv, kc, vc, cosb, sinb, _ = case
+            kc2, vc2 = kc.clone(), vc.clone()
+            dec = _decode(c, case, H, KVH, past, max_ctx)
+            out = torch.zeros((1, H * HD), dtype=torch.float16, device=qkv.device)
+            c.attn_span(qkv, kc2, vc2, cosb, sinb, out, 1.0 / np.sqrt(HD), 1, past, H, KVH, HD, max_ctx)
+            torch.cuda.synchronize()
+            assert torch.equal(bits(out[0].cpu()), bits(dec)), past
+            assert torch.equal(bits(kc2), bits(kc)) and torch.equal(bits(vc2), bits(vc)), past
+    finally:
+        c.close()
+
+
 @pytest.mark.parametrize("H,KVH,hd,max_ctx,chunk,status", [
     (8, 2, 64, 64, None, -2),      # head_dim 64: TCE_ERR_UNSUPPORTED
     (6, 4, 128, 64, None, -1),     # H % KVH != 0: TCE_ERR_INVALID

@@ -178,6 +178,32 @@ def _one_row(model, tok, pos, slot):
     return lg.numpy()[0].copy()
 
 
+def test_span_of_one_row_is_the_batched_step(monkeypatch):
+    """TCE_DETERMINISTIC=1, GQA 4:1, 256-row splits (the span runs the same split): the span step of one token and the batched step of one
+    sequence give the same logits and K / V cache bits, on slot 0 and another slot, in one split, on a split boundary and over many."""
+    ctx, model = _model("tiny-gqa", 1024, monkeypatch=monkeypatch, chunk=256)
+    g = model.geom
+    for slot in (0, 3):
+        for pos in (0, 255, 256, 1000):
+            _fill(model, 4, 10 * slot + pos)
+            before = _snap(model, 4)
+            tok = (31 * pos + 7 * slot + 1) % g.vocab_size
+            lg = torch.empty((1, g.vocab_size), dtype=torch.float32).pin_memory()
+            model.decode_span([tok], pos, slot, lg)
+            span_lg, span_kv = lg.numpy()[0].copy(), _snap(model, 4)
+            for s in range(4):
+                for l in range(g.num_layers):
+                    for w in (0, 1):
+                        model.kv_cache(l, w, s).copy_(before[s][l][w].cuda())
+            assert np.array_equal(span_lg, _one_row(model, tok, pos, slot)), (slot, pos)
+            after = _snap(model, 4)
+            for s in range(4):
+                for l in range(g.num_layers):
+                    for w in (0, 1):
+                        assert torch.equal(span_kv[s][l][w], after[s][l][w]), (slot, pos, s, l, w)
+    _close(model, ctx)
+
+
 def test_span_step_long_context(monkeypatch):
     """Contexts up to 4096 with the default 256-row splits (16 of them), GQA 4:1: the span rows against the oracle, also with the new rows
     across a split boundary (pos0 = 253, 510)."""

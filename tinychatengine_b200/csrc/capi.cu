@@ -334,16 +334,13 @@ static cudaError_t attn_ws_reserve(tce_ctx *ctx, size_t floats, size_t counters)
     return cudaSuccess;
 }
 
-int tce_attn_decode(tce_ctx *ctx, const void *qkv, void *k_cache, void *v_cache, const float *cosb, const float *sinb, const int *pos,
-                    void *out, float alpha, int num_heads, int num_kv_heads, int head_dim, int max_ctx) {
-    if (!ctx || !qkv || !k_cache || !v_cache || !cosb || !sinb || !pos || !out) return fail(TCE_ERR_INVALID, "tce_attn_decode: null pointer");
-    if (head_dim != 128) return fail(TCE_ERR_UNSUPPORTED, "tce_attn_decode: head_dim %d (only 128)", head_dim);
-    if (num_heads < 1 || num_kv_heads < 1 || num_heads % num_kv_heads || max_ctx < 1) return fail(TCE_ERR_INVALID, "tce_attn_decode: bad shape");
-    // one call takes at most 128 heads x 1024 splits of records and 1024 KV heads
-    const size_t floats = attn_decode_ws_floats(num_heads, max_ctx, ctx->attn_chunk);
-    if (floats > (size_t)128 * 1024 * (128 + 2) || num_kv_heads > 1024) return tce_fail_cuda(cudaErrorInvalidValue, "tce_attn_decode");
+// the decode attention over a caller's cache: n rows at position *pos (device) or pos0 (host), `chunk` rows per split, in the context's
+// workspace of `floats` split records
+static int attn_run(tce_ctx *ctx, const char *what, const void *qkv, void *k_cache, void *v_cache, const float *cosb, const float *sinb, const int *pos,
+                    int pos0, void *out, float alpha, int n, int num_heads, int num_kv_heads, int head_dim, int max_ctx, int chunk, size_t floats) {
     CK(cudaSetDevice(ctx->c.device), "cudaSetDevice");
-    CK(attn_ws_reserve(ctx, floats, num_kv_heads), "tce_attn_decode workspace");
+    const cudaError_t e = attn_ws_reserve(ctx, floats, num_kv_heads);
+    if (e != cudaSuccess) return fail(TCE_ERR_CUDA, "%s workspace: %s", what, cudaGetErrorString(e));
     AttnDecodeArgs a = {};
     a.qkv = (const __half *)qkv;
     a.k_cache = (__half *)k_cache;
@@ -351,40 +348,7 @@ int tce_attn_decode(tce_ctx *ctx, const void *qkv, void *k_cache, void *v_cache,
     a.cos = cosb;
     a.sin = sinb;
     a.pos = pos;
-    a.out = (__half *)out;
-    a.alpha = alpha;
-    a.num_heads = num_heads;
-    a.num_kv_heads = num_kv_heads;
-    a.head_dim = head_dim;
-    a.max_ctx = max_ctx;
-    a.chunk = ctx->attn_chunk;
-    a.ws = ctx->attn_ws;
-    a.ws_floats = ctx->attn_ws_floats;
-    a.counters = reinterpret_cast<unsigned *>(ctx->attn_ws + ctx->attn_ws_floats);
-    a.n_counters = ctx->attn_n_counters;
-    CK(launch_attn_decode(&ctx->c, a, 1, false), "tce_attn_decode");
-    return TCE_OK;
-}
-
-int tce_attn_span(tce_ctx *ctx, const void *qkv, void *k_cache, void *v_cache, const float *cosb, const float *sinb, void *out, float alpha, int n, int pos0,
-                  int num_heads, int num_kv_heads, int head_dim, int max_ctx) {
-    if (!ctx || !qkv || !k_cache || !v_cache || !cosb || !sinb || !out) return fail(TCE_ERR_INVALID, "tce_attn_span: null pointer");
-    if (head_dim != 128) return fail(TCE_ERR_UNSUPPORTED, "tce_attn_span: head_dim %d (only 128)", head_dim);
-    if (num_heads < 1 || num_kv_heads < 1 || num_heads % num_kv_heads || max_ctx < 1 || n < 1 || n > kMaxSpan || pos0 < 0 || pos0 > max_ctx - n)
-        return fail(TCE_ERR_INVALID, "tce_attn_span: bad shape n=%d pos0=%d max_ctx=%d", n, pos0, max_ctx);
-    const int chunk = attn_span_chunk(num_heads, num_kv_heads, ctx->attn_chunk, ctx->c.smem_optin);
-    if (!chunk) return fail(TCE_ERR_UNSUPPORTED, "tce_attn_span: no split fits shared memory at %d query heads per KV head", num_heads / num_kv_heads);
-    const size_t floats = (size_t)n * attn_decode_ws_floats(num_heads, max_ctx, chunk);
-    if (floats > (size_t)kMaxSpan * 128 * 1024 * (128 + 2) || num_kv_heads > 1024) return tce_fail_cuda(cudaErrorInvalidValue, "tce_attn_span");
-    CK(cudaSetDevice(ctx->c.device), "cudaSetDevice");
-    CK(attn_ws_reserve(ctx, floats, num_kv_heads), "tce_attn_span workspace");
-    AttnDecodeArgs a = {};
-    a.qkv = (const __half *)qkv;
-    a.k_cache = (__half *)k_cache;
-    a.v_cache = (__half *)v_cache;
-    a.cos = cosb;
-    a.sin = sinb;
-    a.span_pos0 = pos0;
+    a.pos0 = pos0;
     a.out = (__half *)out;
     a.alpha = alpha;
     a.num_heads = num_heads;
@@ -398,8 +362,34 @@ int tce_attn_span(tce_ctx *ctx, const void *qkv, void *k_cache, void *v_cache, c
     a.ws_floats = ctx->attn_ws_floats;
     a.counters = reinterpret_cast<unsigned *>(ctx->attn_ws + ctx->attn_ws_floats);
     a.n_counters = ctx->attn_n_counters;
-    CK(launch_attn_span(&ctx->c, a, n, false), "tce_attn_span");
+    CK(launch_attn_decode(&ctx->c, a, 1, n, false), what);
     return TCE_OK;
+}
+
+int tce_attn_decode(tce_ctx *ctx, const void *qkv, void *k_cache, void *v_cache, const float *cosb, const float *sinb, const int *pos,
+                    void *out, float alpha, int num_heads, int num_kv_heads, int head_dim, int max_ctx) {
+    if (!ctx || !qkv || !k_cache || !v_cache || !cosb || !sinb || !pos || !out) return fail(TCE_ERR_INVALID, "tce_attn_decode: null pointer");
+    if (head_dim != 128) return fail(TCE_ERR_UNSUPPORTED, "tce_attn_decode: head_dim %d (only 128)", head_dim);
+    if (num_heads < 1 || num_kv_heads < 1 || num_heads % num_kv_heads || max_ctx < 1) return fail(TCE_ERR_INVALID, "tce_attn_decode: bad shape");
+    // one call takes at most 128 heads x 1024 splits of records and 1024 KV heads
+    const size_t floats = attn_decode_ws_floats(num_heads, max_ctx, ctx->attn_chunk);
+    if (floats > (size_t)128 * 1024 * (128 + 2) || num_kv_heads > 1024) return tce_fail_cuda(cudaErrorInvalidValue, "tce_attn_decode");
+    return attn_run(ctx, "tce_attn_decode", qkv, k_cache, v_cache, cosb, sinb, pos, 0, out, alpha, 1, num_heads, num_kv_heads, head_dim, max_ctx,
+                    ctx->attn_chunk, floats);
+}
+
+int tce_attn_span(tce_ctx *ctx, const void *qkv, void *k_cache, void *v_cache, const float *cosb, const float *sinb, void *out, float alpha, int n, int pos0,
+                  int num_heads, int num_kv_heads, int head_dim, int max_ctx) {
+    if (!ctx || !qkv || !k_cache || !v_cache || !cosb || !sinb || !out) return fail(TCE_ERR_INVALID, "tce_attn_span: null pointer");
+    if (head_dim != 128) return fail(TCE_ERR_UNSUPPORTED, "tce_attn_span: head_dim %d (only 128)", head_dim);
+    if (num_heads < 1 || num_kv_heads < 1 || num_heads % num_kv_heads || max_ctx < 1 || n < 1 || n > kMaxSpan || pos0 < 0 || pos0 > max_ctx - n)
+        return fail(TCE_ERR_INVALID, "tce_attn_span: bad shape n=%d pos0=%d max_ctx=%d", n, pos0, max_ctx);
+    const int chunk = attn_span_chunk(num_heads, num_kv_heads, ctx->attn_chunk, ctx->c.smem_optin);
+    if (!chunk) return fail(TCE_ERR_UNSUPPORTED, "tce_attn_span: no split fits shared memory at %d query heads per KV head", num_heads / num_kv_heads);
+    const size_t floats = (size_t)n * attn_decode_ws_floats(num_heads, max_ctx, chunk);
+    if (floats > (size_t)kMaxSpan * 128 * 1024 * (128 + 2) || num_kv_heads > 1024) return tce_fail_cuda(cudaErrorInvalidValue, "tce_attn_span");
+    return attn_run(ctx, "tce_attn_span", qkv, k_cache, v_cache, cosb, sinb, nullptr, pos0, out, alpha, n, num_heads, num_kv_heads, head_dim, max_ctx,
+                    chunk, floats);
 }
 
 int tce_attn_prefill(tce_ctx *ctx, void *qkv, void *k_cache, void *v_cache, const float *cosb, const float *sinb, void *out, float alpha, int n, int pos0,

@@ -6,45 +6,43 @@ struct tce_sampling;  // include/tce_b200.h
 
 namespace tce {
 
-// Decode attention (attention.cu) of `batch` sequences: sequence b is grid.z = b, with its own q|k|v and output rows, KV cache and position,
-// and its own split records and counters in the workspace.
+// Decode attention (attention.cu) of `seqs` sequences of n consecutive rows each: sequence s is grid.z = s and owns rows s * n .. s * n + n - 1
+// of qkv / out, and row s * n + i is its position pos0_s + i.  The kernel rotates and appends the n new K / V rows of each sequence, then runs
+// causal attention: row i sees cache rows 0..pos0_s + i.  Every row has its own split records and every sequence its own split counters in
+// the workspace.  n = 1 is the per-token step of `seqs` sequences; seqs = 1, n > 1 is the span step of one sequence.
+constexpr int kMaxSpan = 8;
 struct AttnDecodeArgs {
-    const __half *qkv;   // [batch][qkv_stride]: the (H + 2*KVH) * head_dim projections of the current token (q | k | v), pre-RoPE
-    __half *out;         // [batch][out_stride]: H * head_dim
-    int qkv_stride, out_stride;  // elements between the rows of consecutive sequences
+    const __half *qkv;   // [seqs * n][qkv_stride]: the (H + 2*KVH) * head_dim projections of each row (q | k | v), pre-RoPE
+    __half *out;         // [seqs * n][out_stride]: H * head_dim
+    int qkv_stride, out_stride;  // elements between consecutive rows
     const float *cos;    // [max_ctx][head_dim]  (reference rotary_emb/cos_cached layout)
     const float *sin;    // [max_ctx][head_dim]
     float alpha;         // qk_bmm alpha (1/sqrt(head_dim))
     int num_heads, num_kv_heads, head_dim, max_ctx;
     int chunk;           // cached positions per CTA (<= 0: the default)
     int nsplit_max;      // filled by the launcher
-    float *ws;           // split records: batch * attn_decode_ws_floats(...) are used
+    float *ws;           // split records: seqs * n * attn_decode_ws_floats(...) are used
     size_t ws_floats;    // capacity of ws
-    unsigned *counters;  // zero-initialised split arrival counters (the last split re-arms them): batch * num_kv_heads are used
+    unsigned *counters;  // zero-initialised split arrival counters (the last split re-arms them): seqs * num_kv_heads are used
     size_t n_counters;   // capacity of counters
-    // with a request table (the batched step): each sequence's position and slot
-    const int *req;          // device int[batch][4] {token, position, slot, valid} (launch_embedding_batch), 16-byte aligned; valid = 0: the CTA writes nothing
+    // with a request table (the batched and span steps): row s * n gives sequence s's slot and first position; the other rows of a span
+    // name the same slot at consecutive positions (host-checked)
+    const int *req;          // device int[seqs * n][4] {token, position, slot, valid} (launch_embedding_batch), 16-byte aligned; valid = 0: the CTA writes nothing
     __half *const *slots;    // device table of slot bases, each [L][2][KVH][max_ctx][head_dim]
     long long k_off, v_off;  // elements from a slot's base to this layer's K / V slab
-    // without one (req == nullptr, batch 1): the cache and position of the one sequence
+    // without one (req == nullptr, seqs 1): the cache and first position of the one sequence
     __half *k_cache;     // [KVH][max_ctx][head_dim]
     __half *v_cache;     // [KVH][max_ctx][head_dim]
-    const int *pos;      // device scalar: index of the token being decoded (= number of cached tokens)
-    int span_pos0;       // span attention without a request table: the position of row 0
+    const int *pos;      // device scalar: the position of row 0 (= number of cached tokens); nullptr: pos0
+    int pos0;            // host value of the position of row 0 when pos is nullptr
 };
-// returns cudaErrorNotSupported for a head_dim or a query-heads-per-KV-head ratio the kernel does not cover, cudaErrorInvalidValue for a
-// workspace too small for the batch
-cudaError_t launch_attn_decode(Ctx *ctx, const AttnDecodeArgs &a, int batch, bool pdl);
-// floats of split workspace the kernel needs per sequence
+// returns cudaErrorNotSupported for a head_dim or a query-heads-per-KV-head ratio the kernel does not cover, cudaErrorInvalidValue for n outside
+// 1..kMaxSpan or a workspace too small, cudaErrorInvalidConfiguration when the CTA of the chunk does not fit shared memory
+cudaError_t launch_attn_decode(Ctx *ctx, const AttnDecodeArgs &a, int seqs, int n, bool pdl);
+// floats of split workspace the kernel needs per row
 size_t attn_decode_ws_floats(int num_heads, int max_ctx, int chunk);
-// Span attention (attention.cu): rows 0..n-1 of qkv / out are tokens at positions pos0..pos0+n-1 of ONE sequence, given by the request table
-// (a.req rows 0..n-1 {token, pos0 + i, slot, valid}, host-checked: one slot, consecutive positions) or, without one, by k_cache / v_cache
-// and span_pos0.  Rotates and appends the n new K / V rows, then causal multi-query attention: row i sees cache rows 0..pos0+i.  Uses
-// n * attn_decode_ws_floats(H, max_ctx, chunk) floats of split records and KVH counters; a.chunk must be at most attn_span_chunk(...).
-constexpr int kMaxSpan = 8;
-cudaError_t launch_attn_span(Ctx *ctx, const AttnDecodeArgs &a, int n, bool pdl);
-// the largest multiple of 16 rows <= chunk (<= 0: the default) whose span CTA, at n = kMaxSpan, fits smem_optin bytes of shared memory;
-// 0 when none does.  At 8 query heads per KV head the 256-row default does not fit an H100's 227 KiB: the span runs 224-row splits.
+// the largest multiple of 16 rows <= chunk (<= 0: the default) whose CTA, at n = kMaxSpan, fits smem_optin bytes of shared memory; 0 when
+// none does.  At 8 query heads per KV head the 256-row default does not fit an H100's 227 KiB: the span runs 224-row splits.
 int attn_span_chunk(int num_heads, int num_kv_heads, int chunk, int smem_optin);
 
 // prompt processing (sqlen = n > 1): RoPE + KV append for rows pos0..pos0+n-1, causal attention over the cache.  Up to

@@ -832,7 +832,7 @@ cudaError_t LlamaDecoder::enqueue_batch(int batch, const int *req, float *logits
         AttnDecodeArgs a = st.attn_ops[l];
         a.slots = st.slot_table.get();
         if (span) a.chunk = st.span_chunk;
-        DCK(span ? launch_attn_span(c, a, batch, pdl) : launch_attn_decode(c, a, batch, pdl));
+        DCK(launch_attn_decode(c, a, span ? 1 : batch, span ? batch : 1, pdl));
         for (int i = 1; i < 4; i++) DCK(gemv(st.gemv_ops[4 * l + i]));
     }
     W4GemvParams lm = st.gemv_ops.back();

@@ -165,7 +165,7 @@ class LlamaDecoder {
     // the batched step's buffers and parameters; cudaErrorNotSupported (+ *err) for a model the batched step does not cover
     cudaError_t batch_alloc(std::string *err);
     // raw kernel sequence of one batched step on req = device int[batch][3]; lm_head rows into logits[batch][V], greedy ids into next
-    // span: the rows are consecutive tokens of one slot (launch_attn_span instead of the per-sequence attention)
+    // span: the rows are consecutive tokens of one slot (the attention runs them as one sequence of `batch` rows, at the span chunk)
     cudaError_t enqueue_batch(int batch, const int *req, float *logits, int *next, cudaStream_t s, bool pdl, bool span = false);
     // the generate loop of `rows` requests on kind k (single: one request on slot 0), checked before anything is enqueued
     cudaError_t generate_rows(Step k, int rows, const tce_gen_request *reqs, int *out_tokens_host, int out_stride, int *n_out, std::string *err);
