@@ -105,3 +105,49 @@ def test_prompt_pass_matches_llama_forward(geom):
     for l in range(nl):
         assert torch.equal(Kb[l][0], K1[l][0]) and torch.equal(Kb[l][1], K2[l][0])
         assert torch.equal(Vb[l][0], V1[l][0]) and torch.equal(Vb[l][1], V2[l][0])
+
+
+@pytest.mark.parametrize("geom", ["tiny-mha", "tiny-gqa"])
+def test_decode_step_matches_oracle_decode_step(geom):
+    """decode_step with the RMSNorm outputs rounded to fp16 and the scaled query unrounded (round_norm=True, round_q=False) against
+    helpers.oracle_decode_step, the composition tests/test_gpu_llama.py checks the decode steps with: the first step (no cached rows),
+    then steps after 30 random fp16 rows, each over the rows the oracle returned (fp16 K rows, fp16 V rows).  The logits, the appended K
+    and V rows; and, with the kernels' rounding points (the defaults), the same step differs from the oracle's by about fp16 rounding."""
+    from types import SimpleNamespace
+
+    from helpers import oracle_decode_step
+    from tinychatengine_b200.llama import GEOMETRIES, make_random_weights
+
+    g = GEOMETRIES[geom]
+    W = make_random_weights(g, torch.device("cpu"), seed=9, random_zeros=True)
+    model = SimpleNamespace(geom=g, max_ctx=64, embed=W["embed"], final_norm=W["final_norm"], tensors=[W["lm_head"]],
+                            layer_tensors=lambda l: W["layers"][l])
+    cosb, sinb = capi.rope_tables(64, g.head_dim, g.rope_theta)
+    rng = np.random.default_rng(11)
+    nl, KVH = g.num_layers, g.num_kv_heads
+    worst = {"logits": 0.0, "K": 0.0, "V": 0.0, "logits (kernel points)": 0.0}
+    for start in (None, 30):
+        if start is None:
+            pk, pv, steps = [None] * nl, [None] * nl, [(17, 0)]
+        else:
+            pk = [(rng.standard_normal((KVH, start, HD)) * 0.7).astype(np.float16).astype(np.float32) for _ in range(nl)]
+            pv = [rng.standard_normal((KVH, start, HD)).astype(np.float16).astype(np.float32) for _ in range(nl)]
+            steps = [(int(t), start + i) for i, t in enumerate(rng.integers(0, g.vocab_size, 3))]
+        for tok, pos in steps:
+            past = [(torch.from_numpy(pk[l]), torch.from_numpy(pv[l])) for l in range(nl)] if pos else None
+            want, fk, fv = oracle_decode_step(model, tok, pos, pk, pv)
+            got, K, V = wide_ref.decode_step(W, g, tok, pos, past, cosb, sinb, round_norm=True, round_q=False)
+            kern, _, _ = wide_ref.decode_step(W, g, tok, pos, past, cosb, sinb)
+            worst["logits"] = max(worst["logits"], wide_ref.row_rel_err(got, torch.from_numpy(want)).item())
+            worst["logits (kernel points)"] = max(worst["logits (kernel points)"], wide_ref.row_rel_err(kern, torch.from_numpy(want)).item())
+            for l in range(nl):
+                worst["K"] = max(worst["K"], wide_ref.row_rel_err(K[l], torch.from_numpy(fk[l][:, pos])).max().item())
+                worst["V"] = max(worst["V"], wide_ref.row_rel_err(V[l], torch.from_numpy(fv[l][:, pos])).max().item())
+            pk, pv = [a.astype(np.float16).astype(np.float32) for a in fk], [a.astype(np.float16).astype(np.float32) for a in fv]
+    print(f"[wide_ref decode step {geom}] worst row rel err: " + ", ".join(f"{k} {v:.2e}" for k, v in worst.items()))
+    # as in the prompt-pass pin: fp32 against float64 arithmetic between the same fp16 rounding points moves a few q|k|v and SiLU*up
+    # elements by one fp16 ulp (~1e-3 of a row's max).  Measured at most 5.9e-4 (logits), 9.2e-4 (K) and 9.0e-4 (V, one ulp)
+    assert worst["logits"] <= 2e-3 and worst["K"] <= 2e-3 and worst["V"] <= 2e-3, worst
+    # the kernels' points drop the fp16 rounding of the RMSNorm outputs and round q * alpha: a step apart from the oracle's by that
+    # rounding only (measured 1.2e-3), far inside the 1e-2 the decode tests allow against it
+    assert worst["logits (kernel points)"] <= 5e-3, worst

@@ -1,11 +1,13 @@
-"""A float64 restatement of the W4A16 prompt pass in torch -- TEST INFRASTRUCTURE ONLY.
+"""A float64 restatement of the W4A16 prompt pass and decode step in torch -- TEST INFRASTRUCTURE ONLY.
 
 The scalar C oracle (oracle/tce_oracle.c) is far too slow at the widths the benchmark times (one Llama-2-13B gate|up GEMM at M = 2048 is
 about 145 G multiply-adds), so the kernels are checked there against this module, which runs on any torch device: on the CPU it is pinned
-against the oracle's composition (tests/test_wide_ref.py), on the GPU it is the reference of tests/test_gpu_wide.py.
+against the oracle's composition (tests/test_wide_ref.py), on the GPU it is the reference of tests/test_gpu_wide.py and
+tests/test_gpu_decode_wide.py.
 
 Every product of the projections is exact: fp16 x fp16 products are exact in float64, and a float64 sum of a few thousand of them is
-the exact sum to ~1e-16 relative.  The only roundings are the fp16 ones the prompt pass itself makes, at the same points (``prompt_pass``).
+the exact sum to ~1e-16 relative.  The only roundings are the fp16 ones the prompt pass and the decode step themselves make, at the same
+points (``prompt_pass``, ``decode_step``).
 """
 from __future__ import annotations
 
@@ -28,9 +30,11 @@ def ulp_f16(a: torch.Tensor) -> torch.Tensor:
     return torch.exp2(e - 10)
 
 
-def expand_w4(w: torch.Tensor, zeros: torch.Tensor, scales: torch.Tensor, group: int = GROUP) -> torch.Tensor:
+def expand_w4(w: torch.Tensor, zeros: torch.Tensor, scales: torch.Tensor, group: int = GROUP, exact: bool = False) -> torch.Tensor:
     """fp16 [OC, IC] = fp16(float(q - z) * float(s)) of QM_CUDA tensors (w int32 [OC, IC/8], zeros int32 [OC, zw], scales fp16 [OC, zw*8]):
-    what w4_expand_kernel writes.  Weight 8c + i is nibble i of word c; the product is exact in fp32, so there is one rounding."""
+    what w4_expand_kernel writes.  Weight 8c + i is nibble i of word c; the product is exact in fp32, so there is one rounding.
+    exact=True: the float64 products (q - z) * s without that rounding -- the weights of the W4A16 GEMVs, which multiply the integer
+    dot products by the scales."""
     OC, wpr = w.shape
     IC = wpr * 8
     ng = IC // group
@@ -39,12 +43,12 @@ def expand_w4(w: torch.Tensor, zeros: torch.Tensor, scales: torch.Tensor, group:
     z = ((zeros.to(torch.int64).unsqueeze(-1) >> sh) & 0xF).reshape(OC, -1)[:, :ng]
     s = scales[:, :ng].float()
     d = (q.reshape(OC, ng, group) - z.unsqueeze(-1)).float() * s.unsqueeze(-1)
-    return d.half().reshape(OC, IC)
+    return d.double().reshape(OC, IC) if exact else d.half().reshape(OC, IC)
 
 
-def w16_linear(x16: torch.Tensor, t) -> torch.Tensor:
-    """float64 [M, OC] = x16 . expand_w4(t)^T, exact (x16: fp16 values in any float dtype).  The weights are expanded a slice of rows at a
-    time, and each slice's float64 copy is freed before the next."""
+def w16_linear(x16: torch.Tensor, t, exact: bool = False) -> torch.Tensor:
+    """float64 [M, OC] = x16 . expand_w4(t, exact=exact)^T, exact (x16: fp16 values in any float dtype).  The weights are expanded a slice
+    of rows at a time, and each slice's float64 copy is freed before the next."""
     w, z, s = t
     x = x16.double()
     OC, IC = w.shape[0], w.shape[1] * 8
@@ -52,7 +56,7 @@ def w16_linear(x16: torch.Tensor, t) -> torch.Tensor:
     out = torch.empty((x.shape[0], OC), dtype=torch.float64, device=x.device)
     for r0 in range(0, OC, step):
         r1 = min(OC, r0 + step)
-        wd = expand_w4(w[r0:r1], z[r0:r1], s[r0:r1]).double()
+        wd = expand_w4(w[r0:r1], z[r0:r1], s[r0:r1], exact=exact).double()
         out[:, r0:r1] = x @ wd.T
         del wd
     return out
@@ -107,7 +111,7 @@ def prompt_pass(W, geom, prompts, pos0s, past, cos, sin, *, round_qk: bool = Tru
     (EpiHalf), the rotated q and k and the V rows (rope_kv_append_kernel), the attention output, and SiLU(gate) * up, computed from the
     unrounded gate and up (EpiSiluMul).  The o_proj and down_proj products are added UNROUNDED into the residual (EpiAddF32), which stays
     float64 here (fp32 on the device), and the logits are the product of the fp16 final-norm output with the fp16-expanded lm_head.
-    These are not the decode step's rounding points: there the GEMV output is fp16 before the residual add (helpers.oracle_decode_step).
+    These are not the decode step's rounding points (``decode_step``).
     round_qk=False keeps the rotated q and k unrounded, as oracle.llama_ref.llama_forward does."""
     g = geom
     H, KVH, hd = g.num_heads, g.num_kv_heads, g.head_dim
@@ -147,6 +151,81 @@ def prompt_pass(W, geom, prompts, pos0s, past, cos, sin, *, round_qk: bool = Tru
         del xn, q, k, v, att, gate, up
     xn = f16(rmsnorm(x, W["final_norm"], g.rms_eps))
     return w16_linear(xn, W["lm_head"]).float(), K, V
+
+
+def decode_qkv(qkv16: torch.Tensor, H: int, KVH: int, cos_row, sin_row, alpha: float, *, round_q: bool = True):
+    """The token's q|k|v words (fp16 values, [(H + 2 KVH) * hd]) -> (q * alpha after RoPE [H, hd], fp16 when round_q; the rotated key
+    rounded to fp16 [KVH, hd], as the cache holds it; v [KVH, hd]), all float64.  cos_row / sin_row: the position's table rows [hd]."""
+    hd = cos_row.shape[-1]
+    x = qkv16.double().reshape(H + 2 * KVH, hd)
+    c, s = torch.as_tensor(cos_row, device=x.device)[None], torch.as_tensor(sin_row, device=x.device)[None]
+    q = rope(x[None, :H], c, s)[0] * alpha
+    k = f16(rope(x[None, H:H + KVH], c, s)[0])
+    return (f16(q) if round_q else q), k, x[H + KVH:]
+
+
+def decode_attention(qa: torch.Tensor, K: torch.Tensor, V: torch.Tensor):
+    """softmax(qa K^T) V of one token over every row of K / V [KVH, T, hd] (the cached rows and the token's own, fp16 values), qa [H, hd]
+    the scaled query; query head h reads KV head h // (H / KVH).  Returns (out float64 [H, hd], p [H, T] = exp(s - max s), L [H] = sum p)."""
+    H, KVH = qa.shape[0], K.shape[0]
+    rep = H // KVH
+    Kh = K.double().repeat_interleave(rep, dim=0)  # [H, T, hd]
+    S = torch.einsum("hd,htd->ht", qa.double(), Kh)
+    p = torch.exp(S - S.amax(-1, keepdim=True))
+    L = p.sum(-1)
+    out = torch.einsum("ht,htd->hd", p, V.double().repeat_interleave(rep, dim=0)) / L[:, None]
+    return out, p, L
+
+
+def silu_mul(gate: torch.Tensor, up: torch.Tensor) -> torch.Tensor:
+    return gate / (1.0 + torch.exp(-gate)) * up
+
+
+def decode_step(W, geom, token: int, pos: int, past, cos, sin, *, round_norm: bool = False, round_q: bool = True):
+    """One decode step of a W4A16 Llama after `pos` cached rows: past[l] = (K, V) fp16 values [KVH, pos, hd] of layer l (None when
+    pos = 0).  W: the weight dict of llama.make_random_weights; cos / sin: the fp32 tables of oracle.capi.rope_tables.  Returns (logits
+    float64 [vocab], K, V) with K[l] / V[l] = float64 [KVH, hd], the row layer l appends.
+
+    The projections take the exact products (q - z) * s as their weights (expand_w4(exact=True)), as the W4A16 GEMVs of both steps
+    do: the prompt pass's fp16 expansion is not theirs.  Rounded where both decode steps -- the persistent kernel (decode_persistent.cu) and the kernel-per-op step (w4a16_gemv.cu +
+    attention.cu) -- hold fp16, which are the same points in both:
+      * q|k|v: the GEMV output is fp16 (PE_HALF_LL / EPI_STORE_HALF);
+      * RoPE runs in fp32 on those words; q * alpha is rounded to fp16 for the tensor-core product, the rotated key to fp16 (the
+        cache row), v is the GEMV's fp16 word;
+      * the attention output is fp16;
+      * SiLU(gate) * up is formed from the unrounded gate and up and rounded to fp16 (PE_SILU_LL / EPI_SILU_MUL_HALF).
+    NOT rounded: the RMSNorm outputs (both GEMVs take x * gamma as 32-bit block fixed point, exact to ~2^-24 of the group maximum, and
+    scale the product by 1 / rms), the o_proj and down_proj outputs (fp32, added to the fp32 residual in the order o, then down:
+    PE_DELTA_LL / EPI_ADD_F32), the softmax weights (the kernels round P to fp16 against a running per-block / per-chunk maximum
+    while the denominator sums the fp32 weights: below what a per-element reference can restate, so the tests bound it instead)
+    and the logits (fp32).
+    round_norm=True rounds the RMSNorm outputs to fp16 and round_q=False keeps the scaled query unrounded: the composition of
+    helpers.oracle_decode_step (oracle/llama_ref.py::llama_forward with the W4A16 GEMV oracle), which tests/test_wide_ref.py pins."""
+    g = geom
+    H, KVH = g.num_heads, g.num_kv_heads
+    dev = W["embed"].device
+    alpha = 1.0 / math.sqrt(g.head_dim)
+    cos_r, sin_r = torch.as_tensor(cos[pos], device=dev), torch.as_tensor(sin[pos], device=dev)
+    norm = (lambda t: f16(t)) if round_norm else (lambda t: t)
+    x = W["embed"][token].double()[None]  # residual stream [1, E]
+    Ks, Vs = [], []
+    for l, L in enumerate(W["layers"]):
+        xn = norm(rmsnorm(x, L["input_norm"], g.rms_eps))
+        qkv = f16(torch.cat([w16_linear(xn, L[n], exact=True) for n in ("q", "k", "v")], dim=1))[0]
+        qa, k, v = decode_qkv(qkv, H, KVH, cos_r, sin_r, alpha, round_q=round_q)
+        K, V = k[:, None], v[:, None]
+        if past is not None and past[l] is not None:
+            K = torch.cat([past[l][0].double(), K], dim=1)
+            V = torch.cat([past[l][1].double(), V], dim=1)
+        att, _, _ = decode_attention(qa, K, V)
+        Ks.append(k)
+        Vs.append(v)
+        x = x + w16_linear(f16(att.reshape(1, -1)), L["o"], exact=True)
+        xn = norm(rmsnorm(x, L["post_norm"], g.rms_eps))
+        gate, up = w16_linear(xn, L["gate"], exact=True), w16_linear(xn, L["up"], exact=True)
+        x = x + w16_linear(f16(silu_mul(gate, up)), L["down"], exact=True)
+    xn = norm(rmsnorm(x, W["final_norm"], g.rms_eps))
+    return w16_linear(xn, W["lm_head"], exact=True)[0], Ks, Vs
 
 
 def row_rel_err(got: torch.Tensor, ref: torch.Tensor) -> torch.Tensor:

@@ -119,6 +119,8 @@ class LlamaDecoder {
             case 2: return bs_ ? bs_->attn.get() : nullptr;
             case 3: return bs_ ? bs_->act.get() : nullptr;
             case 4: return pargs_.dbg;  // persistent-kernel phase timestamps (TCE_PK_DEBUG=1), [#CTAs][5 * layers + 1][4] u64 ns
+            case 5: return pargs_.qkv_ll;  // persistent-kernel hand-off words {payload, tag} (null until it exists): q|k|v, attention
+                                           // output, SiLU*up, split partials, o_proj / down_proj outputs, laid out as build_persistent cuts them
             default: return nullptr;
         }
     }

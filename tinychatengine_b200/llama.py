@@ -532,13 +532,53 @@ class LlamaModel:
         return _tensor_from_ptr(ptr, (self.geom.num_kv_heads, self.max_ctx, self.geom.head_dim), torch.float16, self.ctx.device)
 
     def debug_buffer(self, which: int) -> torch.Tensor:
+        """0..3: row 0 of the kernel-per-op step's residual, q|k|v, attention output and SiLU*up; 5: the persistent kernel's hand-off
+        words as int32 [n, 2] {payload, tag} (cut into its vectors by handoff_views)."""
         g = self.geom
-        shape, dt = {0: ((g.embed_dim,), torch.float32), 1: (((g.num_heads + 2 * g.num_kv_heads) * g.head_dim,), torch.float16),
-                     2: ((g.num_heads * g.head_dim,), torch.float16), 3: ((g.hidden_dim,), torch.float16)}[which]
+        if which == 5:
+            shape, dt = (sum(self._handoff_words().values()), 2), torch.int32
+        else:
+            shape, dt = {0: ((g.embed_dim,), torch.float32), 1: (((g.num_heads + 2 * g.num_kv_heads) * g.head_dim,), torch.float16),
+                         2: ((g.num_heads * g.head_dim,), torch.float16), 3: ((g.hidden_dim,), torch.float16)}[which]
         ptr = self.ctx.L.tce_llama_debug_buffer(self.h, which)
         if not ptr:
-            raise _lib.TceError(f"debug buffer {which}: the kernel-per-op step has not run on this model")
+            raise _lib.TceError(f"debug buffer {which}: " + ("this model has no persistent kernel" if which == 5 else
+                                                              "the kernel-per-op step has not run on this model"))
         return _tensor_from_ptr(ptr, shape, dt, self.ctx.device)
+
+    def attn_nsplit_max(self) -> int:
+        """Split records per head of the persistent kernel's attention (pk::attn_nsplit_max): #CTAs / KVH, at most one per 64-row chunk."""
+        return min(max(1, self.ctx.num_sms // self.geom.num_kv_heads), -(-self.max_ctx // 64))
+
+    def _handoff_words(self) -> dict:
+        """Words of each hand-off vector, in the order LlamaDecoder::build_persistent lays them out (tensor parallel: the o_proj /
+        down_proj words live in the peer-visible buffer instead)."""
+        g = self.geom
+        n = {"qkv": (g.num_heads + 2 * g.num_kv_heads) * 64, "attn": g.num_heads * 64, "act": g.hidden_dim // 2,
+             "part": g.num_heads * self.attn_nsplit_max() * 130}
+        if self.tp_size == 1:
+            n.update(delta0=g.embed_dim, delta1=g.embed_dim)
+        return n
+
+    def handoff_views(self) -> dict:
+        """The persistent kernel's hand-off words after a step (they hold the last layer's vectors): name -> (payload, tag).  qkv, attn,
+        act: fp16 [2 * words] (two halfs per word); part: fp32 [H, nsplit_max, 130] (per split: output[128], max, sum); delta0 / delta1:
+        the o_proj / down_proj outputs, fp32 [E].  tag: int64 per word (same shape as the words: [H, nsplit_max, 130] for part)."""
+        words = self.debug_buffer(5)
+        out, o = {}, 0
+        for name, n in self._handoff_words().items():
+            w = words[o:o + n]
+            o += n
+            pay = w[:, 0].contiguous()
+            tag = w[:, 1].to(torch.int64) & 0xFFFFFFFF
+            if name in ("qkv", "attn", "act"):
+                out[name] = (pay.view(torch.float16), tag)
+            elif name == "part":
+                shape = (self.geom.num_heads, self.attn_nsplit_max(), 130)
+                out[name] = (pay.view(torch.float32).reshape(shape), tag.reshape(shape))
+            else:
+                out[name] = (pay.view(torch.float32), tag)
+        return out
 
     def close(self):
         if self.h:
