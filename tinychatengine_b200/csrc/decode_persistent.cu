@@ -13,7 +13,8 @@
 //   consumers (16 warps)  per phase: spin on the flag-carrying words of their input vector, quantise it (fused RMSNorm, four int8 planes
 //        per 128-group), run the integer-MMA GEMV over this CTA's tiles (two 128-k groups per warp and stage), or run flash-decoding
 //        attention straight out of the ring stages (mma.sync m16n8k16, ldmatrix on the swizzled K/V rows).
-//   epilogue (1 warp)  reduces the 16 consumer partials of every tile and publishes the results as {value, phase tag} words.
+//   epilogue (1 warp)  reduces the 16 consumer partials of every tile and publishes the results as {value, phase tag} words.  In pair mode
+//        (clusters of two CTAs that split K) one CTA per tile first adds its partner's row sums.
 //
 // There is NO grid barrier between phases.  Every vector that crosses CTAs (q|k|v, attention partials and outputs, SiLU*mul
 // activations, the o_proj / down_proj outputs) is an array of 8-byte words {payload, tag} written with one 8-byte store and read with
@@ -147,12 +148,6 @@ TCE_DEVINL void mbar_wait_u32(uint32_t bar, uint32_t parity) {
 }
 TCE_DEVINL void mbar_arrive_u32(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
 
-TCE_DEVINL int lds_volatile_i32(const int *p) {
-    int v;
-    asm volatile("ld.volatile.shared.s32 %0, [%1];" : "=r"(v) : "r"(smem_u32(p)) : "memory");
-    return v;
-}
-
 TCE_DEVINL void stamp(const Args &a, int cta, int nphase, int p, int k) {  // one thread
     if (a.dbg) {
         unsigned long long t;
@@ -169,20 +164,26 @@ TCE_DEVINL unsigned long long argmax_key(float v, int idx) {
 
 struct PSmem {
     uint8_t *ring;      // [nst][kStageBytes], 1024-B aligned
-    uint8_t *xs;        // activation planes (4 * IC bytes) | attention scratch
-    float *resid;       // [E] this CTA's copy of the fp32 residual stream
+    uint8_t *xs;        // activation planes (4 bytes per input channel of the CTA's K range) | attention scratch
+    float *resid;       // this CTA's copy of the fp32 residual stream: all E channels, or in pair mode the channels of its K range
     float *gx;          // [max_ng] group steps
     int *gsum;          // [max_ng][2] group sums
     float *red;         // [kRedBufs][kCW][16] tile partials
-    float *rms;         // [kCW]
+    float *rms;         // [2][kCW] partial sums of squares (rank, warp)
+    float *inv;         // [kCW] each consumer warp's 1/rms of the current phase (see hand_tile)
     float *rope;        // cos[128] | sin[128] of the token position
     uint64_t *full, *empty, *red_full, *red_empty;
-    uint64_t *rx;       // pair staging: counts the bytes the partner has mirrored into this CTA for the current staging
-    int *free_gen;      // pair staging: written by the partner: the number of phases it has finished (its buffers may be overwritten)
+    uint64_t *rx;       // pair mode: counts the bytes of the partner's 16 partial sums of squares (RMSNorm)
+    float *prx;         // pair mode: [kPairSlots][16] tile row sums received from the partner
+    uint64_t *prx_full; // [kPairSlots] pair mode: completed by the partner's st.async of a slot of `prx`
+    uint64_t *pfree;    // [kPairSlots] pair mode: arrived on by the partner once it has read the row sums this CTA sent into its slot
     int2 *red_pos;      // [kCW] each consumer warp's position in the red-buffer ring between GEMV phases (see consume_gemv)
     uint32_t ring_u32, xs_u32, gx_u32, gsum_u32, full_u32, empty_u32, redfull_u32, redempty_u32;
     int nst;
 };
+
+// residual floats a CTA keeps: pair mode the channels of its K range of the E-wide RMSNorm ops (the larger half: rank 0)
+__host__ __device__ inline int resid_floats(const Args &a) { return a.pair ? plane_ic(a.E / kW4Group, 1) : a.E; }
 
 TCE_DEVINL PSmem carve(uint8_t *raw, const Args &a) {
     PSmem s;
@@ -193,7 +194,7 @@ TCE_DEVINL PSmem carve(uint8_t *raw, const Args &a) {
     s.xs = p;
     p += a.xs_bytes;
     s.resid = reinterpret_cast<float *>(p);
-    p += (size_t)a.E * 4;
+    p += (size_t)resid_floats(a) * 4;
     s.gx = reinterpret_cast<float *>(p);
     p += (size_t)a.max_ng * 4;
     s.gsum = reinterpret_cast<int *>(p);
@@ -202,15 +203,20 @@ TCE_DEVINL PSmem carve(uint8_t *raw, const Args &a) {
     p += (size_t)kRedBufs * kCW * 16 * 4;
     s.rms = reinterpret_cast<float *>(p);
     p += 32 * 4;
+    s.inv = reinterpret_cast<float *>(p);
+    p += kCW * 4;
     s.rope = reinterpret_cast<float *>(p);
     p += 256 * 4;
+    s.prx = reinterpret_cast<float *>(p);
+    p += kPairSlots * 16 * 4;
     s.full = reinterpret_cast<uint64_t *>(p);
     s.empty = s.full + a.nst;
     s.red_full = s.empty + a.nst;
     s.red_empty = s.red_full + kRedBufs;
     s.rx = s.red_empty + kRedBufs;
-    s.free_gen = reinterpret_cast<int *>(s.rx + 1);
-    s.red_pos = reinterpret_cast<int2 *>(s.rx + 2);
+    s.prx_full = s.rx + 1;
+    s.pfree = s.prx_full + kPairSlots;
+    s.red_pos = reinterpret_cast<int2 *>(s.pfree + kPairSlots);
     s.ring_u32 = smem_u32(s.ring);
     s.xs_u32 = smem_u32(s.xs);
     s.gx_u32 = smem_u32(s.gx);
@@ -243,8 +249,13 @@ struct Red {
     }
 };
 
-// this CTA's tile range of one GEMV op: cut at tile boundaries (every output has exactly one writer)
-TCE_DEVINL void partition(const GemvOp &op, int cta, int ncta, int &t0, int &t1) {
+// this CTA's tile range of one GEMV op: cut at tile boundaries (every output has exactly one writer).  Pair mode: both CTAs of a cluster
+// (CTAs 2i, 2i + 1) walk the range of pair i, each over its own K range.
+TCE_DEVINL void partition(const GemvOp &op, int cta, int ncta, int pair, int &t0, int &t1) {
+    if (pair) {
+        cta >>= 1;
+        ncta >>= 1;
+    }
     const unsigned T = (unsigned)op.num_tiles;
     t0 = (int)((T * (unsigned)cta) / (unsigned)ncta);
     t1 = (int)((T * (unsigned)(cta + 1)) / (unsigned)ncta);
@@ -278,40 +289,46 @@ TCE_DEVINL AttnSplit attn_split(int cta, int ncta, int KVH, int pos) {
 }
 
 // ------------------------------------------------------------------------------------------------------------ producer
-// one weight stage: the box of groups 32s + 16b lands at b * 16 KiB (gate | up: the up rows 8 KiB into it); see GemvOp
-TCE_DEVINL void produce_gemv(const GemvOp &op, const CUtensorMap *m0, const uint8_t *meta, const PSmem &sm, Ring &rs, int cta, int ncta, uint32_t leader,
-                             uint64_t policy) {
+// one weight stage: the next two boxes of this CTA's (tile, box) walk (see KRange), slot b at b * 16 KiB (gate | up: the up rows 8 KiB into
+// it), and their two scale|zero records, which are adjacent in the repacked array
+TCE_DEVINL void produce_gemv(const GemvOp &op, const CUtensorMap *m0, const uint8_t *meta, const PSmem &sm, Ring &rs, int cta, int ncta, int pair, int rank,
+                             uint32_t leader, uint64_t policy) {
     int t0, t1;
-    partition(op, cta, ncta, t0, t1);
-    const uint32_t box_bytes = 16u * (uint32_t)op.bw * 64u;  // 16 rows (gate | up: 8 of each matrix) x bw groups x 64 B
-    for (int tile = t0; tile < t1; tile++) {
-        // the tile's matrix (q|k|v: tiles never straddle two segments; gate | up: the gate map, the up map follows it) and first row
-        int row = op.pair ? tile * 8 : tile * 16;
-        const CUtensorMap *m = m0;
-        if (!op.pair && op.nseg > 1 && row >= op.rows0) {
-            row -= op.rows0;
-            m = m0 + 1;
-            if (op.nseg > 2 && row >= op.rows1) {
-                row -= op.rows1;
-                m = m0 + 2;
-            }
-        }
-        for (int s = 0; s < op.S; s++) {
-            const int nbox = (min(kStageGroups, op.NG - kStageGroups * s) + 15) >> 4;
-            mbar_wait(&sm.empty[rs.stage], rs.phase ^ 1);
-            uint64_t *bar = &sm.full[rs.stage];
-            uint8_t *dst = sm.ring + (size_t)rs.stage * kStageBytes;
-            mbar_arrive_expect_tx_pred(bar, (uint32_t)nbox * box_bytes + kMetaBytes, leader);
+    partition(op, cta, ncta, pair, t0, t1);
+    const KRange kr = k_range(op.NG, pair, rank);
+    const uint32_t box_bytes = 16u * (uint32_t)kr.bw * 64u;  // 16 rows (gate | up: 8 of each matrix) x bw groups x 64 B
+    const int nbox = (t1 - t0) * kr.nb;
+    const uint8_t *rec = meta + (size_t)t0 * kr.nb * kBoxMetaBytes;
+    int tile = t0, box = 0;
+    for (int i = 0; i < nbox; i += 2) {
+        const int n = min(2, nbox - i);
+        mbar_wait(&sm.empty[rs.stage], rs.phase ^ 1);
+        uint64_t *bar = &sm.full[rs.stage];
+        uint8_t *dst = sm.ring + (size_t)rs.stage * kStageBytes;
+        mbar_arrive_expect_tx_pred(bar, (uint32_t)n * (box_bytes + kBoxMetaBytes), leader);
 #pragma unroll 1
-            for (int b = 0; b < nbox; b++) {
-                const int grp = kStageGroups * s + 16 * b;
-                tma_load_3d_pred(dst + b * 16384, m, 0, row, grp, bar, policy, leader);
-                if (op.pair) tma_load_3d_pred(dst + b * 16384 + 8192, m + 1, 0, row, grp, bar, policy, leader);
+        for (int b = 0; b < n; b++) {
+            // the tile's matrix (q|k|v: tiles never straddle two segments; gate | up: the gate map, the up map follows it) and first row
+            int row = op.pair ? tile * 8 : tile * 16;
+            const CUtensorMap *m = m0;
+            if (!op.pair && op.nseg > 1 && row >= op.rows0) {
+                row -= op.rows0;
+                m = m0 + 1;
+                if (op.nseg > 2 && row >= op.rows1) {
+                    row -= op.rows1;
+                    m = m0 + 2;
+                }
             }
-            bulk_g2s_pred(dst + kMetaOff, meta + ((size_t)tile * op.S + s) * kMetaBytes, kMetaBytes, bar, policy, leader);
-            __syncwarp();
-            rs.advance(sm.nst);
+            tma_load_3d_pred(dst + b * 16384, m, 0, row, box * kBoxGroups, bar, policy, leader);
+            if (op.pair) tma_load_3d_pred(dst + b * 16384 + 8192, m + 1, 0, row, box * kBoxGroups, bar, policy, leader);
+            if (++box == kr.nb) {
+                box = 0;
+                tile++;
+            }
         }
+        bulk_g2s_pred(dst + kMetaOff, rec + (size_t)i * kBoxMetaBytes, (uint32_t)n * kBoxMetaBytes, bar, policy, leader);
+        __syncwarp();
+        rs.advance(sm.nst);
     }
 }
 
@@ -334,63 +351,65 @@ TCE_DEVINL void produce_attn(const Args &a, const LayerDesc &L, const CUtensorMa
 }
 
 // the loader warp: every byte this CTA needs from HBM, in consumption order, as ring slots free up
-TCE_DEVINL void producer_walk(const Args &a, const PSmem &sm, int cta, int ncta, int pos, int lane) {
+TCE_DEVINL void producer_walk(const Args &a, const PSmem &sm, int cta, int ncta, int rank, int pos, int lane) {
     Ring rs;
     const uint64_t policy = l2_policy_evict_first();
     const uint32_t leader = (lane == 0) ? 1u : 0u;
     const int Lyr = a.num_layers, nphase = 5 * Lyr + 1;
     const CUtensorMap *kvmap = a.maps + (size_t)Lyr * 7 + 1;
+    const int set = a.pair ? 1 + rank : 0;
+    const CUtensorMap *wmaps = a.maps + (size_t)set * (Lyr * 7 + 2);
 #pragma unroll 1
     for (int p = 0; p < nphase; p++) {
         const int l = p / 5, k = p - 5 * l;
         if (l == Lyr) {
-            produce_gemv(a.op[OPI_LMHEAD], a.maps + (size_t)Lyr * 7, a.lm_meta, sm, rs, cta, ncta, leader, policy);
+            produce_gemv(a.op[OPI_LMHEAD], wmaps + (size_t)Lyr * 7, a.lm_meta[set], sm, rs, cta, ncta, a.pair, rank, leader, policy);
         } else if (k == 1) {
             produce_attn(a, a.layers[l], kvmap, sm, rs, cta, ncta, pos, leader, policy);
         } else {
             const int oi = (k == 0) ? OPI_QKV : (k - 1);       // k = 2,3,4 -> OPI_O, OPI_GATEUP, OPI_DOWN
             const int mi = (k == 0) ? 0 : (k == 2 ? 3 : (k == 3 ? 4 : 6));  // first tensor map of the op within the layer's seven
-            produce_gemv(a.op[oi], a.maps + (size_t)l * 7 + mi, a.layers[l].meta[oi], sm, rs, cta, ncta, leader, policy);
+            produce_gemv(a.op[oi], wmaps + (size_t)l * 7 + mi, a.layers[l].meta[set][oi], sm, rs, cta, ncta, a.pair, rank, leader, policy);
         }
     }
 }
 
-// ------------------------------------------------------------------------------------------------------------ pair staging (clusters of two CTAs)
-// Every CTA needs the whole quantised input vector of a GEMV phase.  In pair mode the two CTAs of a cluster split that work: CTA `rank` polls and
-// quantises the 128-groups g = rank (mod 2) and mirrors planes / steps / sums into its partner with st.async (remote shared-memory stores that
-// complete transaction bytes on the partner's `rx` mbarrier: no fence, no flag).  A CTA tells its partner when its buffers may be overwritten
-// (`free_gen` = phases finished, a relaxed remote store: it only orders the partner's writes after this CTA's reads).
+// ------------------------------------------------------------------------------------------------------------ pair mode (clusters of two CTAs)
+// The two CTAs of a cluster walk the same tiles, CTA `rank` over its K range (k_range): each stages, keeps and reads only its own half of the
+// activation planes and of the residual stream.  What crosses between them goes by st.async (remote shared-memory stores that complete
+// transaction bytes on the receiver's mbarrier: no fence, no flag): the 16 partial sums of squares of an RMSNorm, and the 16 row sums of
+// every tile the partner publishes.
 struct PairCtx {
     bool on = false;
     uint32_t rank = 0;
-    gemv::PairDst dst = {0u, 0u, 0u, 0u};
-    uint32_t r_rms = 0, r_free = 0;  // partner's rms[16..31] and free_gen
-    uint32_t nstage = 0;             // stagings done so far (parity of the rx barrier)
+    uint32_t r_rms = 0, r_bar = 0;  // partner's rms[] and rx barrier
+    uint32_t nstage = 0;            // RMSNorm exchanges so far (parity of the rx barrier)
 };
 TCE_DEVINL uint32_t map_to_cta(uint32_t local_u32, uint32_t rank) {
     uint32_t r;
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_u32), "r"(rank));
     return r;
 }
-TCE_DEVINL void st_cluster_u32(uint32_t raddr, uint32_t v) { asm volatile("st.relaxed.cluster.shared::cluster.u32 [%0], %1;" ::"r"(raddr), "r"(v) : "memory"); }
-// groups a CTA stages itself / expects from its partner
-TCE_DEVINL int own_groups(const PairCtx &pc, int NG) { return pc.on ? (NG + 1 - (int)pc.rank) / 2 : NG; }
-TCE_DEVINL int peer_groups(const PairCtx &pc, int NG) { return pc.on ? (NG + (int)pc.rank) / 2 : 0; }
-// before the first mirrored store of phase p: the partner has finished phase p - 1 (it no longer reads the buffers this CTA writes into)
-TCE_DEVINL void wait_partner_free(const PSmem &sm, const PairCtx &pc, int p) {
-    if (!pc.on || p == 0) return;
+TCE_DEVINL void st_async_b32(uint32_t raddr, uint32_t v, uint32_t rbar) {
+    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(raddr), "r"(v), "r"(rbar) : "memory");
+}
+// Relaxed: the only access it has to follow is a shared-memory read whose value an earlier instruction has already used (a release at
+// cluster scope also waits for the warp's global stores, the results it has just published, to drain).
+TCE_DEVINL void mbar_arrive_remote(uint32_t rbar) { asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(rbar) : "memory"); }
+TCE_DEVINL void mbar_wait_cluster(uint32_t bar, uint32_t parity) {  // acquire at cluster scope: the arrival came from the partner
     const long long t0 = clock64();
-    while (lds_volatile_i32(sm.free_gen) < p) {
+    while (true) {
+        uint32_t ok;
+        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                     : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
+        if (ok) return;
         if (clock64() - t0 > kSpinLimit) __trap();
     }
 }
-// arm the rx barrier for this staging (one thread) / wait for the partner's bytes (every consumer thread)
-TCE_DEVINL void rx_expect(const PSmem &sm, const PairCtx &pc, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(sm.rx)), "r"(bytes) : "memory");
-}
-TCE_DEVINL void rx_wait(const PSmem &sm, PairCtx &pc) {
-    mbar_wait_u32(smem_u32(sm.rx), pc.nstage & 1u);
-    pc.nstage++;
+TCE_DEVINL uint32_t cluster_rank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
 }
 
 // ------------------------------------------------------------------------------------------------------------ consumers: staging
@@ -403,14 +422,11 @@ TCE_DEVINL int rot_unit(int u, int units, int cta) {
     return (g << 4) | (u & 15);
 }
 
-// fp16 input vector (attention output / SiLU*mul activations) published as {half2, tag} words -> activation planes
-TCE_DEVINL void stage_half(const GemvOp &op, const PSmem &sm, PairCtx &pc, const uint2 *src, uint32_t tag, int cta, int ctid, int lane, int p) {
-    const int ng_own = own_groups(pc, op.NG);
-    const int units = ng_own * 16;  // 8 halfs = 4 words = 32 B per unit; this CTA's groups only (pair mode: every other group)
-    if (pc.on) {
-        if (ctid == 0) rx_expect(sm, pc, (uint32_t)peer_groups(pc, op.NG) * 524u);  // 16 units x 32 B of planes + step + two sums per group
-        wait_partner_free(sm, pc, p);
-    }
+// fp16 input vector (attention output / SiLU*mul activations) published as {half2, tag} words -> activation planes of this CTA's K range
+TCE_DEVINL void stage_half(const GemvOp &op, const PSmem &sm, const PairCtx &pc, const uint2 *src, uint32_t tag, int cta, int ctid, int lane) {
+    const KRange kr = k_range(op.NG, pc.on, pc.rank);
+    const int units = kr.ng * 16;  // 8 halfs = 4 words = 32 B per unit
+    const int xic = plane_ic(op.NG, pc.on);
     constexpr int PRE = 4;        // iterations whose words are requested together: one L2 round trip for up to 4 * 512 units
     for (int ub = 0; ub < units; ub += PRE * kConsumerThreads) {
         uint4 w[PRE][2];
@@ -419,14 +435,11 @@ TCE_DEVINL void stage_half(const GemvOp &op, const PSmem &sm, PairCtx &pc, const
         for (int k = 0; k < PRE; k++) {
             const int u = ub + k * kConsumerThreads + ctid;
             ui[k] = -1;
-            if (u < units) {
-                const int ru = rot_unit(u, units, cta);  // index among this CTA's groups
-                ui[k] = pc.on ? (((ru >> 4) * 2 + (int)pc.rank) << 4) | (ru & 15) : ru;
-            }
+            if (u < units) ui[k] = rot_unit(u, units, cta);  // index within this CTA's K range
             w[k][0] = w[k][1] = make_uint4(0u, tag, 0u, tag);
             if (ui[k] >= 0) {
-                w[k][0] = ld_ll2(src + (size_t)ui[k] * 4, false);
-                w[k][1] = ld_ll2(src + (size_t)ui[k] * 4 + 2, false);
+                w[k][0] = ld_ll2(src + (size_t)(kr.g0 * 16 + ui[k]) * 4, false);
+                w[k][1] = ld_ll2(src + (size_t)(kr.g0 * 16 + ui[k]) * 4 + 2, false);
             }
         }
         {
@@ -441,8 +454,8 @@ TCE_DEVINL void stage_half(const GemvOp &op, const PSmem &sm, PairCtx &pc, const
 #pragma unroll
                 for (int k = 0; k < PRE; k++) {
                     if (ui[k] >= 0 && !(w[k][0].y == tag && w[k][0].w == tag && w[k][1].y == tag && w[k][1].w == tag)) {
-                        w[k][0] = ld_ll2(src + (size_t)ui[k] * 4, false);
-                        w[k][1] = ld_ll2(src + (size_t)ui[k] * 4 + 2, false);
+                        w[k][0] = ld_ll2(src + (size_t)(kr.g0 * 16 + ui[k]) * 4, false);
+                        w[k][1] = ld_ll2(src + (size_t)(kr.g0 * 16 + ui[k]) * 4 + 2, false);
                     }
                 }
             }
@@ -456,14 +469,10 @@ TCE_DEVINL void stage_half(const GemvOp &op, const PSmem &sm, PairCtx &pc, const
             const float2 f0 = h2_to_f2(w[k][0].x), f1 = h2_to_f2(w[k][0].z), f2 = h2_to_f2(w[k][1].x), f3 = h2_to_f2(w[k][1].z);
             v[0] = f0.x; v[1] = f0.y; v[2] = f1.x; v[3] = f1.y;
             v[4] = f2.x; v[5] = f2.y; v[6] = f3.x; v[7] = f3.y;
-            if (pc.on)
-                gemv::emit_unit<1, true>(sm.xs, op.IC, sm.gx, sm.gsum, valid ? ui[k] : 0, valid, v, lane, &pc.dst);
-            else
-                gemv::emit_unit<1>(sm.xs, op.IC, sm.gx, sm.gsum, valid ? ui[k] : 0, valid, v, lane);
+            gemv::emit_unit<1>(sm.xs, xic, sm.gx, sm.gsum, valid ? ui[k] : 0, valid, v, lane);
         }
     }
     named_bar_sync(1, kConsumerThreads);
-    if (pc.on) rx_wait(sm, pc);
 }
 
 // Tensor parallel: x[0..7] += the eight output words of every rank's slot, in rank order (bit-identical on all ranks).  The slots of two ranks
@@ -501,35 +510,40 @@ TCE_DEVINL void tp_accumulate(float (&x)[8], const uint2 *slot0, int tp_size, in
     }
 }
 
-// fp32 residual stream with fused RMSNorm.  Every CTA holds the stream in shared memory; `delta` (o_proj or down_proj outputs of all
-// tensor-parallel ranks, {float, tag} words) is added to it here by every CTA in the same (rank) order.  Returns 1/rms: y = inv * W (x . gamma).
-TCE_DEVINL float stage_rms(const Args &a, const GemvOp &op, const PSmem &sm, PairCtx &pc, const uint2 *delta, uint32_t tag, const float *gamma, int token,
-                           bool first, bool emit, int cta, int ctid, int cw, int lane, int p) {
-    const int units = own_groups(pc, op.NG) * 16;  // pair mode: this CTA keeps (and normalises) every other 128-group of the residual stream
-    const bool sys = a.tp_size > 1;
-    if (pc.on && emit) {
-        if (ctid == 0) rx_expect(sm, pc, (uint32_t)peer_groups(pc, op.NG) * 524u + (uint32_t)kCW * 4u);  // + the partner's 16 partial sums of squares
-        wait_partner_free(sm, pc, p);
-    }
+// 1/rms from the `nparts` partial sums of squares of an IC-wide vector
+TCE_DEVINL float rms_inv(const PSmem &sm, int nparts, int IC, float eps) {
+    float tot = 0.f;
+    for (int w = 0; w < nparts; w++) tot += sm.rms[w];
+    return rsqrtf(tot / (float)IC + eps);  // LlamaRMSNorm (llm/src/ops/LlamaRMSNorm.cc): x / sqrt(mean(x^2) + eps) * weight
+}
+
+// fp32 residual stream with fused RMSNorm.  Every CTA holds the stream (pair mode: the channels of its K range) in shared memory; `delta`
+// (o_proj or down_proj outputs of all tensor-parallel ranks, {float, tag} words) is added to it here by every CTA in the same (rank) order.
+// Single-CTA: returns 1/rms (y = inv * W (x . gamma)).  Pair mode: returns once this CTA's 16 partial sums of squares are written; the
+// partner's arrive on the rx barrier, and hand_tile() takes 1/rms from all 32 at a consumer's first tile hand-off.
+TCE_DEVINL float stage_rms(const Args &a, const GemvOp &op, const PSmem &sm, const PairCtx &pc, const uint2 *delta, uint32_t tag, const float *gamma, int token,
+                           bool first, bool emit, int cta, int ctid, int cw, int lane) {
+    const KRange kr = k_range(op.NG, pc.on, pc.rank);
+    const int units = kr.ng * 16;
+    const int xic = plane_ic(op.NG, pc.on);
+    if (pc.on && emit && ctid == 0)
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(sm.rx)), "r"((uint32_t)kCW * 4u) : "memory");  // the partner's 16 sums
     float ss = 0.f;
     for (int ui0 = 0; ui0 < units; ui0 += kConsumerThreads) {  // warp-uniform trip count
         const int u = ui0 + ctid;
         const bool valid = u < units;
-        int ui = 0;
-        if (valid) {
-            const int ru = rot_unit(u, units, cta);
-            ui = pc.on ? (((ru >> 4) * 2 + (int)pc.rank) << 4) | (ru & 15) : ru;
-        }
+        const int ui = valid ? rot_unit(u, units, cta) : 0;  // unit within this CTA's K range (residual copy, planes)
+        const int gu = kr.g0 * 16 + ui;                       // unit of the E-wide vectors
         float x[8], v[8];
 #pragma unroll
         for (int i = 0; i < 8; i++) x[i] = 0.f;
         float4 g0 = make_float4(0.f, 0.f, 0.f, 0.f), g1 = g0;
         if (valid) {
-            g0 = *reinterpret_cast<const float4 *>(gamma + (size_t)ui * 8);  // static: requested before the spin
-            g1 = *reinterpret_cast<const float4 *>(gamma + (size_t)ui * 8 + 4);
+            g0 = *reinterpret_cast<const float4 *>(gamma + (size_t)gu * 8);  // static: requested before the spin
+            g1 = *reinterpret_cast<const float4 *>(gamma + (size_t)gu * 8 + 4);
             if (first) {
                 // the token's embedding row is the residual stream (reference: CPU Embedding, cuda/Int4llamaDecoder.cu:62-69)
-                const uint4 raw = *reinterpret_cast<const uint4 *>(a.embed + (size_t)token * a.E + (size_t)ui * 8);
+                const uint4 raw = *reinterpret_cast<const uint4 *>(a.embed + (size_t)token * a.E + (size_t)gu * 8);
                 const __half2 *h2 = reinterpret_cast<const __half2 *>(&raw);
 #pragma unroll
                 for (int i = 0; i < 4; i++) {
@@ -546,11 +560,11 @@ TCE_DEVINL float stage_rms(const Args &a, const GemvOp &op, const PSmem &sm, Pai
                 // one L2 round trip per batch instead of one per rank (measured at P = 8: the per-rank round trips made 8 GPUs slower than 4)
                 if (a.tp_size == 1) {
                     uint4 w[4];
-                    wait_ll2xN<4>(delta + (size_t)ui * 8, tag, false, w);
+                    wait_ll2xN<4>(delta + (size_t)gu * 8, tag, false, w);
                     x[0] += __uint_as_float(w[0].x); x[1] += __uint_as_float(w[0].z); x[2] += __uint_as_float(w[1].x); x[3] += __uint_as_float(w[1].z);
                     x[4] += __uint_as_float(w[2].x); x[5] += __uint_as_float(w[2].z); x[6] += __uint_as_float(w[3].x); x[7] += __uint_as_float(w[3].z);
                 } else {
-                    tp_accumulate(x, delta + (size_t)ui * 8, a.tp_size, a.E, tag);
+                    tp_accumulate(x, delta + (size_t)gu * 8, a.tp_size, a.E, tag);
                 }
             }
             *reinterpret_cast<float4 *>(sm.resid + (size_t)ui * 8) = make_float4(x[0], x[1], x[2], x[3]);
@@ -561,25 +575,18 @@ TCE_DEVINL float stage_rms(const Args &a, const GemvOp &op, const PSmem &sm, Pai
             for (int i = 0; i < 8; i++) ss += x[i] * x[i];
             v[0] = x[0] * g0.x; v[1] = x[1] * g0.y; v[2] = x[2] * g0.z; v[3] = x[3] * g0.w;
             v[4] = x[4] * g1.x; v[5] = x[5] * g1.y; v[6] = x[6] * g1.z; v[7] = x[7] * g1.w;
-            if (pc.on)
-                gemv::emit_unit<1, true>(sm.xs, op.IC, sm.gx, sm.gsum, ui, valid, v, lane, &pc.dst);
-            else
-                gemv::emit_unit<1>(sm.xs, op.IC, sm.gx, sm.gsum, ui, valid, v, lane);
+            gemv::emit_unit<1>(sm.xs, xic, sm.gx, sm.gsum, ui, valid, v, lane);
         }
     }
     if (!emit) return 1.f;
     ss = warp_sum(ss);
-    // partial sums of squares: slot (staging rank, warp) on both CTAs of a pair, so that both add them in the same order
+    // partial sums of squares: slot (rank, warp) on both CTAs of a pair, so that both add them in the same order
     if (lane == 0) {
         sm.rms[pc.rank * kCW + cw] = ss;
-        if (pc.on) gemv::st_async_b32(pc.r_rms + (uint32_t)(pc.rank * kCW + cw) * 4u, __float_as_uint(ss), pc.dst.bar);
+        if (pc.on) st_async_b32(pc.r_rms + (uint32_t)(pc.rank * kCW + cw) * 4u, __float_as_uint(ss), pc.r_bar);
     }
     named_bar_sync(1, kConsumerThreads);
-    if (pc.on) rx_wait(sm, pc);
-    float tot = 0.f;
-    const int nparts = pc.on ? 2 * kCW : kCW;
-    for (int w = 0; w < nparts; w++) tot += sm.rms[w];
-    return rsqrtf(tot / (float)op.IC + a.eps);  // LlamaRMSNorm (llm/src/ops/LlamaRMSNorm.cc): x / sqrt(mean(x^2) + eps) * weight
+    return pc.on ? 0.f : rms_inv(sm, kCW, op.IC, a.eps);
 }
 
 // ------------------------------------------------------------------------------------------------------------ consumers: GEMV
@@ -590,9 +597,9 @@ struct UnitRegs {
     uint32_t z;   // zero points of rows g (bits 0..7) and g + 8 (bits 8..15)
     uint32_t sc;  // half2: scales of rows g, g + 8
     int sxv;
-    float st;
 };
-TCE_DEVINL void unit_compute(const UnitRegs &u, float lscale, float &totA, float &totB) {
+// st_addr: the group's activation step, read after the MMAs are issued (held from the operand loads on, it was spilled to local memory)
+TCE_DEVINL void unit_compute(const UnitRegs &u, uint32_t st_addr, float lscale, float &totA, float &totB) {
     constexpr uint32_t ML = 0x0f0f0f0fu, MH = 0xf0f0f0f0u;
     int accL[4], accH[4];
     mma_m16n8k32_u8s8_z(accL, u.wa.x & ML, u.wb.x & ML, u.wa.y & ML, u.wb.y & ML, u.xe.x, u.xe.y);
@@ -600,7 +607,7 @@ TCE_DEVINL void unit_compute(const UnitRegs &u, float lscale, float &totA, float
     mma_m16n8k32_u8s8(accL, u.wa.z & ML, u.wb.z & ML, u.wa.w & ML, u.wb.w & ML, u.xe.z, u.xe.w);
     mma_m16n8k32_u8s8(accH, u.wa.z & MH, u.wb.z & MH, u.wa.w & MH, u.wb.w & MH, u.xo.z, u.xo.w);
     const float2 sc = h2_to_f2(u.sc);
-    const float st = u.st * lscale;
+    const float st = lds_f32(st_addr) * lscale;
     const int zAq = (int)(u.z & 0xFFu), zBq = (int)(u.z >> 8);
     // X = 2^24*p3 + 2^16*p2 + 2^8*p1 + p0; odd slots carry 16 x nibble (exact multiple of 16): c0 * 256 + c1 per parity, then q*X - z*sum X
     const int vA = (accL[0] << 8) + accL[1] + (((accH[0] << 8) + accH[1]) >> 4) - zAq * u.sxv;
@@ -609,17 +616,46 @@ TCE_DEVINL void unit_compute(const UnitRegs &u, float lscale, float &totA, float
     totB += (sc.y * st) * (float)vB;
 }
 
-// Warp cw consumes groups cw and cw + 16 of every stage.  Group gi of a stage sits at a fixed place whatever the shape (see GemvOp), so
-// every operand address is a per-lane constant plus the slot base, and the second unit of a warp sits at fixed distances (+16 KiB weights,
-// +4 KiB planes, +512 B scales ...): the inner loop carries almost no address arithmetic (the ALU pipe is what bounds this loop).
+// Hand one tile's row sums of this warp, times 1/rms, to the epilogue warp (red buffer `cs`).  1/rms is the warp's word sm.inv[cw]; a
+// negative word -1 - parity (pair mode, RMSNorm phase, first tile) means: wait for the partner's sums of squares on the rx barrier, then
+// take 1/rms from all 32.
+TCE_DEVINL void hand_tile(const Args &a, const GemvOp &op, const PSmem &sm, Red &cs, float totA, float totB, int cw, int lane) {
+    const int g = lane >> 2, t = lane & 3;
+    float inv = sm.inv[cw];
+    if (inv < 0.f) {
+        mbar_wait_u32(smem_u32(sm.rx), inv < -1.5f ? 1u : 0u);
+        inv = rms_inv(sm, 2 * kCW, op.IC, a.eps);
+        __syncwarp();  // every lane has read the flag
+        if (lane == 0) sm.inv[cw] = inv;
+    }
+    totA += __shfl_xor_sync(0xffffffffu, totA, 1);  // (p3, p2) share of t = 0 + (p1, p0) share of t = 1
+    totB += __shfl_xor_sync(0xffffffffu, totB, 1);
+    mbar_wait_u32(sm.redempty_u32 + (uint32_t)cs.rb * 8u, cs.rphase ^ 1);
+    float *rbuf = sm.red + ((size_t)cs.rb * kCW + cw) * 16;
+    if (t == 0) {
+        rbuf[g] = totA * inv;
+        rbuf[g + 8] = totB * inv;
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive_u32(sm.redfull_u32 + (uint32_t)cs.rb * 8u);
+    cs.advance();
+}
+
+// A stage holds two boxes of this CTA's (tile, box) walk (see KRange); warp cw consumes group cw of each (slot 0, and slot 1 16 KiB
+// further).  The two boxes may belong to two tiles, and a tile is handed to the epilogue after its last box.  Group gi of a slot sits at a
+// fixed place whatever the shape, so every operand address is a per-lane constant plus the slot base and the box's place in the planes
+// (+4 KiB planes, +128 B sums, +64 B steps per box): the inner loop carries almost no address arithmetic (the ALU pipe is what bounds it).
 // Stamps of consumer warp 0 (TCE_PK_DEBUG): 4 first stage landed, 5 last stage released, 6 last tile handed to the epilogue.
 // The warp's red-buffer position, its lane id and 1/rms are taken afresh here (shared memory, %laneid, a shuffle of the same value), not
 // carried in registers across the phase loop: held there, they were spilled to local memory (the attention and staging code set the
-// register budget) and reloaded on the path of every tile.
-TCE_DEVINL void consume_gemv(const Args &a, const GemvOp &op, const PSmem &sm, Ring &rs, float inv_in, int cta, int ncta, int cw, int p, int nphase) {
+// register budget) and reloaded on the path of every tile.  rx_parity >= 0 (pair mode, RMSNorm phases): 1/rms waits for the partner's
+// sums of squares, which are needed only when the first tile is handed over.
+TCE_DEVINL void consume_gemv(const Args &a, const GemvOp &op, const PSmem &sm, Ring &rs, float inv, int rx_parity, int cta, int ncta, int rank, int cw, int p,
+                             int nphase) {
     int lane;
     asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
-    const float inv = __shfl_sync(0xffffffffu, inv_in, 0);  // every lane holds the same value
+    if (lane == 0) sm.inv[cw] = rx_parity >= 0 ? -1.f - (float)rx_parity : inv;
+    __syncwarp();
     Red cs;
     {
         const int2 rp = sm.red_pos[cw];
@@ -628,76 +664,80 @@ TCE_DEVINL void consume_gemv(const Args &a, const GemvOp &op, const PSmem &sm, R
     }
     const int g = lane >> 2, t = lane & 3;
     int t0, t1;
-    partition(op, cta, ncta, t0, t1);
-    const int NG = op.NG, S = op.S;
+    partition(op, cta, ncta, a.pair, t0, t1);
+    const KRange kr = k_range(op.NG, a.pair, rank);
+    const int nb = kr.nb, nbox = (t1 - t0) * nb;
+    const int lim = kr.ng - cw;  // box b carries this warp's group when 16 b < lim (the last box of a K range may have fewer than 16)
     // row g of group cw, this lane's 16-byte chunk: the 16 rows of a group 64 B apart (conflict-free LDS.128), gate | up as two 8-row regions
     const uint32_t w_lane = (uint32_t)cw * (op.pair ? 512u : 1024u) + (uint32_t)g * 64u + (uint32_t)t * 16u;
     const uint32_t wb_off = op.pair ? 8192u : 512u;  // row g + 8
     const uint32_t m_lane = (uint32_t)kMetaOff + (uint32_t)(cw * 8 + g) * 4u;                            // scales of rows g, g + 8 of group cw
-    const uint32_t z_lane = (uint32_t)kMetaOff + 1024u + (uint32_t)(cw * 8 + g) * 2u;
-    const uint32_t x_lane = sm.xs_u32 + (uint32_t)((g >> 1) & 1) * (uint32_t)op.IC * 2u + (uint32_t)(t * 2 + (g & 1)) * 16u + (uint32_t)cw * 256u;
+    const uint32_t z_lane = (uint32_t)kMetaOff + 512u + (uint32_t)(cw * 8 + g) * 2u;
+    const uint32_t x_lane = sm.xs_u32 + (uint32_t)((g >> 1) & 1) * (uint32_t)plane_ic(op.NG, a.pair) * 2u + (uint32_t)(t * 2 + (g & 1)) * 16u + (uint32_t)cw * 256u;
     const uint32_t s_lane = sm.gsum_u32 + (uint32_t)(2 * cw + (t & 1)) * 4u;
     const uint32_t q_lane = sm.gx_u32 + (uint32_t)cw * 4u;
     const float lscale = (t == 0) ? 65536.f : (t == 1 ? 1.f : 0.f);
     const bool xl = g < 4;  // MMA columns 4..7 are don't-cares
-    if (a.dbg && t1 > t0 && cw == 0 && lane == 0) {  // outside the stage loop: a second wait on the same phase returns at once
+    if (a.dbg && nbox > 0 && cw == 0 && lane == 0) {  // outside the stage loop: a second wait on the same phase returns at once
         mbar_wait_u32(sm.full_u32 + (uint32_t)rs.stage * 8u, rs.phase);
         stamp(a, cta, nphase, p, 4);
     }
-    for (int tile = t0; tile < t1; tile++) {
-        float totA = 0.f, totB = 0.f;
-        for (int s = 0; s < S; s++) {
-            // the stage carries this warp's groups (warp-uniform; a partly filled last stage has fewer than 32)
-            const bool has0 = kStageGroups * s + cw < NG, has1 = kStageGroups * s + cw + 16 < NG;
-            mbar_wait_u32(sm.full_u32 + (uint32_t)rs.stage * 8u, rs.phase);
-            const uint32_t base = sm.ring_u32 + (uint32_t)rs.stage * (uint32_t)kStageBytes;
-            const uint32_t wb_ = base + w_lane, mb_ = base + m_lane, zb_ = base + z_lane;
-            const uint32_t xb_ = x_lane + (uint32_t)s * (kStageGroups * 256u), sb_ = s_lane + (uint32_t)s * (kStageGroups * 8u), qb_ = q_lane + (uint32_t)s * (kStageGroups * 4u);
-            UnitRegs u0, u1;
-            u0.xe = u0.xo = u1.xe = u1.xo = make_uint4(0u, 0u, 0u, 0u);
-            if (has0) {
-                u0.wa = lds_u4(wb_);
-                u0.wb = lds_u4(wb_ + wb_off);
-                if (xl) {
-                    u0.xe = lds_u4(xb_);
-                    u0.xo = lds_u4(xb_ + 128u);
-                }
-                u0.sc = lds_u32(mb_);
-                u0.z = lds_u16(zb_);
-                u0.sxv = (int)lds_u32(sb_);
-                u0.st = lds_f32(qb_);
+    int box = 0;  // box of the next slot within its tile
+    float totA = 0.f, totB = 0.f;
+    for (int left = nbox; left > 0; left -= 2) {
+        const int box0 = box, box1 = (box0 + 1 == nb) ? 0 : box0 + 1;
+        const bool two = left > 1;
+        box = (box1 + 1 == nb) ? 0 : box1 + 1;  // (unused after a lone last box)
+        const bool has0 = box0 * kBoxGroups < lim, has1 = two && box1 * kBoxGroups < lim;  // warp-uniform
+        mbar_wait_u32(sm.full_u32 + (uint32_t)rs.stage * 8u, rs.phase);
+        const uint32_t base = sm.ring_u32 + (uint32_t)rs.stage * (uint32_t)kStageBytes;
+        const uint32_t wb_ = base + w_lane, mb_ = base + m_lane, zb_ = base + z_lane;
+        UnitRegs u0, u1;
+        u0.xe = u0.xo = u1.xe = u1.xo = make_uint4(0u, 0u, 0u, 0u);
+        if (has0) {
+            const uint32_t xb_ = x_lane + (uint32_t)box0 * 4096u;
+            u0.wa = lds_u4(wb_);
+            u0.wb = lds_u4(wb_ + wb_off);
+            if (xl) {
+                u0.xe = lds_u4(xb_);
+                u0.xo = lds_u4(xb_ + 128u);
             }
-            if (has1) {
-                u1.wa = lds_u4(wb_ + 16384u);
-                u1.wb = lds_u4(wb_ + 16384u + wb_off);
-                if (xl) {
-                    u1.xe = lds_u4(xb_ + 4096u);
-                    u1.xo = lds_u4(xb_ + 4096u + 128u);
-                }
-                u1.sc = lds_u32(mb_ + 512u);
-                u1.z = lds_u16(zb_ + 256u);
-                u1.sxv = (int)lds_u32(sb_ + 128u);
-                u1.st = lds_f32(qb_ + 64u);
+            u0.sc = lds_u32(mb_);
+            u0.z = lds_u16(zb_);
+            u0.sxv = (int)lds_u32(s_lane + (uint32_t)box0 * 128u);
+        }
+        if (has1) {
+            const uint32_t xb_ = x_lane + (uint32_t)box1 * 4096u;
+            u1.wa = lds_u4(wb_ + 16384u);
+            u1.wb = lds_u4(wb_ + 16384u + wb_off);
+            if (xl) {
+                u1.xe = lds_u4(xb_);
+                u1.xo = lds_u4(xb_ + 128u);
             }
-            if (has0) unit_compute(u0, lscale, totA, totB);
-            if (has1) unit_compute(u1, lscale, totA, totB);
-            __syncwarp();
-            if (lane == 0) mbar_arrive_u32(sm.empty_u32 + (uint32_t)rs.stage * 8u);
-            rs.advance(sm.nst);
+            u1.sc = lds_u32(mb_ + (uint32_t)kBoxMetaBytes);
+            u1.z = lds_u16(zb_ + (uint32_t)kBoxMetaBytes);
+            u1.sxv = (int)lds_u32(s_lane + (uint32_t)box1 * 128u);
         }
-        if (tile == t1 - 1 && cw == 0 && lane == 0) stamp(a, cta, nphase, p, 5);
-        // ---- hand the tile sums to the epilogue warp ----
-        totA += __shfl_xor_sync(0xffffffffu, totA, 1);  // (p3, p2) share of t = 0 + (p1, p0) share of t = 1
-        totB += __shfl_xor_sync(0xffffffffu, totB, 1);
-        mbar_wait_u32(sm.redempty_u32 + (uint32_t)cs.rb * 8u, cs.rphase ^ 1);
-        float *rbuf = sm.red + ((size_t)cs.rb * kCW + cw) * 16;
-        if (t == 0) {
-            rbuf[g] = totA * inv;
-            rbuf[g + 8] = totB * inv;
+        if (has0) unit_compute(u0, q_lane + (uint32_t)box0 * 64u, lscale, totA, totB);
+        // slot 0 ends a tile: its sums wait in hA / hB while slot 1 starts the next one
+        const bool end0 = box0 + 1 == nb;
+        float hA = 0.f, hB = 0.f;
+        if (end0) {
+            hA = totA;
+            hB = totB;
+            totA = totB = 0.f;
         }
+        if (has1) unit_compute(u1, q_lane + (uint32_t)box1 * 64u, lscale, totA, totB);
         __syncwarp();
-        if (lane == 0) mbar_arrive_u32(sm.redfull_u32 + (uint32_t)cs.rb * 8u);
-        cs.advance();
+        if (lane == 0) mbar_arrive_u32(sm.empty_u32 + (uint32_t)rs.stage * 8u);
+        rs.advance(sm.nst);
+        if (left <= 2 && cw == 0 && lane == 0) stamp(a, cta, nphase, p, 5);
+        const bool end1 = two && box1 + 1 == nb;
+        if (end0) hand_tile(a, op, sm, cs, hA, hB, cw, lane);
+        if (end1) {
+            hand_tile(a, op, sm, cs, totA, totB, cw, lane);
+            totA = totB = 0.f;
+        }
     }
     __syncwarp();  // every lane has read the old position
     if (lane == 0) sm.red_pos[cw] = make_int2(cs.rb, (int)cs.rphase);
@@ -708,18 +748,25 @@ TCE_DEVINL void consume_gemv(const Args &a, const GemvOp &op, const PSmem &sm, R
 // ------------------------------------------------------------------------------------------------------------ epilogue warp
 struct EpiState {
     unsigned long long best;  // PE_LOGITS: running arg-max key of this warp
+    uint32_t nsent, nrecv;    // pair mode: tile row sums sent to / received from the partner so far (slot = n % kPairSlots)
 };
 
 // Stamp (TCE_PK_DEBUG): 7 the last tile's partials are in; the caller stamps 3 after its last publish.
 // The lane id is read here (%laneid), as in consume_gemv: passed in, the lane-derived offsets and predicates were hoisted out of the phase
 // loop, spilled, and reloaded on every tile.
+// Pair mode: rank 0 publishes the first half of the pair's tiles and rank 1 the rest (both epilogue warps publish), adding the partner's 16
+// row sums, received by st.async into a `prx` slot, to its own: the same bits on every run.  Contiguous halves let each direction stream up
+// to kPairSlots tiles ahead; tiles owned alternately made the two epilogues wait for each other on every tile (on H100 the Llama-3-8B step
+// took 2.96 ms instead of 2.01).
 TCE_DEVINL void epilogue_gemv(const Args &a, const GemvOp &op, const PSmem &sm, Red &es, EpiState &st, uint2 *out_ll, int which, uint32_t tag, int cta, int ncta,
                               int p, int nphase) {
     int lane;
     asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
     int t0, t1;
-    partition(op, cta, ncta, t0, t1);
+    partition(op, cta, ncta, a.pair, t0, t1);
     const bool tp = a.tp_size > 1;
+    const uint32_t rank = a.pair ? cluster_rank() : 2u;  // 2: no partner (tested on this register: a flag kept beside it was spilled)
+    const int tsplit = t0 + (t1 - t0 + 1) / 2;            // pair mode: first tile published by rank 1
     for (int tile = t0; tile < t1; tile++) {
         mbar_wait_u32(sm.redfull_u32 + (uint32_t)es.rb * 8u, es.rphase);
         if (tile == t1 - 1 && lane == 0) stamp(a, cta, nphase, p, 7);
@@ -735,6 +782,24 @@ TCE_DEVINL void epilogue_gemv(const Args &a, const GemvOp &op, const PSmem &sm, 
         __syncwarp();
         if (lane == 0) mbar_arrive_u32(sm.redempty_u32 + (uint32_t)es.rb * 8u);
         es.advance();
+        if (rank < 2u) {
+            const bool mine = (tile >= tsplit) == (rank == 1u);
+            const uint32_t slot = (mine ? st.nrecv : st.nsent) % kPairSlots;
+            if (!mine) {  // the partner publishes this tile: send it this CTA's row sums
+                const uint32_t n = st.nsent++;
+                mbar_wait_cluster(smem_u32(sm.pfree + slot), ((n / kPairSlots) & 1u) ^ 1u);
+                if (lane < 16)
+                    st_async_b32(map_to_cta(smem_u32(sm.prx + slot * 16 + lane), rank ^ 1u), __float_as_uint(v), map_to_cta(smem_u32(sm.prx_full + slot), rank ^ 1u));
+                continue;
+            }
+            const uint32_t n = st.nrecv++;
+            const uint32_t fb = smem_u32(sm.prx_full + slot);
+            if (lane == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(fb), "r"(64u) : "memory");
+            mbar_wait_u32(fb, (n / kPairSlots) & 1u);
+            v += sm.prx[slot * 16 + (lane & 15)];  // a sum of two terms: the same bits whichever rank publishes
+            __syncwarp();
+            if (lane == 0) mbar_arrive_remote(map_to_cta(smem_u32(sm.pfree + slot), rank ^ 1u));
+        }
         switch (op.epi) {
             case PE_DELTA_LL:
                 // o_proj / down_proj output rows: one {float, tag} word each, into slot `rank` of every rank's buffer (NVLink peer stores
@@ -1033,9 +1098,10 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
             mbar_init(&sm.red_full[lane - 16], kCW);
             mbar_init(&sm.red_empty[lane - 16], 1);
         }
-        if (lane == 30) {
-            mbar_init(sm.rx, 1);
-            *sm.free_gen = 0;
+        if (lane == 30) mbar_init(sm.rx, 1);
+        if (lane >= 24 && lane < 24 + kPairSlots) {
+            mbar_init(&sm.prx_full[lane - 24], 1);
+            mbar_init(&sm.pfree[lane - 24], 1);
         }
         mbar_fence_init();
     }
@@ -1046,14 +1112,9 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
         asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
         asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
         pc.on = true;
-        asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(pc.rank));
-        const uint32_t peer = pc.rank ^ 1u;
-        pc.dst.xs = map_to_cta(sm.xs_u32, peer);
-        pc.dst.gx = map_to_cta(sm.gx_u32, peer);
-        pc.dst.gsum = map_to_cta(sm.gsum_u32, peer);
-        pc.dst.bar = map_to_cta(smem_u32(sm.rx), peer);
-        pc.r_rms = map_to_cta(smem_u32(sm.rms), peer);
-        pc.r_free = map_to_cta(smem_u32(sm.free_gen), peer);
+        pc.rank = cluster_rank();
+        pc.r_rms = map_to_cta(smem_u32(sm.rms), pc.rank ^ 1u);
+        pc.r_bar = map_to_cta(smem_u32(sm.rx), pc.rank ^ 1u);
     }
     // phase p = 5 * layer + k, k: 0 RMSNorm + q|k|v, 1 attention, 2 o_proj, 3 RMSNorm + gate|up, 4 down_proj; p = 5 * Lyr: lm_head
     const int nphase = 5 * Lyr + 1;
@@ -1069,13 +1130,14 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
         if (warp >= 2) return;  // warps 2 and 3 only donate their registers
         if (warp == 0) {
             // ================= loader: every byte this CTA needs from HBM, in consumption order =================
-            producer_walk(a, sm, cta, ncta, pos, lane);
+            producer_walk(a, sm, cta, ncta, (int)pc.rank, pos, lane);
             return;
         }
         // ================= epilogue warp =================
         Red es;
         EpiState st;
         st.best = 0ull;
+        st.nsent = st.nrecv = 0u;
 #pragma unroll 1
         for (int p = 0; p < nphase; p++) {
             const int l = p / 5, k = p - 5 * l;
@@ -1084,6 +1146,10 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
             uint2 *out = (oi == OPI_QKV) ? a.qkv_ll : (oi == OPI_GATEUP ? a.act_ll : (oi == OPI_O ? a.delta_ll[0] : a.delta_ll[1]));
             epilogue_gemv(a, a.op[oi], sm, es, st, out, (oi == OPI_DOWN) ? 1 : 0, tag_base + 2u * (uint32_t)p, cta, ncta, p, nphase);
             if (lane == 0) stamp(a, cta, nphase, p, 3);
+        }
+        // pair mode: stay resident until the partner has read every row sum sent to it (its last arrivals target this CTA's barriers)
+        if (a.pair) {
+            for (uint32_t n = st.nsent; n < st.nsent + kPairSlots; n++) mbar_wait_cluster(smem_u32(sm.pfree + n % kPairSlots), ((n / kPairSlots) & 1u) ^ 1u);
         }
         unsigned long long key = st.best;
 #pragma unroll
@@ -1117,36 +1183,30 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
             attention_phase(a, a.layers[l], sm, rs, tag_in, tag_base + 2u * (uint32_t)p + 1u, tag_base + 2u * (uint32_t)p, cta, ncta, pos, ctid, cw, lane, p, nphase);
             if (ctid == 0) stamp(a, cta, nphase, p, 2);
             named_bar_sync(1, kConsumerThreads);  // the scratch aliases the activation planes of the next phase
-            if (pc.on && ctid == 0) st_cluster_u32(pc.r_free, (uint32_t)(p + 1));  // the partner may mirror the next phase's planes into this CTA
             continue;
         }
         const int oi = (l == Lyr) ? OPI_LMHEAD : ((k == 0) ? OPI_QKV : (k - 1));
         const GemvOp &op = a.op[oi];
         int t0, t1;
-        partition(op, cta, ncta, t0, t1);
-        const bool work = t1 > t0;
-        bool stage = work;  // pair mode: a CTA stages its half whenever either CTA of the pair has tiles in this phase
-        if (pc.on) {
-            int u0, u1;
-            partition(op, cta ^ 1, ncta, u0, u1);
-            stage = work || u1 > u0;
-        }
+        partition(op, cta, ncta, pc.on, t0, t1);
+        const bool work = t1 > t0;  // pair mode: the same for both CTAs of the cluster
         float inv = 1.f;
+        int rx_parity = -1;
         if (oi == OPI_O) {
-            if (stage) stage_half(op, sm, pc, a.attn_ll, tag_in, cta, ctid, lane, p);
+            if (work) stage_half(op, sm, pc, a.attn_ll, tag_in, cta, ctid, lane);
         } else if (oi == OPI_DOWN) {
-            if (stage) stage_half(op, sm, pc, a.act_ll, tag_in, cta, ctid, lane, p);
+            if (work) stage_half(op, sm, pc, a.act_ll, tag_in, cta, ctid, lane);
         } else {
             // the residual copy of this CTA must see every o_proj / down_proj output, whether or not the CTA owns tiles of this phase
             const float *gamma = (oi == OPI_LMHEAD) ? a.final_norm : (oi == OPI_QKV ? a.layers[l].input_norm : a.layers[l].post_norm);
             const uint2 *delta = (oi == OPI_GATEUP) ? a.delta_ll[0] : a.delta_ll[1];
-            inv = stage_rms(a, op, sm, pc, delta, tag_in, gamma, token, p == 0, stage, cta, ctid, cw, lane, p);
+            inv = stage_rms(a, op, sm, pc, delta, tag_in, gamma, token, p == 0, work, cta, ctid, cw, lane);
+            if (pc.on && work) rx_parity = (int)(pc.nstage++ & 1u);
         }
         if (ctid == 0) stamp(a, cta, nphase, p, 1);
-        if (work) consume_gemv(a, op, sm, rs, inv, cta, ncta, cw, p, nphase);
+        if (work) consume_gemv(a, op, sm, rs, inv, rx_parity, cta, ncta, (int)pc.rank, cw, p, nphase);
         if (ctid == 0) stamp(a, cta, nphase, p, 2);
         named_bar_sync(1, kConsumerThreads);  // every warp is done with the planes before the next phase overwrites them
-        if (pc.on && ctid == 0 && p + 1 < nphase) st_cluster_u32(pc.r_free, (uint32_t)(p + 1));  // (not after the last phase: the partner may be gone)
     }
     // ---- greedy token: decoded once every CTA's epilogue has contributed its maximum ----
     if (cta == 0 && ctid == 0) {
@@ -1177,17 +1237,18 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
 }
 
 // ------------------------------------------------------------------------------------------------------------ repack kernel
-// scales half[rows][sf_w] + zeros u32[rows][zeros_w] (QM_CUDA, llm/tools/quantize_methods.py:370-442) -> one 1280-byte record per
-// (16-row tile, 32-group stage): scales half[32 groups][8][2] (rows g and g + 8 adjacent), then zero points u8[32 groups][8][2] in the same order.
-__global__ void repack_meta_kernel(W4Seg s0, W4Seg s1, W4Seg s2, int nseg, int pair, int NG, int zeros_w, int sf_w, int S, int num_tiles, uint8_t *out) {
-    const int idx = blockIdx.x * blockDim.x + threadIdx.x;  // (tile, s, gi)
-    if (idx >= num_tiles * S * kStageGroups) return;
-    const int gi = idx % kStageGroups, su = idx / kStageGroups;
-    const int tile = su / S, s = su - tile * S;
-    const int G = kStageGroups * s + gi;
-    uint8_t *rec = out + (size_t)su * kMetaBytes;
+// scales half[rows][sf_w] + zeros u32[rows][zeros_w] (QM_CUDA, llm/tools/quantize_methods.py:370-442) -> one 768-byte record per
+// (16-row tile, 16-group box of the K range [g0, g0 + ng)): scales half[16 groups][8][2] (rows g and g + 8 adjacent), then zero points
+// u8[16 groups][8][2] in the same order.
+__global__ void repack_meta_kernel(W4Seg s0, W4Seg s1, W4Seg s2, int nseg, int pair, int g0, int ng, int nb, int zeros_w, int sf_w, int num_tiles, uint8_t *out) {
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;  // (tile, box, gi)
+    if (idx >= num_tiles * nb * kBoxGroups) return;
+    const int gi = idx % kBoxGroups, rb = idx / kBoxGroups;
+    const int tile = rb / nb, box = rb - tile * nb;
+    const int lg = kBoxGroups * box + gi, G = g0 + lg;
+    uint8_t *rec = out + (size_t)rb * kBoxMetaBytes;
     __half *so = reinterpret_cast<__half *>(rec) + gi * 16;  // [g][2]: rows g and g + 8 adjacent
-    uint8_t *zo = rec + 1024 + gi * 16;                        // zero points, same order, one byte each
+    uint8_t *zo = rec + 512 + gi * 16;                         // zero points, same order, one byte each
     for (int r = 0; r < 16; r++) {
         const W4Seg *seg = &s0;
         int row;
@@ -1206,7 +1267,7 @@ __global__ void repack_meta_kernel(W4Seg s0, W4Seg s1, W4Seg s2, int nseg, int p
             }
         }
         const int slot = (r & 7) * 2 + (r >> 3);
-        if (G < NG) {
+        if (lg < ng) {
             so[slot] = seg->scales[(size_t)row * sf_w + G];
             zo[slot] = (uint8_t)((seg->zeros[(size_t)row * zeros_w + (G >> 3)] >> ((G & 7) * 4)) & 0xFu);
         } else {
@@ -1227,27 +1288,29 @@ int attn_nsplit_max(int ncta, int KVH, int max_ctx) {
     return NS < nch ? NS : nch;
 }
 
-static size_t fixed_bytes(int xs_bytes, int max_ng, int E) {
-    return (size_t)xs_bytes + (size_t)E * 4 + (size_t)max_ng * 12 + (size_t)kRedBufs * kCW * 16 * 4 + 32 * 4 + 256 * 4 + (size_t)(2 * kMaxStages + 2 * kRedBufs) * 8 + 16 +
-           (size_t)kCW * 8 + 1024;
+static size_t fixed_bytes(const Args &a) {
+    return (size_t)a.xs_bytes + (size_t)resid_floats(a) * 4 + (size_t)a.max_ng * 12 + (size_t)kRedBufs * kCW * 16 * 4 + 32 * 4 + kCW * 4 + 256 * 4 + (size_t)kPairSlots * 16 * 4 +
+           (size_t)(2 * kMaxStages + 2 * kRedBufs + 1 + 2 * kPairSlots) * 8 + (size_t)kCW * 8 + 1024;
 }
-int pick_stages(int smem_optin, int xs_bytes, int max_ng, int E) {
-    const long long avail = (long long)smem_optin - (long long)fixed_bytes(xs_bytes, max_ng, E);
-    long long n = avail / kStageBytes;
-    if (n > kMaxStages) n = kMaxStages;
-    return n < 2 ? 0 : (int)n;
+void plan_smem(Args &a, int smem_optin) {
+    int xs = attn_scratch_bytes(a.nrep);
+    for (int i = 0; i < OPI_COUNT; i++) xs = max(xs, 4 * plane_ic(a.op[i].NG, a.pair));  // four int8 planes per input channel of the K range
+    a.xs_bytes = (xs + 15) & ~15;
+    a.nst = 0;
+    const long long n = ((long long)smem_optin - (long long)fixed_bytes(a)) / kStageBytes;
+    if (n >= 2) a.nst = (int)(n > kMaxStages ? kMaxStages : n);
 }
-size_t smem_bytes(const Args &a) { return fixed_bytes(a.xs_bytes, a.max_ng, a.E) + (size_t)a.nst * kStageBytes; }
+size_t smem_bytes(const Args &a) { return fixed_bytes(a) + (size_t)a.nst * kStageBytes; }
 
-cudaError_t repack_meta(Ctx *ctx, const W4Seg *segs, int nseg, int pair, int IC, uint8_t *out, cudaStream_t stream) {
-    const int NG = IC / kW4Group, S = (NG + kStageGroups - 1) / kStageGroups;
+cudaError_t repack_meta(Ctx *ctx, const W4Seg *segs, int nseg, int pair, int IC, const KRange &kr, uint8_t *out, cudaStream_t stream) {
     int rows = 0;
     for (int i = 0; i < nseg; i++) rows += segs[i].rows;
     const int num_tiles = rows / 16;
     const int zw = zeros_width(IC, kW4Group);
-    const int total = num_tiles * S * kStageGroups;
+    const int total = num_tiles * kr.nb * kBoxGroups;
     if (total == 0) return cudaSuccess;
-    repack_meta_kernel<<<(total + 127) / 128, 128, 0, stream>>>(segs[0], segs[nseg > 1 ? 1 : 0], segs[nseg > 2 ? 2 : 0], nseg, pair, NG, zw, zw * 8, S, num_tiles, out);
+    repack_meta_kernel<<<(total + 127) / 128, 128, 0, stream>>>(segs[0], segs[nseg > 1 ? 1 : 0], segs[nseg > 2 ? 2 : 0], nseg, pair, kr.g0, kr.ng, kr.nb, zw, zw * 8,
+                                                               num_tiles, out);
     (void)ctx;
     return cudaGetLastError();
 }
@@ -1305,7 +1368,7 @@ cudaError_t launch(Ctx *ctx, const Args &a, cudaStream_t stream) {
     cfg.numAttrs = 1;
     static bool pair_refused = false;  // a cluster launch was refused once in this process
     if (a.pair && !pair_refused) {
-        // Clusters of two CTAs (one TPC) share the activation staging over distributed shared memory.  Launched with the cluster attribute ALONE:
+        // Clusters of two CTAs (one TPC) split K and add each other's tile row sums over distributed shared memory.  Launched with the cluster attribute ALONE:
         // profilers (ncu) cannot intercept a launch that is both cooperative and clustered (LaunchFailed), and co-residency -- what the cooperative
         // attribute would assert -- is established instead by pair_supported(): one CTA per SM fits for all num_sms / 2 clusters, and the step is the only
         // work on its stream.  A CTA that were not resident would surface through the bounded spins (__trap after ~10 s), not as a silent hang.
@@ -1318,13 +1381,18 @@ cudaError_t launch(Ctx *ctx, const Args &a, cudaStream_t stream) {
         cfg.numAttrs = 1;
         e = cudaLaunchKernelEx(&cfg, decode_persistent_kernel, a);
         if (e == cudaSuccess) return e;
-        cudaGetLastError();  // a launch-configuration error is not sticky: run without clusters (every CTA stages the whole vector itself)
+        cudaGetLastError();  // a launch-configuration error is not sticky: run without clusters (every CTA reduces over all of K itself)
         pair_refused = true;
         cfg.attrs = attr;
         cfg.numAttrs = 1;
     }
     Args single = a;
-    single.pair = 0;
+    if (a.pair) {
+        single.pair = 0;
+        plan_smem(single, ctx->smem_optin);
+        if (single.nst < 2) return cudaErrorInvalidConfiguration;
+        cfg.dynamicSmemBytes = smem_bytes(single);
+    }
     return cudaLaunchKernelEx(&cfg, decode_persistent_kernel, single);
 }
 

@@ -94,7 +94,8 @@ cudaError_t gemv_partials_reserve(Ctx *ctx, long long records);
 cudaError_t launch_w4a16_gemv_simple(Ctx *ctx, const W4GemvParams &p);
 cudaError_t launch_w4a16_gemv_g64(Ctx *ctx, const __half *x, const uint32_t *w, const uint32_t *zeros, const __half *scales, __half *y, int M, int IC, int OC);
 cudaError_t encode_w4_tmap(CUtensorMap *out, const void *w, int rows, int IC, int sg, int box_rows);
-cudaError_t encode_w4_tmap_units(CUtensorMap *out, const void *w, int rows, int IC, int sg, int box_rows);  // [group][row][64 B] boxes
+// [group][row][64 B] boxes over the groups [g0, g0 + ng) of each row (ng = 0: all IC / 128)
+cudaError_t encode_w4_tmap_units(CUtensorMap *out, const void *w, int rows, int IC, int sg, int box_rows, int g0 = 0, int ng = 0);
 
 cudaError_t launch_naive_fp16_int4(Ctx *ctx, const __half *A, const int32_t *B, const __half *scales, __half *C, int M, int IC, int OC, int block);
 cudaError_t launch_f32_matmul_transposed(Ctx *ctx, const float *A, const float *B, float *C, int M, int N, int K);

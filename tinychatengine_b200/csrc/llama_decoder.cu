@@ -186,7 +186,6 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         pk::GemvOp o{};
         o.IC = IC;
         o.NG = IC / kW4Group;
-        o.S = (o.NG + pk::kStageGroups - 1) / pk::kStageGroups;
         o.num_tiles = rows / 16;
         o.nseg = nseg;
         o.pair = pair;
@@ -202,23 +201,25 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
     a.op[pk::OPI_GATEUP] = mk(E, 2 * F, 2, 1, F, F, pk::PX_RMS_F32, pk::PE_SILU_LL);
     a.op[pk::OPI_DOWN] = mk(F, E, 1, 0, E, 0, pk::PX_HALF, pk::PE_DELTA_LL);
     a.op[pk::OPI_LMHEAD] = mk(E, V, 1, 0, V, 0, pk::PX_RMS_F32, pk::PE_LOGITS);
-    int max_ic = 0, max_ng = 0;
+    int max_ng = 0, min_ng = 1 << 30;
     for (int i = 0; i < pk::OPI_COUNT; i++) {
-        a.op[i].bw = a.op[i].NG < 16 ? a.op[i].NG : 16;
-        if (a.op[i].IC > max_ic) max_ic = a.op[i].IC;
         if (a.op[i].NG > max_ng) max_ng = a.op[i].NG;
+        if (a.op[i].NG < min_ng) min_ng = a.op[i].NG;
         if (a.op[i].IC % kW4Group || a.op[i].num_tiles < 1) return no("bad GEMV shape");
     }
-    max_ng = (max_ng + 3) & ~3;
-    int xs = 4 * max_ic;  // four int8 activation planes
-    if (xs < pk::attn_scratch_bytes(nrep)) xs = pk::attn_scratch_bytes(nrep);
-    xs = (xs + 15) & ~15;
-    a.xs_bytes = xs;
-    a.max_ng = max_ng;
+    a.max_ng = (max_ng + 3) & ~3;
     a.E = E;
-    a.nst = pk::pick_stages(ctx_->smem_optin, xs, max_ng, E);
+    a.nrep = nrep;
+    // pair mode (clusters of two CTAs that split K, see pk::KRange): on unless switched off, or the device cannot co-schedule num_sms / 2
+    // such clusters, or an op has a single 128-group to split
+    a.pair = (!getenv("TCE_PK_PAIR") || atoi(getenv("TCE_PK_PAIR")) != 0) && ncta % 2 == 0 && min_ng >= 2 ? 1 : 0;
+    pk::plan_smem(a, ctx_->smem_optin);
+    if (a.pair && (a.nst < 2 || !pk::pair_supported(ctx_, a))) {
+        a.pair = 0;
+        pk::plan_smem(a, ctx_->smem_optin);
+    }
     if (a.nst < 2) return no("shared memory too small for the persistent kernel");
-    a.pair = 0;  // decided below, once the shared-memory footprint is known
+    const int nsets = a.pair ? pk::kMapSets : 1;  // full K (what a refused cluster launch falls back to), then the pair halves
 
     auto dalloc = [&](size_t bytes) -> void * {
         DevPtr<uint8_t> p;
@@ -227,8 +228,9 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         return pk_allocs_.back().get();
     };
     cudaStream_t s = ctx_->stream;
-    // ---- tensor maps: [Lyr][7] + lm_head + KV cache ----
-    std::vector<CUtensorMap> maps((size_t)Lyr * 7 + 2);
+    // ---- tensor maps: per set [Lyr][7] + lm_head + KV cache ----
+    const size_t nmaps = (size_t)Lyr * 7 + 2;
+    std::vector<CUtensorMap> maps(nsets * nmaps);
     memset(maps.data(), 0, maps.size() * sizeof(CUtensorMap));
     std::vector<pk::LayerDesc> descs(Lyr);
     const size_t per_kv = (size_t)KVH * cfg_.max_ctx;  // rows per (layer, K|V) slab
@@ -236,9 +238,12 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         const tce_llama_layer &L = layers_[l];
         const tce_w4_tensor *t7[7] = {&L.q, &L.k, &L.v, &L.o, &L.gate, &L.up, &L.down};
         const int opi[7] = {pk::OPI_QKV, pk::OPI_QKV, pk::OPI_QKV, pk::OPI_O, pk::OPI_GATEUP, pk::OPI_GATEUP, pk::OPI_DOWN};
-        for (int i = 0; i < 7; i++) {
-            const pk::GemvOp &o = a.op[opi[i]];
-            DCK(encode_w4_tmap_units(&maps[(size_t)l * 7 + i], t7[i]->w, t7[i]->oc, t7[i]->ic, o.bw, o.pair ? 8 : 16));
+        for (int set = 0; set < nsets; set++) {
+            for (int i = 0; i < 7; i++) {
+                const pk::GemvOp &o = a.op[opi[i]];
+                const pk::KRange kr = pk::k_range(o.NG, set > 0, set - 1);
+                DCK(encode_w4_tmap_units(&maps[set * nmaps + (size_t)l * 7 + i], t7[i]->w, t7[i]->oc, t7[i]->ic, kr.bw, o.pair ? 8 : 16, kr.g0, kr.ng));
+            }
         }
         pk::LayerDesc &D = descs[l];
         memset(&D, 0, sizeof(D));
@@ -246,12 +251,15 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         const W4Seg *segs[4] = {qkv, o1, gu, d1};
         const int nsegs[4] = {3, 1, 2, 1}, pairs[4] = {0, 0, 1, 0};
         const int ops4[4] = {pk::OPI_QKV, pk::OPI_O, pk::OPI_GATEUP, pk::OPI_DOWN};
-        for (int i = 0; i < 4; i++) {
-            const pk::GemvOp &o = a.op[ops4[i]];
-            uint8_t *m = (uint8_t *)dalloc((size_t)o.num_tiles * o.S * pk::kMetaBytes);
-            if (!m) return cudaErrorMemoryAllocation;
-            DCK(pk::repack_meta(ctx_, segs[i], nsegs[i], pairs[i], o.IC, m, s));
-            D.meta[i] = m;
+        for (int set = 0; set < nsets; set++) {
+            for (int i = 0; i < 4; i++) {
+                const pk::GemvOp &o = a.op[ops4[i]];
+                const pk::KRange kr = pk::k_range(o.NG, set > 0, set - 1);
+                uint8_t *m = (uint8_t *)dalloc((size_t)o.num_tiles * kr.nb * pk::kBoxMetaBytes);
+                if (!m) return cudaErrorMemoryAllocation;
+                DCK(pk::repack_meta(ctx_, segs[i], nsegs[i], pairs[i], o.IC, kr, m, s));
+                D.meta[set][i] = m;
+            }
         }
         D.input_norm = L.input_norm;
         D.post_norm = L.post_norm;
@@ -262,13 +270,16 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
     }
     {
         const pk::GemvOp &o = a.op[pk::OPI_LMHEAD];
-        DCK(encode_w4_tmap_units(&maps[(size_t)Lyr * 7], w_.lm_head.w, w_.lm_head.oc, w_.lm_head.ic, o.bw, 16));
-        uint8_t *m = (uint8_t *)dalloc((size_t)o.num_tiles * o.S * pk::kMetaBytes);
-        if (!m) return cudaErrorMemoryAllocation;
         const W4Seg lm[1] = {seg_of(w_.lm_head)};
-        DCK(pk::repack_meta(ctx_, lm, 1, 0, o.IC, m, s));
-        a.lm_meta = m;
-        DCK(pk::encode_kv_tmap(&maps[(size_t)Lyr * 7 + 1], d_kv_.get(), (long long)Lyr * 2 * per_kv));
+        for (int set = 0; set < nsets; set++) {
+            const pk::KRange kr = pk::k_range(o.NG, set > 0, set - 1);
+            DCK(encode_w4_tmap_units(&maps[set * nmaps + (size_t)Lyr * 7], w_.lm_head.w, w_.lm_head.oc, w_.lm_head.ic, kr.bw, 16, kr.g0, kr.ng));
+            uint8_t *m = (uint8_t *)dalloc((size_t)o.num_tiles * kr.nb * pk::kBoxMetaBytes);
+            if (!m) return cudaErrorMemoryAllocation;
+            DCK(pk::repack_meta(ctx_, lm, 1, 0, o.IC, kr, m, s));
+            a.lm_meta[set] = m;
+            DCK(pk::encode_kv_tmap(&maps[set * nmaps + (size_t)Lyr * 7 + 1], d_kv_.get(), (long long)Lyr * 2 * per_kv));
+        }
     }
     CUtensorMap *dmaps = (CUtensorMap *)dalloc(maps.size() * sizeof(CUtensorMap));
     pk::LayerDesc *ddesc = (pk::LayerDesc *)dalloc(descs.size() * sizeof(pk::LayerDesc));
@@ -308,7 +319,6 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
     a.eps = cfg_.rms_eps;
     a.H = H;
     a.KVH = KVH;
-    a.nrep = nrep;
     a.max_ctx = cfg_.max_ctx;
     a.V = V;
     a.F = F;
@@ -336,9 +346,6 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         DCK(cudaMemset(a.dbg, 0, n));
     }
     if ((int)pk::smem_bytes(a) > ctx_->smem_optin) return no("shared memory");
-    // pair staging (clusters of two CTAs share the activation staging over DSMEM): on unless switched off or the device cannot co-schedule
-    // num_sms / 2 such clusters
-    a.pair = (!getenv("TCE_PK_PAIR") || atoi(getenv("TCE_PK_PAIR")) != 0) && pk::pair_supported(ctx_, a) ? 1 : 0;
     pargs_ = a;
     return cudaSuccess;
 }

@@ -9,20 +9,11 @@ namespace gemv {
 
 constexpr float kActQ = 2130706432.f;  // 127 * 2^24: activation fixed-point full scale (four balanced base-256 digits = int8 planes)
 
-// Mirror of a unit into the partner CTA of a cluster (persistent decode kernel, pair staging): shared::cluster addresses of the partner's
-// plane buffer, group steps / sums and of the mbarrier that counts the bytes it receives (st.async completes them as transactions).
-struct PairDst {
-    uint32_t xs, gx, gsum, bar;
-};
-TCE_DEVINL void st_async_b32(uint32_t raddr, uint32_t v, uint32_t rbar) {
-    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(raddr), "r"(v), "r"(rbar) : "memory");
-}
-
 // quantise + stage one 8-element unit (v) of one activation column: xcol = the column's plane buffer (IC = its width in elements; region B
 // starts at byte IC * 2), gx / gsum = the column's per-group step and integer sums.  Must be called by all 32 lanes of a warp (half-warp
 // shuffles); `valid` masks the stores.
-template <int NCOLS, bool PAIR = false>
-TCE_DEVINL void emit_unit(uint8_t *xcol, int IC, float *gx, int *gsum, int ui, bool valid, const float (&v)[8], int lane, const PairDst *pd = nullptr) {
+template <int NCOLS>
+TCE_DEVINL void emit_unit(uint8_t *xcol, int IC, float *gx, int *gsum, int ui, bool valid, const float (&v)[8], int lane) {
     // Activations enter the integer tensor path as 32-bit block fixed point: per 128-group,
     // X = rint(x * Q / max|x|), Q = 127 * 2^24, X = 2^24*p3 + 2^16*p2 + 2^8*p1 + p0  (four int8 planes = the balanced base-256 digits of
     // X, p3 in [-127,127], the others in [-128,127]).  |x - step*X| <= max(|x| * 2^-24, max|x_group| * 2^-32): every fp16 activation whose
@@ -76,17 +67,6 @@ TCE_DEVINL void emit_unit(uint8_t *xcol, int IC, float *gx, int *gsum, int ui, b
             dl[4] = o0e;
             dl[32] = o1o;
             dl[36] = o0o;
-            if (PAIR) {  // the same eight words into the partner's buffer
-                const uint32_t ra = pd->xs + (uint32_t)G * 256u + (uint32_t)(tj >> 2) * 32u + (uint32_t)(tj & 3) * 4u, rb = ra + (uint32_t)IC * 2u;
-                st_async_b32(ra, o3e, pd->bar);
-                st_async_b32(ra + 16u, o2e, pd->bar);
-                st_async_b32(ra + 128u, o3o, pd->bar);
-                st_async_b32(ra + 144u, o2o, pd->bar);
-                st_async_b32(rb, o1e, pd->bar);
-                st_async_b32(rb + 16u, o0e, pd->bar);
-                st_async_b32(rb + 128u, o1o, pd->bar);
-                st_async_b32(rb + 144u, o0o, pd->bar);
-            }
         }
     } else {
         // units of a group are stored j-major so that the four t-lanes of one LDS.128 hit consecutive slots
@@ -103,11 +83,6 @@ TCE_DEVINL void emit_unit(uint8_t *xcol, int IC, float *gx, int *gsum, int ui, b
         gx[G] = step;              // step of the group
         gsum[G * 2] = sxh;         // 256 * sum(p3) + sum(p2) over the group
         gsum[G * 2 + 1] = sxl;     // 256 * sum(p1) + sum(p0)
-        if (PAIR) {
-            st_async_b32(pd->gx + (uint32_t)G * 4u, __float_as_uint(step), pd->bar);
-            st_async_b32(pd->gsum + (uint32_t)G * 8u, (uint32_t)sxh, pd->bar);
-            st_async_b32(pd->gsum + (uint32_t)G * 8u + 4u, (uint32_t)sxl, pd->bar);
-        }
     }
 }
 

@@ -165,10 +165,11 @@ cudaError_t encode_w4_tmap(CUtensorMap *out, const void *w, int rows, int IC, in
 
 // 3-D view [group][row][64 B] of the same matrix: a box {64 B, box_rows, sg groups} lands in shared memory group-major with the rows of a group 64 B apart,
 // so the 16 rows x 64 B of one (tile, group) unit are 1 KiB contiguous and a quarter-warp's LDS.128 covers 128 consecutive bytes (no bank conflicts)
-cudaError_t encode_w4_tmap_units(CUtensorMap *out, const void *w, int rows, int IC, int sg, int box_rows) {
+cudaError_t encode_w4_tmap_units(CUtensorMap *out, const void *w, int rows, int IC, int sg, int box_rows, int g0, int ng) {
     const TmapEncodeFn fn = tmap_encoder();
     if (!fn) return cudaErrorNotSupported;
-    const cuuint64_t gdim[3] = {16, (cuuint64_t)rows, (cuuint64_t)(IC / 128)};
+    w = static_cast<const uint8_t *>(w) + (size_t)g0 * 64;  // a group is 64 B of a row
+    const cuuint64_t gdim[3] = {16, (cuuint64_t)rows, (cuuint64_t)(ng ? ng : IC / 128)};
     const cuuint64_t gstride[2] = {(cuuint64_t)(IC / 2), 64};
     const cuuint32_t box[3] = {16, (cuuint32_t)box_rows, (cuuint32_t)sg};
     const cuuint32_t estr[3] = {1, 1, 1};
