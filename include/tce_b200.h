@@ -373,9 +373,10 @@ TCE_API int tce_llama_kernels_per_step(tce_llama *m);
  * (float[vocab_local]) and the GLOBAL greedy token; all ranks must call it with the same token/pos sequence.   */
 TCE_API int tce_llama_tp_handle(tce_llama *m, void *handle_out_64_bytes);
 TCE_API int tce_llama_tp_connect(tce_llama *m, const void *handles_P_times_64_bytes);
-/* debugging aid: device pointers of row 0 of the kernel-per-op step's intermediate buffers: 0 residual float[E], 1 qkv half[(H+2KVH)*hd],
- * 2 attention output half[H*hd], 3 SiLU(gate)*up half[F] (values of the LAST layer after a step); NULL until those buffers exist (the
- * persistent kernel keeps its intermediates on chip).  4: the persistent kernel's phase timestamps (TCE_PK_DEBUG=1). */
+/* debugging aid: device pointers of the batched step's intermediate buffers, TCE_LLAMA_MAX_BATCH rows each (row b = request b of the last
+ * batched or span step; the kernel-per-op single-sequence step, TCE_PERSISTENT=0, writes row 0): 0 residual float[E], 1 qkv
+ * half[(H+2KVH)*hd], 2 attention output half[H*hd], 3 SiLU(gate)*up half[F] (values of the LAST layer after a step); NULL until those
+ * buffers exist (the persistent kernel keeps its intermediates on chip).  4: the persistent kernel's phase timestamps (TCE_PK_DEBUG=1). */
 TCE_API void *tce_llama_debug_buffer(tce_llama *m, int which);
 /* measurement aid: enqueue only the W4A16 GEMV launches of one decode step (4 per layer + lm_head, the same fused
  * kernels with the same arguments) so the dominant kernel can be timed with CUDA events; returns the launch count */

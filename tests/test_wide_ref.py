@@ -53,6 +53,31 @@ def test_gqa_causal_attention_matches_oracle(H, KVH, n, pos0):
     assert err <= 1e-5
 
 
+@pytest.mark.parametrize("H,KVH", [(8, 2), (4, 4), (8, 1)])
+@pytest.mark.parametrize("n,pos0", [(1, 0), (8, 0), (5, 30)])
+def test_span_rows_decode_attention_matches_oracle(H, KVH, n, pos0):
+    """The span step's attention reference of tests/test_gpu_decode_wide.py: row i is decode_attention of its rotated, scaled query over
+    the cached rows and the span's rows 0..i, against capi.llama_attention_core under the causal mask of n rows after pos0."""
+    rng = np.random.default_rng(200 * H + 10 * KVH + n + pos0)
+    cosb, sinb = capi.rope_tables(128, HD, 10000.0)
+    q = rng.standard_normal((n, H * HD)).astype(np.float16).astype(np.float32)
+    k = rng.standard_normal((n, KVH * HD)).astype(np.float16).astype(np.float32)
+    v = rng.standard_normal((n, KVH * HD)).astype(np.float16).astype(np.float32)
+    pk = (rng.standard_normal((KVH, pos0, HD)) * 0.7).astype(np.float16)
+    pv = rng.standard_normal((KVH, pos0, HD)).astype(np.float16)
+    alpha = 1.0 / np.sqrt(HD)
+    want, _, _ = capi.llama_attention_core(q, k, v, pk.astype(np.float32) if pos0 else None, pv.astype(np.float32) if pos0 else None,
+                                           capi.causal_mask(n, pos0), cosb, sinb, alpha, H, KVH, HD)
+    c, s = torch.from_numpy(cosb[pos0:pos0 + n]), torch.from_numpy(sinb[pos0:pos0 + n])
+    qa = wide_ref.rope(torch.from_numpy(q).reshape(n, H, HD), c, s) * alpha
+    K = torch.cat([torch.from_numpy(pk).double(), wide_ref.rope(torch.from_numpy(k).reshape(n, KVH, HD), c, s).transpose(0, 1)], dim=1)
+    V = torch.cat([torch.from_numpy(pv).double(), torch.from_numpy(v).double().reshape(n, KVH, HD).transpose(0, 1)], dim=1)
+    got = torch.stack([wide_ref.decode_attention(qa[i], K[:, :pos0 + i + 1], V[:, :pos0 + i + 1])[0].reshape(-1) for i in range(n)])
+    err = wide_ref.row_rel_err(got, torch.from_numpy(want).double()).max().item()
+    print(f"[wide_ref span rows H={H} KVH={KVH} n={n} pos0={pos0}] worst row rel err {err:.2e}")
+    assert err <= 1e-5
+
+
 @pytest.mark.parametrize("geom", ["tiny-mha", "tiny-gqa"])
 def test_prompt_pass_matches_llama_forward(geom):
     """prompt_pass (rotated q/k unrounded) against llama_forward with the fp32 product of the fp16-expanded weights as its linear and fp16 as

@@ -111,7 +111,7 @@ class LlamaDecoder {
     // host-checked, then one launch on the context's stream (tce_llama_kv_copy)
     cudaError_t kv_copy(int src_slot, int src_pos, int n, int n_dst, const int *dst_slots, const int *dst_pos, std::string *err);
     int kernels_per_step() const { return persistent_ ? 1 : 1 + 5 * cfg_.num_layers + 2; }
-    // 0..3: row 0 of the kernel-per-op step's buffers (null until they exist)
+    // 0..3: the batched step's buffers, TCE_LLAMA_MAX_BATCH rows each (null until they exist)
     void *debug_buffer(int which) const {
         switch (which) {
             case 0: return bs_ ? bs_->resid.get() : nullptr;

@@ -532,14 +532,16 @@ class LlamaModel:
         return _tensor_from_ptr(ptr, (self.geom.num_kv_heads, self.max_ctx, self.geom.head_dim), torch.float16, self.ctx.device)
 
     def debug_buffer(self, which: int) -> torch.Tensor:
-        """0..3: row 0 of the kernel-per-op step's residual, q|k|v, attention output and SiLU*up; 5: the persistent kernel's hand-off
-        words as int32 [n, 2] {payload, tag} (cut into its vectors by handoff_views)."""
+        """0..3: the batched step's residual (float32 [MAX_BATCH, E]), q|k|v, attention output and SiLU*up (float16 [MAX_BATCH, ...]),
+        row b = request b of the last batched or span step; 5: the persistent kernel's hand-off words as int32 [n, 2] {payload, tag} (cut
+        into its vectors by handoff_views)."""
         g = self.geom
+        B = self.MAX_BATCH
         if which == 5:
             shape, dt = (sum(self._handoff_words().values()), 2), torch.int32
         else:
-            shape, dt = {0: ((g.embed_dim,), torch.float32), 1: (((g.num_heads + 2 * g.num_kv_heads) * g.head_dim,), torch.float16),
-                         2: ((g.num_heads * g.head_dim,), torch.float16), 3: ((g.hidden_dim,), torch.float16)}[which]
+            shape, dt = {0: ((B, g.embed_dim), torch.float32), 1: ((B, (g.num_heads + 2 * g.num_kv_heads) * g.head_dim), torch.float16),
+                         2: ((B, g.num_heads * g.head_dim), torch.float16), 3: ((B, g.hidden_dim), torch.float16)}[which]
         ptr = self.ctx.L.tce_llama_debug_buffer(self.h, which)
         if not ptr:
             raise _lib.TceError(f"debug buffer {which}: " + ("this model has no persistent kernel" if which == 5 else
