@@ -100,7 +100,7 @@ def pick_positions(ncta: int, KVH: int, max_ctx: int) -> list:
 # ------------------------------------------------------------------------------------------------ models and their float64 weights
 
 class Wide:
-    """A 1-layer model at a benchmarked geometry: its weights expanded to float64 once, and one LlamaModel per staging mode."""
+    """A 1-layer model at a benchmarked geometry: its weights expanded to float64 once, and one LlamaModel per decode path."""
 
     def __init__(self, ctx, widths: str, max_ctx: int):
         import dataclasses
@@ -140,9 +140,11 @@ class Wide:
                         os.environ[k] = v
         return self.models[key]
 
-    def model(self, pair: bool):
-        """The persistent kernel, with CTA-pair staging or without (TCE_PK_PAIR=0)."""
-        return self._build(pair, {"TCE_PERSISTENT": "1", "TCE_PK_PAIR": None if pair else "0"})
+    def model(self):
+        """The persistent kernel."""
+        m = self._build("persistent", {"TCE_PERSISTENT": "1"})
+        assert m.kernels_per_step == 1
+        return m
 
     def step_model(self, deterministic: bool, zero_down: bool = False):
         """The kernel-per-op step (TCE_PERSISTENT=0) with every KV-cache slot, its o_proj / down_proj partials added by RED.ADD or, with
@@ -315,11 +317,11 @@ def _attention_check(tag, w, qkv16, positions, kc, vc, got, units, kind, plan, c
     return worst, power, cpow, top
 
 
-def _phase_case(w, pos, pair, tok=4321, seed=0):
+def _phase_case(w, pos, tok=4321, seed=0):
     g = w.g
     H, KVH = g.num_heads, g.num_kv_heads
-    model = w.model(pair)
-    tag = f"{g.name} max_ctx={w.max_ctx} pos={pos} {'pair' if pair else 'pair0'}"
+    model = w.model()
+    tag = f"{g.name} max_ctx={w.max_ctx} pos={pos}"
     _fill_cache(model, pos, seed=pos + 1 + seed)
     kc, vc = model.kv_cache(0, 0), model.kv_cache(0, 1)
     before = (_bits(kc), _bits(vc))
@@ -416,17 +418,16 @@ def _phase_case(w, pos, pair, tok=4321, seed=0):
 
 
 def _phase_cases():
-    """(widths, max_ctx, pair, position index or an explicit position): pair staging at every position of the plan, single-CTA staging
-    at a subset; max_ctx 4000 (not a multiple of 64) at its last rows."""
-    out = [pytest.param("llama3-8b", 4096, True, i, id=f"llama3-8b-pair-{i}") for i in range(10)]
-    out += [pytest.param("llama3-8b", 4096, False, i, id=f"llama3-8b-pair0-{i}") for i in (1, 4, 8)]
-    out += [pytest.param("llama2-7b", 4096, True, i, id=f"llama2-7b-pair-{i}") for i in range(10)]
-    out += [pytest.param("llama3-8b", 4000, True, p, id=f"llama3-8b-ctx4000-last{-p}") for p in (-1, -32)]
+    """(widths, max_ctx, position index or an explicit position): every position of the plan; max_ctx 4000 (not a multiple of 64) at its
+    last rows.  "pair" in an id: the kernel runs on clusters of two CTAs."""
+    out = [pytest.param("llama3-8b", 4096, i, id=f"llama3-8b-pair-{i}") for i in range(10)]
+    out += [pytest.param("llama2-7b", 4096, i, id=f"llama2-7b-pair-{i}") for i in range(10)]
+    out += [pytest.param("llama3-8b", 4000, p, id=f"llama3-8b-ctx4000-last{-p}") for p in (-1, -32)]
     return out
 
 
-@pytest.mark.parametrize("widths,max_ctx,pair,which", _phase_cases())
-def test_persistent_step_phases(wide, widths, max_ctx, pair, which):
+@pytest.mark.parametrize("widths,max_ctx,which", _phase_cases())
+def test_persistent_step_phases(wide, widths, max_ctx, which):
     """One step of a 1-layer model at Llama-3-8B (GQA 32:8, full vocabulary) or Llama-2-7B (MHA) widths on a cache that is random below
     the token and NaN from it on: every phase against float64 from its own inputs (see the module docstring).  `which` indexes the
     positions of pick_positions at this device's SM count, or (negative) counts back from max_ctx."""
@@ -438,7 +439,7 @@ def test_persistent_step_phases(wide, widths, max_ctx, pair, which):
         if which >= len(positions):
             pytest.skip(f"{len(positions)} positions at this SM count")
         pos = positions[which]
-    _phase_case(w, pos, pair)
+    _phase_case(w, pos)
 
 
 @pytest.mark.parametrize("widths", ["llama3-8b", "llama2-7b"])
@@ -921,6 +922,7 @@ def test_two_layer_steps_across_boundaries(widths, mega, monkeypatch):
     g = dataclasses.replace(GEOMETRIES[widths], name=f"{widths}-2l", num_layers=2)
     ctx = Context(0)
     model = LlamaModel(ctx, g, max_ctx=4096, seed=23, random_zeros=True)
+    assert (model.kernels_per_step == 1) == (mega == "1")
     cosb, sinb = capi.rope_tables(4096, HD, g.rope_theta)
     lg = torch.empty(g.vocab_size, dtype=torch.float32).pin_memory()
     worst = {"logits": 0.0, "kv layer0 ulps": 0.0, "kv layer1": 0.0, "decode vs decode_host": 0.0}

@@ -21,6 +21,7 @@ def _run(monkeypatch, graphs, script, persistent="1"):
         monkeypatch.setenv("TCE_NO_GRAPH", "1")
     ctx = Context(0)
     model = LlamaModel(ctx, GEOMETRIES["tiny-gqa"], max_ctx=128, seed=13, random_zeros=True)
+    assert (model.kernels_per_step == 1) == (persistent == "1")
     try:
         out, slots = script(ctx, model)
         torch.cuda.synchronize()

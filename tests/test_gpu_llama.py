@@ -1,4 +1,6 @@
 """Fused decode step (tce_llama_*: one persistent kernel per token, or one kernel per op inside a CUDA graph) vs the oracle-composed step."""
+import dataclasses
+
 import numpy as np
 import pytest
 import torch
@@ -8,23 +10,23 @@ from helpers import oracle_decode_step, rel_err
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("mega,pair", [("1", None), ("0", None), ("1", "0")], ids=["1", "0", "1-pair0"])
-@pytest.mark.parametrize("geom", ["tiny-gqa", "tiny-mha"])
-def test_decode_steps_match_oracle(geom, mega, pair, monkeypatch):
-    """mega=1: one persistent cooperative kernel per token (the default), with pair staging (clusters of two CTAs) where the device
-    allows it, or with TCE_PK_PAIR=0 single-CTA staging (what a refused cluster launch falls back to); mega=0: one kernel per op
-    inside a CUDA graph."""
+@pytest.mark.parametrize("mega", ["1", "0"])
+@pytest.mark.parametrize("geom", ["tiny-gqa", "tiny-mha", "e128"])
+def test_decode_steps_match_oracle(geom, mega, monkeypatch):
+    """mega=1: one persistent kernel per token (the default); mega=0: one kernel per op inside a CUDA graph.  e128 (embed_dim 128,
+    one layer) has a single 128-group in q|k|v, gate|up and lm_head, nothing to split across the two CTAs of a cluster: it is outside
+    the persistent kernel's envelope and runs one kernel per op either way."""
     monkeypatch.setenv("TCE_PERSISTENT", mega)
-    if pair is None:
-        monkeypatch.delenv("TCE_PK_PAIR", raising=False)
-    else:
-        monkeypatch.setenv("TCE_PK_PAIR", pair)
     from tinychatengine_b200.llama import GEOMETRIES, LlamaModel
     from tinychatengine_b200.runtime import Context
 
     ctx = Context(0)
-    g = GEOMETRIES[geom]
+    if geom == "e128":
+        g = dataclasses.replace(GEOMETRIES["tiny-gqa"], name="e128", num_layers=1, num_heads=1, num_kv_heads=1, embed_dim=128, hidden_dim=384)
+    else:
+        g = GEOMETRIES[geom]
     model = LlamaModel(ctx, g, max_ctx=256, seed=7, random_zeros=True)
+    assert (model.kernels_per_step == 1) == (mega == "1" and geom != "e128")
     past_k = [None] * g.num_layers
     past_v = [None] * g.num_layers
     tokens = [3, 77, 1000, 5, 900, 17, 256, 999]
@@ -86,6 +88,7 @@ def test_persistent_kernel_long_context_matches_graph_path(monkeypatch):
         monkeypatch.setenv("TCE_PERSISTENT", mega)
         ctx = Context(0)
         model = LlamaModel(ctx, g, max_ctx=256, seed=11)
+        assert (model.kernels_per_step == 1) == (mega == "1")
         lg = torch.empty(g.vocab_size, dtype=torch.float32)
         seq = []
         tok = 5
@@ -112,6 +115,7 @@ def test_persistent_kernel_is_deterministic_when_asked(monkeypatch):
     for _ in range(2):
         ctx = Context(0)
         model = LlamaModel(ctx, GEOMETRIES["tiny-gqa"], max_ctx=128, seed=3)
+        assert model.kernels_per_step == 1
         lg = torch.empty(model.geom.vocab_size, dtype=torch.float32)
         seq = []
         for pos, tok in enumerate([1, 2, 3, 4, 5, 6]):
@@ -141,6 +145,7 @@ def test_benchmarked_geometry_step_matches_oracle(widths, pos, mega, monkeypatch
     g = dataclasses.replace(GEOMETRIES[widths], name=f"{widths}-2l", num_layers=2)
     ctx = Context(0)
     model = LlamaModel(ctx, g, max_ctx=4096, seed=21, random_zeros=True)
+    assert (model.kernels_per_step == 1) == (mega == "1")
     gen = torch.Generator(device="cuda")
     gen.manual_seed(pos + 1)
     past_k, past_v = [], []
@@ -227,6 +232,7 @@ def test_device_resident_token_and_position_are_range_checked(mega, monkeypatch)
     g = GEOMETRIES["tiny-gqa"]
     a = LlamaModel(ctx, g, max_ctx=32, seed=4)
     b = LlamaModel(ctx, g, max_ctx=32, seed=4)
+    assert (a.kernels_per_step == 1) == (mega == "1")
     la, lb = torch.empty(g.vocab_size), torch.empty(g.vocab_size)
     assert a.decode_host(5, 0, la) == b.decode_host(5, 0, lb)
     kv_before = [a.kv_cache(l, w).clone() for l in range(g.num_layers) for w in (0, 1)]

@@ -1,6 +1,6 @@
 """Attention inside the persistent decode kernel at single positions on a random-filled cache: with one attention split per KV head
 (every visible key in one CTA) and with several (flash-decode partials merged across CTAs), the token's key and value landing at
-the start, inside and at the end of a 64-key chunk, with pair staging where the device allows it and with TCE_PK_PAIR=0."""
+the start, inside and at the end of a 64-key chunk."""
 import numpy as np
 import pytest
 import torch
@@ -14,21 +14,17 @@ pytestmark = pytest.mark.gpu
 POSITIONS = [0, 37, 63, 64, 130, 1000, 2047]
 
 
-@pytest.mark.parametrize("pair", [None, "0"], ids=["pair", "pair0"])
-@pytest.mark.parametrize("pos", POSITIONS)
+@pytest.mark.parametrize("pos", POSITIONS, ids=lambda pos: f"{pos}-pair")  # "pair": the kernel runs on clusters of two CTAs
 @pytest.mark.parametrize("geom", ["tiny-gqa", "tiny-mha"])
-def test_persistent_attention_step_matches_oracle(geom, pos, pair, monkeypatch):
+def test_persistent_attention_step_matches_oracle(geom, pos, monkeypatch):
     monkeypatch.setenv("TCE_PERSISTENT", "1")
-    if pair is None:
-        monkeypatch.delenv("TCE_PK_PAIR", raising=False)
-    else:
-        monkeypatch.setenv("TCE_PK_PAIR", pair)
     from tinychatengine_b200.llama import GEOMETRIES, LlamaModel
     from tinychatengine_b200.runtime import Context
 
     g = GEOMETRIES[geom]
     ctx = Context(0)
     model = LlamaModel(ctx, g, max_ctx=2048, seed=13, random_zeros=True)
+    assert model.kernels_per_step == 1
     gen = torch.Generator(device="cuda")
     gen.manual_seed(pos + 7)
     past_k, past_v = [], []

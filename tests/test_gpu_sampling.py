@@ -147,6 +147,7 @@ def test_generate_kv_rows(ctx, monkeypatch, persistent):
     monkeypatch.setenv("TCE_DETERMINISTIC", "1")
     g = GEOMETRIES["tiny-gqa"]
     model = LlamaModel(ctx, g, max_ctx=128, seed=3)
+    assert (model.kernels_per_step == 1) == (persistent == "1")
     gen = torch.Generator(device="cuda")
     gen.manual_seed(5)
     caches = [model.kv_cache(l, w) for l in range(g.num_layers) for w in (0, 1)]

@@ -1,9 +1,10 @@
-// decode_persistent.cu -- one persistent cooperative kernel per decoded token (Llama, AWQ-INT4, batch 1) on sm_90a.
+// decode_persistent.cu -- one persistent kernel per decoded token (Llama, AWQ-INT4, batch 1) on sm_90a, launched as clusters of two CTAs.
 //
 // Call sites restated (reference, CUDA build): Int4LlamaForCausalLM::forward (cuda/Int4llamaForCausalLM.cu:17-50) ->
 // Int4llamaDecoder::forward (cuda/Int4llamaDecoder.cu:57-112) -> 32 x Int4llamaDecoderLayer::forward (cuda/Int4llamaDecoderLayer.cu:73-115)
 // -> Int4llamaAttention::forward (cuda/Int4llamaAttention.cu:116-229): ~19 kernels + 128 memcpys per layer on stream 0.  Here the whole
-// token is ONE kernel of one CTA per SM whose warp roles persist across all phases (5 per layer + lm_head):
+// token is ONE kernel of one CTA per SM whose warp roles persist across all phases (5 per layer + lm_head).  The two CTAs of a cluster
+// walk the same GEMV tiles, each over its half of K (see KRange):
 //
 //   producer (1 warp, 1 elected lane)  walks the phases in order and keeps a ring of `nst` TMA stages full.  A stage is either
 //        [16 rows x <=32 groups] of packed int4 weights (one or two 3-D UTMALDG boxes of 16 groups through the [group][row][64 B] view,
@@ -13,8 +14,8 @@
 //   consumers (16 warps)  per phase: spin on the flag-carrying words of their input vector, quantise it (fused RMSNorm, four int8 planes
 //        per 128-group), run the integer-MMA GEMV over this CTA's tiles (two 128-k groups per warp and stage), or run flash-decoding
 //        attention straight out of the ring stages (mma.sync m16n8k16, ldmatrix on the swizzled K/V rows).
-//   epilogue (1 warp)  reduces the 16 consumer partials of every tile and publishes the results as {value, phase tag} words.  In pair mode
-//        (clusters of two CTAs that split K) one CTA per tile first adds its partner's row sums.
+//   epilogue (1 warp)  reduces the 16 consumer partials of every tile and publishes the results as {value, phase tag} words; one CTA of
+//        the cluster per tile first adds its partner's row sums.
 //
 // There is NO grid barrier between phases.  Every vector that crosses CTAs (q|k|v, attention partials and outputs, SiLU*mul
 // activations, the o_proj / down_proj outputs) is an array of 8-byte words {payload, tag} written with one 8-byte store and read with
@@ -165,7 +166,7 @@ TCE_DEVINL unsigned long long argmax_key(float v, int idx) {
 struct PSmem {
     uint8_t *ring;      // [nst][kStageBytes], 1024-B aligned
     uint8_t *xs;        // activation planes (4 bytes per input channel of the CTA's K range) | attention scratch
-    float *resid;       // this CTA's copy of the fp32 residual stream: all E channels, or in pair mode the channels of its K range
+    float *resid;       // this CTA's copy of the fp32 residual stream: the channels of its K range
     float *gx;          // [max_ng] group steps
     int *gsum;          // [max_ng][2] group sums
     float *red;         // [kRedBufs][kCW][16] tile partials
@@ -173,17 +174,17 @@ struct PSmem {
     float *inv;         // [kCW] each consumer warp's 1/rms of the current phase (see hand_tile)
     float *rope;        // cos[128] | sin[128] of the token position
     uint64_t *full, *empty, *red_full, *red_empty;
-    uint64_t *rx;       // pair mode: counts the bytes of the partner's 16 partial sums of squares (RMSNorm)
-    float *prx;         // pair mode: [kPairSlots][16] tile row sums received from the partner
-    uint64_t *prx_full; // [kPairSlots] pair mode: completed by the partner's st.async of a slot of `prx`
-    uint64_t *pfree;    // [kPairSlots] pair mode: arrived on by the partner once it has read the row sums this CTA sent into its slot
+    uint64_t *rx;       // counts the bytes of the partner's 16 partial sums of squares (RMSNorm)
+    float *prx;         // [kPairSlots][16] tile row sums received from the partner
+    uint64_t *prx_full; // [kPairSlots] completed by the partner's st.async of a slot of `prx`
+    uint64_t *pfree;    // [kPairSlots] arrived on by the partner once it has read the row sums this CTA sent into its slot
     int2 *red_pos;      // [kCW] each consumer warp's position in the red-buffer ring between GEMV phases (see consume_gemv)
     uint32_t ring_u32, xs_u32, gx_u32, gsum_u32, full_u32, empty_u32, redfull_u32, redempty_u32;
     int nst;
 };
 
-// residual floats a CTA keeps: pair mode the channels of its K range of the E-wide RMSNorm ops (the larger half: rank 0)
-__host__ __device__ inline int resid_floats(const Args &a) { return a.pair ? plane_ic(a.E / kW4Group, 1) : a.E; }
+// residual floats a CTA keeps: the channels of its K range of the E-wide RMSNorm ops (the larger half: rank 0)
+__host__ __device__ inline int resid_floats(const Args &a) { return plane_ic(a.E / kW4Group); }
 
 TCE_DEVINL PSmem carve(uint8_t *raw, const Args &a) {
     PSmem s;
@@ -249,13 +250,11 @@ struct Red {
     }
 };
 
-// this CTA's tile range of one GEMV op: cut at tile boundaries (every output has exactly one writer).  Pair mode: both CTAs of a cluster
-// (CTAs 2i, 2i + 1) walk the range of pair i, each over its own K range.
-TCE_DEVINL void partition(const GemvOp &op, int cta, int ncta, int pair, int &t0, int &t1) {
-    if (pair) {
-        cta >>= 1;
-        ncta >>= 1;
-    }
+// this CTA's tile range of one GEMV op: cut at tile boundaries (every output has exactly one writer).  Both CTAs of a cluster (CTAs 2i,
+// 2i + 1) walk the range of pair i, each over its own K range.
+TCE_DEVINL void partition(const GemvOp &op, int cta, int ncta, int &t0, int &t1) {
+    cta >>= 1;
+    ncta >>= 1;
     const unsigned T = (unsigned)op.num_tiles;
     t0 = (int)((T * (unsigned)cta) / (unsigned)ncta);
     t1 = (int)((T * (unsigned)(cta + 1)) / (unsigned)ncta);
@@ -291,11 +290,11 @@ TCE_DEVINL AttnSplit attn_split(int cta, int ncta, int KVH, int pos) {
 // ------------------------------------------------------------------------------------------------------------ producer
 // one weight stage: the next two boxes of this CTA's (tile, box) walk (see KRange), slot b at b * 16 KiB (gate | up: the up rows 8 KiB into
 // it), and their two scale|zero records, which are adjacent in the repacked array
-TCE_DEVINL void produce_gemv(const GemvOp &op, const CUtensorMap *m0, const uint8_t *meta, const PSmem &sm, Ring &rs, int cta, int ncta, int pair, int rank,
+TCE_DEVINL void produce_gemv(const GemvOp &op, const CUtensorMap *m0, const uint8_t *meta, const PSmem &sm, Ring &rs, int cta, int ncta, int rank,
                              uint32_t leader, uint64_t policy) {
     int t0, t1;
-    partition(op, cta, ncta, pair, t0, t1);
-    const KRange kr = k_range(op.NG, pair, rank);
+    partition(op, cta, ncta, t0, t1);
+    const KRange kr = k_range(op.NG, rank);
     const uint32_t box_bytes = 16u * (uint32_t)kr.bw * 64u;  // 16 rows (gate | up: 8 of each matrix) x bw groups x 64 B
     const int nbox = (t1 - t0) * kr.nb;
     const uint8_t *rec = meta + (size_t)t0 * kr.nb * kBoxMetaBytes;
@@ -309,9 +308,9 @@ TCE_DEVINL void produce_gemv(const GemvOp &op, const CUtensorMap *m0, const uint
 #pragma unroll 1
         for (int b = 0; b < n; b++) {
             // the tile's matrix (q|k|v: tiles never straddle two segments; gate | up: the gate map, the up map follows it) and first row
-            int row = op.pair ? tile * 8 : tile * 16;
+            int row = op.gate_up ? tile * 8 : tile * 16;
             const CUtensorMap *m = m0;
-            if (!op.pair && op.nseg > 1 && row >= op.rows0) {
+            if (!op.gate_up && op.nseg > 1 && row >= op.rows0) {
                 row -= op.rows0;
                 m = m0 + 1;
                 if (op.nseg > 2 && row >= op.rows1) {
@@ -320,7 +319,7 @@ TCE_DEVINL void produce_gemv(const GemvOp &op, const CUtensorMap *m0, const uint
                 }
             }
             tma_load_3d_pred(dst + b * 16384, m, 0, row, box * kBoxGroups, bar, policy, leader);
-            if (op.pair) tma_load_3d_pred(dst + b * 16384 + 8192, m + 1, 0, row, box * kBoxGroups, bar, policy, leader);
+            if (op.gate_up) tma_load_3d_pred(dst + b * 16384 + 8192, m + 1, 0, row, box * kBoxGroups, bar, policy, leader);
             if (++box == kr.nb) {
                 box = 0;
                 tile++;
@@ -356,34 +355,31 @@ TCE_DEVINL void producer_walk(const Args &a, const PSmem &sm, int cta, int ncta,
     const uint64_t policy = l2_policy_evict_first();
     const uint32_t leader = (lane == 0) ? 1u : 0u;
     const int Lyr = a.num_layers, nphase = 5 * Lyr + 1;
-    const CUtensorMap *kvmap = a.maps + (size_t)Lyr * 7 + 1;
-    const int set = a.pair ? 1 + rank : 0;
-    const CUtensorMap *wmaps = a.maps + (size_t)set * (Lyr * 7 + 2);
+    const CUtensorMap *wmaps = a.maps + (size_t)rank * (Lyr * 7 + 1);
+    const CUtensorMap *kvmap = a.maps + (size_t)2 * (Lyr * 7 + 1);
 #pragma unroll 1
     for (int p = 0; p < nphase; p++) {
         const int l = p / 5, k = p - 5 * l;
         if (l == Lyr) {
-            produce_gemv(a.op[OPI_LMHEAD], wmaps + (size_t)Lyr * 7, a.lm_meta[set], sm, rs, cta, ncta, a.pair, rank, leader, policy);
+            produce_gemv(a.op[OPI_LMHEAD], wmaps + (size_t)Lyr * 7, a.lm_meta[rank], sm, rs, cta, ncta, rank, leader, policy);
         } else if (k == 1) {
             produce_attn(a, a.layers[l], kvmap, sm, rs, cta, ncta, pos, leader, policy);
         } else {
             const int oi = (k == 0) ? OPI_QKV : (k - 1);       // k = 2,3,4 -> OPI_O, OPI_GATEUP, OPI_DOWN
             const int mi = (k == 0) ? 0 : (k == 2 ? 3 : (k == 3 ? 4 : 6));  // first tensor map of the op within the layer's seven
-            produce_gemv(a.op[oi], wmaps + (size_t)l * 7 + mi, a.layers[l].meta[set][oi], sm, rs, cta, ncta, a.pair, rank, leader, policy);
+            produce_gemv(a.op[oi], wmaps + (size_t)l * 7 + mi, a.layers[l].meta[rank][oi], sm, rs, cta, ncta, rank, leader, policy);
         }
     }
 }
 
-// ------------------------------------------------------------------------------------------------------------ pair mode (clusters of two CTAs)
+// ------------------------------------------------------------------------------------------------------------ clusters of two CTAs
 // The two CTAs of a cluster walk the same tiles, CTA `rank` over its K range (k_range): each stages, keeps and reads only its own half of the
 // activation planes and of the residual stream.  What crosses between them goes by st.async (remote shared-memory stores that complete
 // transaction bytes on the receiver's mbarrier: no fence, no flag): the 16 partial sums of squares of an RMSNorm, and the 16 row sums of
 // every tile the partner publishes.
 struct PairCtx {
-    bool on = false;
-    uint32_t rank = 0;
-    uint32_t r_rms = 0, r_bar = 0;  // partner's rms[] and rx barrier
-    uint32_t nstage = 0;            // RMSNorm exchanges so far (parity of the rx barrier)
+    uint32_t rank;
+    uint32_t r_rms, r_bar;  // partner's rms[] and rx barrier
 };
 TCE_DEVINL uint32_t map_to_cta(uint32_t local_u32, uint32_t rank) {
     uint32_t r;
@@ -424,9 +420,9 @@ TCE_DEVINL int rot_unit(int u, int units, int cta) {
 
 // fp16 input vector (attention output / SiLU*mul activations) published as {half2, tag} words -> activation planes of this CTA's K range
 TCE_DEVINL void stage_half(const GemvOp &op, const PSmem &sm, const PairCtx &pc, const uint2 *src, uint32_t tag, int cta, int ctid, int lane) {
-    const KRange kr = k_range(op.NG, pc.on, pc.rank);
+    const KRange kr = k_range(op.NG, pc.rank);
     const int units = kr.ng * 16;  // 8 halfs = 4 words = 32 B per unit
-    const int xic = plane_ic(op.NG, pc.on);
+    const int xic = plane_ic(op.NG);
     constexpr int PRE = 4;        // iterations whose words are requested together: one L2 round trip for up to 4 * 512 units
     for (int ub = 0; ub < units; ub += PRE * kConsumerThreads) {
         uint4 w[PRE][2];
@@ -510,23 +506,23 @@ TCE_DEVINL void tp_accumulate(float (&x)[8], const uint2 *slot0, int tp_size, in
     }
 }
 
-// 1/rms from the `nparts` partial sums of squares of an IC-wide vector
-TCE_DEVINL float rms_inv(const PSmem &sm, int nparts, int IC, float eps) {
+// 1/rms from the 2 x 16 partial sums of squares (both CTAs of the cluster) of an IC-wide vector
+TCE_DEVINL float rms_inv(const PSmem &sm, int IC, float eps) {
     float tot = 0.f;
-    for (int w = 0; w < nparts; w++) tot += sm.rms[w];
+    for (int w = 0; w < 2 * kCW; w++) tot += sm.rms[w];
     return rsqrtf(tot / (float)IC + eps);  // LlamaRMSNorm (llm/src/ops/LlamaRMSNorm.cc): x / sqrt(mean(x^2) + eps) * weight
 }
 
-// fp32 residual stream with fused RMSNorm.  Every CTA holds the stream (pair mode: the channels of its K range) in shared memory; `delta`
-// (o_proj or down_proj outputs of all tensor-parallel ranks, {float, tag} words) is added to it here by every CTA in the same (rank) order.
-// Single-CTA: returns 1/rms (y = inv * W (x . gamma)).  Pair mode: returns once this CTA's 16 partial sums of squares are written; the
-// partner's arrive on the rx barrier, and hand_tile() takes 1/rms from all 32 at a consumer's first tile hand-off.
-TCE_DEVINL float stage_rms(const Args &a, const GemvOp &op, const PSmem &sm, const PairCtx &pc, const uint2 *delta, uint32_t tag, const float *gamma, int token,
-                           bool first, bool emit, int cta, int ctid, int cw, int lane) {
-    const KRange kr = k_range(op.NG, pc.on, pc.rank);
+// fp32 residual stream with fused RMSNorm.  Every CTA holds the channels of its K range of the stream in shared memory; `delta` (o_proj or
+// down_proj outputs of all tensor-parallel ranks, {float, tag} words) is added to it here by every CTA in the same (rank) order.  Returns
+// once this CTA's 16 partial sums of squares are written here and sent to the partner; the partner's arrive on the rx barrier, and
+// hand_tile() takes 1/rms (y = inv * W (x . gamma)) from all 32 at a consumer's first tile hand-off.
+TCE_DEVINL void stage_rms(const Args &a, const GemvOp &op, const PSmem &sm, const PairCtx &pc, const uint2 *delta, uint32_t tag, const float *gamma, int token,
+                          bool first, bool emit, int cta, int ctid, int cw, int lane) {
+    const KRange kr = k_range(op.NG, pc.rank);
     const int units = kr.ng * 16;
-    const int xic = plane_ic(op.NG, pc.on);
-    if (pc.on && emit && ctid == 0)
+    const int xic = plane_ic(op.NG);
+    if (emit && ctid == 0)
         asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(sm.rx)), "r"((uint32_t)kCW * 4u) : "memory");  // the partner's 16 sums
     float ss = 0.f;
     for (int ui0 = 0; ui0 < units; ui0 += kConsumerThreads) {  // warp-uniform trip count
@@ -578,15 +574,14 @@ TCE_DEVINL float stage_rms(const Args &a, const GemvOp &op, const PSmem &sm, con
             gemv::emit_unit<1>(sm.xs, xic, sm.gx, sm.gsum, ui, valid, v, lane);
         }
     }
-    if (!emit) return 1.f;
+    if (!emit) return;
     ss = warp_sum(ss);
     // partial sums of squares: slot (rank, warp) on both CTAs of a pair, so that both add them in the same order
     if (lane == 0) {
         sm.rms[pc.rank * kCW + cw] = ss;
-        if (pc.on) st_async_b32(pc.r_rms + (uint32_t)(pc.rank * kCW + cw) * 4u, __float_as_uint(ss), pc.r_bar);
+        st_async_b32(pc.r_rms + (uint32_t)(pc.rank * kCW + cw) * 4u, __float_as_uint(ss), pc.r_bar);
     }
     named_bar_sync(1, kConsumerThreads);
-    return pc.on ? 0.f : rms_inv(sm, kCW, op.IC, a.eps);
 }
 
 // ------------------------------------------------------------------------------------------------------------ consumers: GEMV
@@ -617,14 +612,14 @@ TCE_DEVINL void unit_compute(const UnitRegs &u, uint32_t st_addr, float lscale, 
 }
 
 // Hand one tile's row sums of this warp, times 1/rms, to the epilogue warp (red buffer `cs`).  1/rms is the warp's word sm.inv[cw]; a
-// negative word -1 - parity (pair mode, RMSNorm phase, first tile) means: wait for the partner's sums of squares on the rx barrier, then
-// take 1/rms from all 32.
+// negative word -1 - parity (RMSNorm phase, first tile) means: wait for the partner's sums of squares on the rx barrier, then take 1/rms
+// from all 32.
 TCE_DEVINL void hand_tile(const Args &a, const GemvOp &op, const PSmem &sm, Red &cs, float totA, float totB, int cw, int lane) {
     const int g = lane >> 2, t = lane & 3;
     float inv = sm.inv[cw];
     if (inv < 0.f) {
         mbar_wait_u32(smem_u32(sm.rx), inv < -1.5f ? 1u : 0u);
-        inv = rms_inv(sm, 2 * kCW, op.IC, a.eps);
+        inv = rms_inv(sm, op.IC, a.eps);
         __syncwarp();  // every lane has read the flag
         if (lane == 0) sm.inv[cw] = inv;
     }
@@ -648,13 +643,12 @@ TCE_DEVINL void hand_tile(const Args &a, const GemvOp &op, const PSmem &sm, Red 
 // Stamps of consumer warp 0 (TCE_PK_DEBUG): 4 first stage landed, 5 last stage released, 6 last tile handed to the epilogue.
 // The warp's red-buffer position, its lane id and 1/rms are taken afresh here (shared memory, %laneid, a shuffle of the same value), not
 // carried in registers across the phase loop: held there, they were spilled to local memory (the attention and staging code set the
-// register budget) and reloaded on the path of every tile.  rx_parity >= 0 (pair mode, RMSNorm phases): 1/rms waits for the partner's
-// sums of squares, which are needed only when the first tile is handed over.
-TCE_DEVINL void consume_gemv(const Args &a, const GemvOp &op, const PSmem &sm, Ring &rs, float inv, int rx_parity, int cta, int ncta, int rank, int cw, int p,
-                             int nphase) {
+// register budget) and reloaded on the path of every tile.  rx_parity >= 0 (RMSNorm phases): 1/rms waits for the partner's sums of
+// squares, which are needed only when the first tile is handed over; rx_parity < 0: the input is not normalised (1/rms = 1).
+TCE_DEVINL void consume_gemv(const Args &a, const GemvOp &op, const PSmem &sm, Ring &rs, int rx_parity, int cta, int ncta, int rank, int cw, int p, int nphase) {
     int lane;
     asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
-    if (lane == 0) sm.inv[cw] = rx_parity >= 0 ? -1.f - (float)rx_parity : inv;
+    if (lane == 0) sm.inv[cw] = rx_parity >= 0 ? -1.f - (float)rx_parity : 1.f;
     __syncwarp();
     Red cs;
     {
@@ -664,16 +658,16 @@ TCE_DEVINL void consume_gemv(const Args &a, const GemvOp &op, const PSmem &sm, R
     }
     const int g = lane >> 2, t = lane & 3;
     int t0, t1;
-    partition(op, cta, ncta, a.pair, t0, t1);
-    const KRange kr = k_range(op.NG, a.pair, rank);
+    partition(op, cta, ncta, t0, t1);
+    const KRange kr = k_range(op.NG, rank);
     const int nb = kr.nb, nbox = (t1 - t0) * nb;
     const int lim = kr.ng - cw;  // box b carries this warp's group when 16 b < lim (the last box of a K range may have fewer than 16)
     // row g of group cw, this lane's 16-byte chunk: the 16 rows of a group 64 B apart (conflict-free LDS.128), gate | up as two 8-row regions
-    const uint32_t w_lane = (uint32_t)cw * (op.pair ? 512u : 1024u) + (uint32_t)g * 64u + (uint32_t)t * 16u;
-    const uint32_t wb_off = op.pair ? 8192u : 512u;  // row g + 8
+    const uint32_t w_lane = (uint32_t)cw * (op.gate_up ? 512u : 1024u) + (uint32_t)g * 64u + (uint32_t)t * 16u;
+    const uint32_t wb_off = op.gate_up ? 8192u : 512u;  // row g + 8
     const uint32_t m_lane = (uint32_t)kMetaOff + (uint32_t)(cw * 8 + g) * 4u;                            // scales of rows g, g + 8 of group cw
     const uint32_t z_lane = (uint32_t)kMetaOff + 512u + (uint32_t)(cw * 8 + g) * 2u;
-    const uint32_t x_lane = sm.xs_u32 + (uint32_t)((g >> 1) & 1) * (uint32_t)plane_ic(op.NG, a.pair) * 2u + (uint32_t)(t * 2 + (g & 1)) * 16u + (uint32_t)cw * 256u;
+    const uint32_t x_lane = sm.xs_u32 + (uint32_t)((g >> 1) & 1) * (uint32_t)plane_ic(op.NG) * 2u + (uint32_t)(t * 2 + (g & 1)) * 16u + (uint32_t)cw * 256u;
     const uint32_t s_lane = sm.gsum_u32 + (uint32_t)(2 * cw + (t & 1)) * 4u;
     const uint32_t q_lane = sm.gx_u32 + (uint32_t)cw * 4u;
     const float lscale = (t == 0) ? 65536.f : (t == 1 ? 1.f : 0.f);
@@ -748,13 +742,13 @@ TCE_DEVINL void consume_gemv(const Args &a, const GemvOp &op, const PSmem &sm, R
 // ------------------------------------------------------------------------------------------------------------ epilogue warp
 struct EpiState {
     unsigned long long best;  // PE_LOGITS: running arg-max key of this warp
-    uint32_t nsent, nrecv;    // pair mode: tile row sums sent to / received from the partner so far (slot = n % kPairSlots)
+    uint32_t nsent, nrecv;    // tile row sums sent to / received from the partner so far (slot = n % kPairSlots)
 };
 
 // Stamp (TCE_PK_DEBUG): 7 the last tile's partials are in; the caller stamps 3 after its last publish.
 // The lane id is read here (%laneid), as in consume_gemv: passed in, the lane-derived offsets and predicates were hoisted out of the phase
 // loop, spilled, and reloaded on every tile.
-// Pair mode: rank 0 publishes the first half of the pair's tiles and rank 1 the rest (both epilogue warps publish), adding the partner's 16
+// Rank 0 publishes the first half of the pair's tiles and rank 1 the rest (both epilogue warps publish), adding the partner's 16
 // row sums, received by st.async into a `prx` slot, to its own: the same bits on every run.  Contiguous halves let each direction stream up
 // to kPairSlots tiles ahead; tiles owned alternately made the two epilogues wait for each other on every tile (on H100 the Llama-3-8B step
 // took 2.96 ms instead of 2.01).
@@ -763,10 +757,10 @@ TCE_DEVINL void epilogue_gemv(const Args &a, const GemvOp &op, const PSmem &sm, 
     int lane;
     asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
     int t0, t1;
-    partition(op, cta, ncta, a.pair, t0, t1);
+    partition(op, cta, ncta, t0, t1);
     const bool tp = a.tp_size > 1;
-    const uint32_t rank = a.pair ? cluster_rank() : 2u;  // 2: no partner (tested on this register: a flag kept beside it was spilled)
-    const int tsplit = t0 + (t1 - t0 + 1) / 2;            // pair mode: first tile published by rank 1
+    const uint32_t rank = cluster_rank();
+    const int tsplit = t0 + (t1 - t0 + 1) / 2;  // first tile published by rank 1
     for (int tile = t0; tile < t1; tile++) {
         mbar_wait_u32(sm.redfull_u32 + (uint32_t)es.rb * 8u, es.rphase);
         if (tile == t1 - 1 && lane == 0) stamp(a, cta, nphase, p, 7);
@@ -782,24 +776,22 @@ TCE_DEVINL void epilogue_gemv(const Args &a, const GemvOp &op, const PSmem &sm, 
         __syncwarp();
         if (lane == 0) mbar_arrive_u32(sm.redempty_u32 + (uint32_t)es.rb * 8u);
         es.advance();
-        if (rank < 2u) {
-            const bool mine = (tile >= tsplit) == (rank == 1u);
-            const uint32_t slot = (mine ? st.nrecv : st.nsent) % kPairSlots;
-            if (!mine) {  // the partner publishes this tile: send it this CTA's row sums
-                const uint32_t n = st.nsent++;
-                mbar_wait_cluster(smem_u32(sm.pfree + slot), ((n / kPairSlots) & 1u) ^ 1u);
-                if (lane < 16)
-                    st_async_b32(map_to_cta(smem_u32(sm.prx + slot * 16 + lane), rank ^ 1u), __float_as_uint(v), map_to_cta(smem_u32(sm.prx_full + slot), rank ^ 1u));
-                continue;
-            }
-            const uint32_t n = st.nrecv++;
-            const uint32_t fb = smem_u32(sm.prx_full + slot);
-            if (lane == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(fb), "r"(64u) : "memory");
-            mbar_wait_u32(fb, (n / kPairSlots) & 1u);
-            v += sm.prx[slot * 16 + (lane & 15)];  // a sum of two terms: the same bits whichever rank publishes
-            __syncwarp();
-            if (lane == 0) mbar_arrive_remote(map_to_cta(smem_u32(sm.pfree + slot), rank ^ 1u));
+        const bool mine = (tile >= tsplit) == (rank == 1u);
+        const uint32_t slot = (mine ? st.nrecv : st.nsent) % kPairSlots;
+        if (!mine) {  // the partner publishes this tile: send it this CTA's row sums
+            const uint32_t n = st.nsent++;
+            mbar_wait_cluster(smem_u32(sm.pfree + slot), ((n / kPairSlots) & 1u) ^ 1u);
+            if (lane < 16)
+                st_async_b32(map_to_cta(smem_u32(sm.prx + slot * 16 + lane), rank ^ 1u), __float_as_uint(v), map_to_cta(smem_u32(sm.prx_full + slot), rank ^ 1u));
+            continue;
         }
+        const uint32_t n = st.nrecv++;
+        const uint32_t fb = smem_u32(sm.prx_full + slot);
+        if (lane == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(fb), "r"(64u) : "memory");
+        mbar_wait_u32(fb, (n / kPairSlots) & 1u);
+        v += sm.prx[slot * 16 + (lane & 15)];  // a sum of two terms: the same bits whichever rank publishes
+        __syncwarp();
+        if (lane == 0) mbar_arrive_remote(map_to_cta(smem_u32(sm.pfree + slot), rank ^ 1u));
         switch (op.epi) {
             case PE_DELTA_LL:
                 // o_proj / down_proj output rows: one {float, tag} word each, into slot `rank` of every rank's buffer (NVLink peer stores
@@ -1106,16 +1098,13 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
         mbar_fence_init();
     }
     __syncthreads();
+    // both CTAs of the cluster have initialised their barriers before either sends
+    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
     PairCtx pc;
-    if (a.pair) {
-        // both CTAs of the cluster have initialised their barriers before either sends
-        asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-        asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-        pc.on = true;
-        pc.rank = cluster_rank();
-        pc.r_rms = map_to_cta(smem_u32(sm.rms), pc.rank ^ 1u);
-        pc.r_bar = map_to_cta(smem_u32(sm.rx), pc.rank ^ 1u);
-    }
+    pc.rank = cluster_rank();
+    pc.r_rms = map_to_cta(smem_u32(sm.rms), pc.rank ^ 1u);
+    pc.r_bar = map_to_cta(smem_u32(sm.rx), pc.rank ^ 1u);
     // phase p = 5 * layer + k, k: 0 RMSNorm + q|k|v, 1 attention, 2 o_proj, 3 RMSNorm + gate|up, 4 down_proj; p = 5 * Lyr: lm_head
     const int nphase = 5 * Lyr + 1;
     const unsigned epoch = *a.epoch;
@@ -1147,10 +1136,8 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
             epilogue_gemv(a, a.op[oi], sm, es, st, out, (oi == OPI_DOWN) ? 1 : 0, tag_base + 2u * (uint32_t)p, cta, ncta, p, nphase);
             if (lane == 0) stamp(a, cta, nphase, p, 3);
         }
-        // pair mode: stay resident until the partner has read every row sum sent to it (its last arrivals target this CTA's barriers)
-        if (a.pair) {
-            for (uint32_t n = st.nsent; n < st.nsent + kPairSlots; n++) mbar_wait_cluster(smem_u32(sm.pfree + n % kPairSlots), ((n / kPairSlots) & 1u) ^ 1u);
-        }
+        // stay resident until the partner has read every row sum sent to it (its last arrivals target this CTA's barriers)
+        for (uint32_t n = st.nsent; n < st.nsent + kPairSlots; n++) mbar_wait_cluster(smem_u32(sm.pfree + n % kPairSlots), ((n / kPairSlots) & 1u) ^ 1u);
         unsigned long long key = st.best;
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) {
@@ -1170,6 +1157,7 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
     const int ctid = tid - 32 * kAuxWarps;
     const int cw = warp - kAuxWarps;
     Ring rs;
+    uint32_t nrms = 0;  // RMSNorm exchanges with the partner so far (parity of the rx barrier)
     if (lane == 0) sm.red_pos[cw] = make_int2(0, 0);
     __syncwarp();
     if (ctid < 256) sm.rope[ctid] = (ctid < 128) ? a.cos[(size_t)pos * 128 + ctid] : a.sin[(size_t)pos * 128 + ctid - 128];  // visible after the first phase's barrier
@@ -1188,9 +1176,8 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
         const int oi = (l == Lyr) ? OPI_LMHEAD : ((k == 0) ? OPI_QKV : (k - 1));
         const GemvOp &op = a.op[oi];
         int t0, t1;
-        partition(op, cta, ncta, pc.on, t0, t1);
-        const bool work = t1 > t0;  // pair mode: the same for both CTAs of the cluster
-        float inv = 1.f;
+        partition(op, cta, ncta, t0, t1);
+        const bool work = t1 > t0;  // the same for both CTAs of the cluster
         int rx_parity = -1;
         if (oi == OPI_O) {
             if (work) stage_half(op, sm, pc, a.attn_ll, tag_in, cta, ctid, lane);
@@ -1200,11 +1187,11 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
             // the residual copy of this CTA must see every o_proj / down_proj output, whether or not the CTA owns tiles of this phase
             const float *gamma = (oi == OPI_LMHEAD) ? a.final_norm : (oi == OPI_QKV ? a.layers[l].input_norm : a.layers[l].post_norm);
             const uint2 *delta = (oi == OPI_GATEUP) ? a.delta_ll[0] : a.delta_ll[1];
-            inv = stage_rms(a, op, sm, pc, delta, tag_in, gamma, token, p == 0, work, cta, ctid, cw, lane);
-            if (pc.on && work) rx_parity = (int)(pc.nstage++ & 1u);
+            stage_rms(a, op, sm, pc, delta, tag_in, gamma, token, p == 0, work, cta, ctid, cw, lane);
+            if (work) rx_parity = (int)(nrms++ & 1u);
         }
         if (ctid == 0) stamp(a, cta, nphase, p, 1);
-        if (work) consume_gemv(a, op, sm, rs, inv, rx_parity, cta, ncta, (int)pc.rank, cw, p, nphase);
+        if (work) consume_gemv(a, op, sm, rs, rx_parity, cta, ncta, (int)pc.rank, cw, p, nphase);
         if (ctid == 0) stamp(a, cta, nphase, p, 2);
         named_bar_sync(1, kConsumerThreads);  // every warp is done with the planes before the next phase overwrites them
     }
@@ -1240,7 +1227,7 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
 // scales half[rows][sf_w] + zeros u32[rows][zeros_w] (QM_CUDA, llm/tools/quantize_methods.py:370-442) -> one 768-byte record per
 // (16-row tile, 16-group box of the K range [g0, g0 + ng)): scales half[16 groups][8][2] (rows g and g + 8 adjacent), then zero points
 // u8[16 groups][8][2] in the same order.
-__global__ void repack_meta_kernel(W4Seg s0, W4Seg s1, W4Seg s2, int nseg, int pair, int g0, int ng, int nb, int zeros_w, int sf_w, int num_tiles, uint8_t *out) {
+__global__ void repack_meta_kernel(W4Seg s0, W4Seg s1, W4Seg s2, int nseg, int gate_up, int g0, int ng, int nb, int zeros_w, int sf_w, int num_tiles, uint8_t *out) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;  // (tile, box, gi)
     if (idx >= num_tiles * nb * kBoxGroups) return;
     const int gi = idx % kBoxGroups, rb = idx / kBoxGroups;
@@ -1252,7 +1239,7 @@ __global__ void repack_meta_kernel(W4Seg s0, W4Seg s1, W4Seg s2, int nseg, int p
     for (int r = 0; r < 16; r++) {
         const W4Seg *seg = &s0;
         int row;
-        if (pair) {
+        if (gate_up) {
             seg = (r < 8) ? &s0 : &s1;
             row = tile * 8 + (r & 7);
         } else {
@@ -1294,7 +1281,7 @@ static size_t fixed_bytes(const Args &a) {
 }
 void plan_smem(Args &a, int smem_optin) {
     int xs = attn_scratch_bytes(a.nrep);
-    for (int i = 0; i < OPI_COUNT; i++) xs = max(xs, 4 * plane_ic(a.op[i].NG, a.pair));  // four int8 planes per input channel of the K range
+    for (int i = 0; i < OPI_COUNT; i++) xs = max(xs, 4 * plane_ic(a.op[i].NG));  // four int8 planes per input channel of the K range
     a.xs_bytes = (xs + 15) & ~15;
     a.nst = 0;
     const long long n = ((long long)smem_optin - (long long)fixed_bytes(a)) / kStageBytes;
@@ -1302,14 +1289,14 @@ void plan_smem(Args &a, int smem_optin) {
 }
 size_t smem_bytes(const Args &a) { return fixed_bytes(a) + (size_t)a.nst * kStageBytes; }
 
-cudaError_t repack_meta(Ctx *ctx, const W4Seg *segs, int nseg, int pair, int IC, const KRange &kr, uint8_t *out, cudaStream_t stream) {
+cudaError_t repack_meta(Ctx *ctx, const W4Seg *segs, int nseg, int gate_up, int IC, const KRange &kr, uint8_t *out, cudaStream_t stream) {
     int rows = 0;
     for (int i = 0; i < nseg; i++) rows += segs[i].rows;
     const int num_tiles = rows / 16;
     const int zw = zeros_width(IC, kW4Group);
     const int total = num_tiles * kr.nb * kBoxGroups;
     if (total == 0) return cudaSuccess;
-    repack_meta_kernel<<<(total + 127) / 128, 128, 0, stream>>>(segs[0], segs[nseg > 1 ? 1 : 0], segs[nseg > 2 ? 2 : 0], nseg, pair, kr.g0, kr.ng, kr.nb, zw, zw * 8,
+    repack_meta_kernel<<<(total + 127) / 128, 128, 0, stream>>>(segs[0], segs[nseg > 1 ? 1 : 0], segs[nseg > 2 ? 2 : 0], nseg, gate_up, kr.g0, kr.ng, kr.nb, zw, zw * 8,
                                                                num_tiles, out);
     (void)ctx;
     return cudaGetLastError();
@@ -1327,22 +1314,30 @@ cudaError_t encode_kv_tmap(CUtensorMap *out, const void *kv, long long rows) {
     return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
-// can the grid run as co-resident clusters of two CTAs (one per TPC)?
-bool pair_supported(Ctx *ctx, const Args &a) {
-    if (ctx->num_sms % 2) return false;
-    const size_t smem = smem_bytes(a);
-    if (cudaFuncSetAttribute(decode_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->smem_optin) != cudaSuccess) return false;
+// Clusters of two CTAs (one TPC) split K and add each other's tile row sums over distributed shared memory.  All CTAs must be co-resident:
+// they wait for each other's results.  The launch carries the cluster attribute alone -- profilers (ncu) cannot intercept a launch that is
+// both cooperative and clustered -- and co-residency is established instead by pair_supported() at model build: one CTA per SM fits for
+// all num_sms / 2 clusters, and the step is the only work on its stream.  A CTA that were not resident would surface through the bounded
+// spins (__trap after ~10 s), not as a silent hang.
+static cudaLaunchConfig_t launch_config(Ctx *ctx, size_t smem, cudaStream_t stream, cudaLaunchAttribute *attr) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(ctx->num_sms);
     cfg.blockDim = dim3(kThreads);
     cfg.dynamicSmemBytes = smem;
-    cudaLaunchAttribute attr[1];
+    cfg.stream = stream;
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = 2;
     attr[0].val.clusterDim.y = 1;
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
+    return cfg;
+}
+
+bool pair_supported(Ctx *ctx, const Args &a) {
+    if (cudaFuncSetAttribute(decode_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->smem_optin) != cudaSuccess) return false;
+    cudaLaunchAttribute attr[1];
+    const cudaLaunchConfig_t cfg = launch_config(ctx, smem_bytes(a), nullptr, attr);
     int nclusters = 0;
     if (cudaOccupancyMaxActiveClusters(&nclusters, decode_persistent_kernel, &cfg) != cudaSuccess) {
         cudaGetLastError();
@@ -1354,46 +1349,11 @@ bool pair_supported(Ctx *ctx, const Args &a) {
 cudaError_t launch(Ctx *ctx, const Args &a, cudaStream_t stream) {
     const size_t smem = smem_bytes(a);
     if ((int)smem > ctx->smem_optin) return cudaErrorInvalidConfiguration;
-    cudaError_t e = cudaFuncSetAttribute(decode_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->smem_optin);
+    const cudaError_t e = cudaFuncSetAttribute(decode_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->smem_optin);
     if (e != cudaSuccess) return e;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(ctx->num_sms);
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeCooperative;  // all CTAs must be co-resident: they wait for each other's results
-    attr[0].val.cooperative = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    static bool pair_refused = false;  // a cluster launch was refused once in this process
-    if (a.pair && !pair_refused) {
-        // Clusters of two CTAs (one TPC) split K and add each other's tile row sums over distributed shared memory.  Launched with the cluster attribute ALONE:
-        // profilers (ncu) cannot intercept a launch that is both cooperative and clustered (LaunchFailed), and co-residency -- what the cooperative
-        // attribute would assert -- is established instead by pair_supported(): one CTA per SM fits for all num_sms / 2 clusters, and the step is the only
-        // work on its stream.  A CTA that were not resident would surface through the bounded spins (__trap after ~10 s), not as a silent hang.
-        cudaLaunchAttribute cattr[1];
-        cattr[0].id = cudaLaunchAttributeClusterDimension;
-        cattr[0].val.clusterDim.x = 2;
-        cattr[0].val.clusterDim.y = 1;
-        cattr[0].val.clusterDim.z = 1;
-        cfg.attrs = cattr;
-        cfg.numAttrs = 1;
-        e = cudaLaunchKernelEx(&cfg, decode_persistent_kernel, a);
-        if (e == cudaSuccess) return e;
-        cudaGetLastError();  // a launch-configuration error is not sticky: run without clusters (every CTA reduces over all of K itself)
-        pair_refused = true;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-    }
-    Args single = a;
-    if (a.pair) {
-        single.pair = 0;
-        plan_smem(single, ctx->smem_optin);
-        if (single.nst < 2) return cudaErrorInvalidConfiguration;
-        cfg.dynamicSmemBytes = smem_bytes(single);
-    }
-    return cudaLaunchKernelEx(&cfg, decode_persistent_kernel, single);
+    cudaLaunchAttribute attr[1];
+    const cudaLaunchConfig_t cfg = launch_config(ctx, smem, stream, attr);
+    return cudaLaunchKernelEx(&cfg, decode_persistent_kernel, a);
 }
 
 }  // namespace pk

@@ -178,17 +178,16 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         return cudaErrorNotSupported;
     };
     if (hd != 128 || nrep > 4 || ncta < KVH || F % 16 || V % 16) return no("shape outside the persistent kernel's envelope");
-    int coop = 0;
-    cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, ctx_->device);
-    if (!coop) return no("device cannot launch cooperative kernels");
+    // clusters of two CTAs split K (see pk::KRange): an even number of SMs, and two 128-groups or more in every op
+    if (ncta % 2) return no("odd SM count: the persistent kernel runs on clusters of two CTAs");
     pk::Args a{};
-    auto mk = [&](int IC, int rows, int nseg, int pair, int rows0, int rows1, int x_mode, int epi) {
+    auto mk = [&](int IC, int rows, int nseg, int gate_up, int rows0, int rows1, int x_mode, int epi) {
         pk::GemvOp o{};
         o.IC = IC;
         o.NG = IC / kW4Group;
         o.num_tiles = rows / 16;
         o.nseg = nseg;
-        o.pair = pair;
+        o.gate_up = gate_up;
         o.rows0 = rows0;
         o.rows1 = rows1;
         o.x_mode = x_mode;
@@ -207,19 +206,13 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         if (a.op[i].NG < min_ng) min_ng = a.op[i].NG;
         if (a.op[i].IC % kW4Group || a.op[i].num_tiles < 1) return no("bad GEMV shape");
     }
+    if (min_ng < 2) return no("a GEMV with a single 128-group: nothing to split across a cluster of two CTAs");
     a.max_ng = (max_ng + 3) & ~3;
     a.E = E;
     a.nrep = nrep;
-    // pair mode (clusters of two CTAs that split K, see pk::KRange): on unless switched off, or the device cannot co-schedule num_sms / 2
-    // such clusters, or an op has a single 128-group to split
-    a.pair = (!getenv("TCE_PK_PAIR") || atoi(getenv("TCE_PK_PAIR")) != 0) && ncta % 2 == 0 && min_ng >= 2 ? 1 : 0;
     pk::plan_smem(a, ctx_->smem_optin);
-    if (a.pair && (a.nst < 2 || !pk::pair_supported(ctx_, a))) {
-        a.pair = 0;
-        pk::plan_smem(a, ctx_->smem_optin);
-    }
     if (a.nst < 2) return no("shared memory too small for the persistent kernel");
-    const int nsets = a.pair ? pk::kMapSets : 1;  // full K (what a refused cluster launch falls back to), then the pair halves
+    if (!pk::pair_supported(ctx_, a)) return no("the device cannot co-schedule num_sms / 2 clusters of two CTAs");
 
     auto dalloc = [&](size_t bytes) -> void * {
         DevPtr<uint8_t> p;
@@ -228,9 +221,9 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         return pk_allocs_.back().get();
     };
     cudaStream_t s = ctx_->stream;
-    // ---- tensor maps: per set [Lyr][7] + lm_head + KV cache ----
-    const size_t nmaps = (size_t)Lyr * 7 + 2;
-    std::vector<CUtensorMap> maps(nsets * nmaps);
+    // ---- tensor maps: per cluster rank [Lyr][7] + lm_head, then the KV cache ----
+    const size_t nmaps = (size_t)Lyr * 7 + 1;
+    std::vector<CUtensorMap> maps(2 * nmaps + 1);
     memset(maps.data(), 0, maps.size() * sizeof(CUtensorMap));
     std::vector<pk::LayerDesc> descs(Lyr);
     const size_t per_kv = (size_t)KVH * cfg_.max_ctx;  // rows per (layer, K|V) slab
@@ -238,27 +231,27 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         const tce_llama_layer &L = layers_[l];
         const tce_w4_tensor *t7[7] = {&L.q, &L.k, &L.v, &L.o, &L.gate, &L.up, &L.down};
         const int opi[7] = {pk::OPI_QKV, pk::OPI_QKV, pk::OPI_QKV, pk::OPI_O, pk::OPI_GATEUP, pk::OPI_GATEUP, pk::OPI_DOWN};
-        for (int set = 0; set < nsets; set++) {
+        for (int rank = 0; rank < 2; rank++) {
             for (int i = 0; i < 7; i++) {
                 const pk::GemvOp &o = a.op[opi[i]];
-                const pk::KRange kr = pk::k_range(o.NG, set > 0, set - 1);
-                DCK(encode_w4_tmap_units(&maps[set * nmaps + (size_t)l * 7 + i], t7[i]->w, t7[i]->oc, t7[i]->ic, kr.bw, o.pair ? 8 : 16, kr.g0, kr.ng));
+                const pk::KRange kr = pk::k_range(o.NG, rank);
+                DCK(encode_w4_tmap_units(&maps[rank * nmaps + (size_t)l * 7 + i], t7[i]->w, t7[i]->oc, t7[i]->ic, kr.bw, o.gate_up ? 8 : 16, kr.g0, kr.ng));
             }
         }
         pk::LayerDesc &D = descs[l];
         memset(&D, 0, sizeof(D));
         const W4Seg qkv[3] = {seg_of(L.q), seg_of(L.k), seg_of(L.v)}, o1[1] = {seg_of(L.o)}, gu[2] = {seg_of(L.gate), seg_of(L.up)}, d1[1] = {seg_of(L.down)};
         const W4Seg *segs[4] = {qkv, o1, gu, d1};
-        const int nsegs[4] = {3, 1, 2, 1}, pairs[4] = {0, 0, 1, 0};
+        const int nsegs[4] = {3, 1, 2, 1};
         const int ops4[4] = {pk::OPI_QKV, pk::OPI_O, pk::OPI_GATEUP, pk::OPI_DOWN};
-        for (int set = 0; set < nsets; set++) {
+        for (int rank = 0; rank < 2; rank++) {
             for (int i = 0; i < 4; i++) {
                 const pk::GemvOp &o = a.op[ops4[i]];
-                const pk::KRange kr = pk::k_range(o.NG, set > 0, set - 1);
+                const pk::KRange kr = pk::k_range(o.NG, rank);
                 uint8_t *m = (uint8_t *)dalloc((size_t)o.num_tiles * kr.nb * pk::kBoxMetaBytes);
                 if (!m) return cudaErrorMemoryAllocation;
-                DCK(pk::repack_meta(ctx_, segs[i], nsegs[i], pairs[i], o.IC, kr, m, s));
-                D.meta[set][i] = m;
+                DCK(pk::repack_meta(ctx_, segs[i], nsegs[i], o.gate_up, o.IC, kr, m, s));
+                D.meta[rank][i] = m;
             }
         }
         D.input_norm = L.input_norm;
@@ -271,16 +264,16 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
     {
         const pk::GemvOp &o = a.op[pk::OPI_LMHEAD];
         const W4Seg lm[1] = {seg_of(w_.lm_head)};
-        for (int set = 0; set < nsets; set++) {
-            const pk::KRange kr = pk::k_range(o.NG, set > 0, set - 1);
-            DCK(encode_w4_tmap_units(&maps[set * nmaps + (size_t)Lyr * 7], w_.lm_head.w, w_.lm_head.oc, w_.lm_head.ic, kr.bw, 16, kr.g0, kr.ng));
+        for (int rank = 0; rank < 2; rank++) {
+            const pk::KRange kr = pk::k_range(o.NG, rank);
+            DCK(encode_w4_tmap_units(&maps[rank * nmaps + (size_t)Lyr * 7], w_.lm_head.w, w_.lm_head.oc, w_.lm_head.ic, kr.bw, 16, kr.g0, kr.ng));
             uint8_t *m = (uint8_t *)dalloc((size_t)o.num_tiles * kr.nb * pk::kBoxMetaBytes);
             if (!m) return cudaErrorMemoryAllocation;
             DCK(pk::repack_meta(ctx_, lm, 1, 0, o.IC, kr, m, s));
-            a.lm_meta[set] = m;
-            DCK(pk::encode_kv_tmap(&maps[set * nmaps + (size_t)Lyr * 7 + 1], d_kv_.get(), (long long)Lyr * 2 * per_kv));
+            a.lm_meta[rank] = m;
         }
     }
+    DCK(pk::encode_kv_tmap(&maps[2 * nmaps], d_kv_.get(), (long long)Lyr * 2 * per_kv));
     CUtensorMap *dmaps = (CUtensorMap *)dalloc(maps.size() * sizeof(CUtensorMap));
     pk::LayerDesc *ddesc = (pk::LayerDesc *)dalloc(descs.size() * sizeof(pk::LayerDesc));
     a.nsplit_max = pk::attn_nsplit_max(ncta, KVH, cfg_.max_ctx);

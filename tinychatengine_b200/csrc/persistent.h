@@ -1,10 +1,11 @@
 // persistent.h -- host/device interface of the persistent Llama decode kernel (decode_persistent.cu).
 //
-// One cooperative kernel per decoded token, one CTA per SM.  Everything a token needs from HBM -- packed weights, their repacked
-// scales/zeros, and the K/V cache rows -- flows through ONE ring of TMA stages per CTA that is filled by a producer warp which depends
-// on nothing but static data, so it runs ahead across all phase boundaries.  Phases hand their results to each other through
-// flag-carrying 8-byte words (value + phase tag, stored and loaded as one unit): there is no grid barrier, fence or counter between
-// the five phases of a layer -- a consumer simply spins on the words it needs.
+// One kernel per decoded token, one CTA per SM, launched as clusters of two CTAs: both CTAs of a cluster walk the same GEMV tiles, each
+// over its half of the 128-groups (k_range), and one CTA per tile adds its partner's 16 row sums (st.async over DSMEM).  Everything a
+// token needs from HBM -- packed weights, their repacked scales/zeros, and the K/V cache rows -- flows through ONE ring of TMA stages per
+// CTA that is filled by a producer warp which depends on nothing but static data, so it runs ahead across all phase boundaries.  Phases
+// hand their results to each other through flag-carrying 8-byte words (value + phase tag, stored and loaded as one unit): there is no
+// grid barrier, fence or counter between the five phases of a layer -- a consumer simply spins on the words it needs.
 #pragma once
 #include "kernels.h"
 
@@ -22,7 +23,7 @@ constexpr int kBoxMetaBytes = 768;
 constexpr int kStageBytes = 34816;               // 32 KiB + 1.5 KiB meta (+ pad), 1 KiB multiple (128B-swizzle atoms of the K/V boxes)
 constexpr int kMaxStages = 6;
 constexpr int kRedBufs = 3;
-constexpr int kPairSlots = 8;                    // pair mode: tile partials in flight from one CTA to its partner
+constexpr int kPairSlots = 8;                    // tile partials in flight from one CTA to its partner
 constexpr int kKvChunk = 64;                     // cached positions per ring stage (K rows in the first half, V rows in the second)
 
 enum XMode : int { PX_HALF = 0, PX_RMS_F32 = 1 };
@@ -32,15 +33,14 @@ enum OpIdx : int { OPI_QKV = 0, OPI_O = 1, OPI_GATEUP = 2, OPI_DOWN = 3, OPI_LMH
 // shape of one GEMV op; identical for every layer, so it lives in the kernel parameter block.
 struct GemvOp {
     int IC, NG;          // input channels, 128-groups per row
-    int num_tiles;       // 16-row tiles (pair mode: 8 gate rows + 8 up rows)
-    int nseg, pair;      // row segments (q|k|v = 3); pair = gate/up interleave
+    int num_tiles;       // 16-row tiles (gate | up: 8 gate rows + 8 up rows)
+    int nseg, gate_up;   // row segments (q|k|v = 3); gate_up: tiles interleave 8 rows of each of the two segments
     int rows0, rows1;    // rows of segments 0 and 1 (tile -> segment)
     int x_mode, epi;
 };
 
-// The K range a CTA reduces over: all NG groups, or in pair mode (clusters of two CTAs that split K) rank 0 the first ceil(NG / 2) groups and
-// rank 1 the rest.  Contiguous halves keep every TMA box a plain range of groups of one tensor map, encoded over the half (box width bw), so a
-// box never reads the partner's groups.  The range is walked as `nb` boxes of 16 groups per tile, tile by tile; a ring stage takes two
+// The K range a CTA reduces over: cluster rank 0 the first ceil(NG / 2) groups, rank 1 the rest.  Contiguous halves keep every TMA box a
+// plain range of groups of one tensor map, encoded over the half (box width bw), so a box never reads the partner's groups.  The range is walked as `nb` boxes of 16 groups per tile, tile by tile; a ring stage takes two
 // consecutive boxes (slot 0 at 0, slot 1 at 16 KiB), which may belong to two tiles: at NG = 32 a stage holds the halves of two tiles.  Group gi
 // of a slot sits at gi KiB (gate | up: the 8 gate rows at gi * 512 B, the 8 up rows 8 KiB further); a box that runs past the range is
 // zero-filled by TMA and still counts its full bytes.  Scales and zeros follow the same walk: one 768-byte record per (tile, box).
@@ -48,22 +48,21 @@ struct KRange {
     int g0, ng;  // first group, groups
     int nb, bw;  // boxes per tile, TMA box width in groups
 };
-__host__ __device__ inline KRange k_range(int NG, int pair, int rank) {
+__host__ __device__ inline KRange k_range(int NG, int rank) {
     KRange k;
     const int h = (NG + 1) / 2;
-    k.g0 = (pair && rank) ? h : 0;
-    k.ng = pair ? (rank ? NG - h : h) : NG;
+    k.g0 = rank ? h : 0;
+    k.ng = rank ? NG - h : h;
     k.nb = (k.ng + kBoxGroups - 1) / kBoxGroups;
     k.bw = k.ng < kBoxGroups ? k.ng : kBoxGroups;
     return k;
 }
-// input channels of the activation-plane buffer of one op (planes of the CTA's K range; region B starts at twice this many bytes)
-__host__ __device__ inline int plane_ic(int NG, int pair) { return k_range(NG, pair, 0).ng * 128; }
-
-constexpr int kMapSets = 3;      // tensor maps and scale|zero records: full K (single-CTA), then the K halves of pair ranks 0 and 1
+// input channels of the activation-plane buffer of one op (planes of the CTA's K range, the larger one of rank 0; region B starts at twice
+// this many bytes)
+__host__ __device__ inline int plane_ic(int NG) { return k_range(NG, 0).ng * 128; }
 
 struct LayerDesc {       // per layer, global memory
-    const uint8_t *meta[kMapSets][4];  // repacked scales|zeros of qkv, o, gate_up, down per set: [tile][box][768 B]
+    const uint8_t *meta[2][4];   // repacked scales|zeros of qkv, o, gate_up, down over the K range of cluster rank 0 / 1: [tile][box][768 B]
     const float *input_norm, *post_norm;
     __half *k_cache, *v_cache;   // [KVH][max_ctx][128] of this layer (append)
     int k_row0, v_row0;          // first row of this layer's K / V slab in the cache tensor map
@@ -74,8 +73,9 @@ struct Args {
     GemvOp op[OPI_COUNT];
     const LayerDesc *layers;
     int num_layers;
-    const CUtensorMap *maps;     // [kMapSets][num_layers * 7 (q k v o gate up down) + 2]: per set the weight maps, lm_head, then the KV cache map
-    const uint8_t *lm_meta[kMapSets];
+    const CUtensorMap *maps;     // [2][num_layers * 7 (q k v o gate up down) + 1 (lm_head)] weight maps over the K range of cluster rank 0 / 1,
+                                 // then the KV cache map
+    const uint8_t *lm_meta[2];
     const float *final_norm;
     const __half *embed;         // [rows][E]
     int embed_rows;
@@ -97,8 +97,6 @@ struct Args {
     int H, KVH, nrep, max_ctx, E, V, F;
     int nsplit_max;
     int nst;                     // ring depth
-    int pair;                    // 1: launched as clusters of two CTAs that split K: both walk the tiles of the pair, each over its half of the
-                                 // 128-groups (k_range), and one CTA per tile adds its partner's 16 row sums (st.async over DSMEM)
     int xs_bytes;                // activation-plane buffer (also the attention scratch)
     int max_ng;
     // tensor parallel (tp_size > 1): every rank writes its o_proj / down_proj outputs into slot `tp_rank` of every rank's delta buffers
@@ -110,16 +108,16 @@ struct Args {
 };
 
 size_t smem_bytes(const Args &a);
-// shared-memory plan for a.pair: the activation-plane buffer and the ring depth that fits `smem_optin` next to the fixed buffers (a.nst = 0:
+// shared-memory plan: the activation-plane buffer and the ring depth that fits `smem_optin` next to the fixed buffers (a.nst = 0:
 // does not fit).  Needs a.op, a.nrep, a.E and a.max_ng.
 void plan_smem(Args &a, int smem_optin);
 int attn_scratch_bytes(int nrep);
 int attn_nsplit_max(int ncta, int KVH, int max_ctx);
 cudaError_t launch(Ctx *ctx, const Args &a, cudaStream_t stream);
 bool pair_supported(Ctx *ctx, const Args &a);  // the grid fits as co-resident clusters of two CTAs
-// one-off repack of a (possibly multi-segment / gate-up paired) matrix's scales and zeros over the K range `kr` into per-(tile, box)
+// one-off repack of a (possibly multi-segment / gate|up interleaved) matrix's scales and zeros over the K range `kr` into per-(tile, box)
 // records (num_tiles * kr.nb * kBoxMetaBytes bytes)
-cudaError_t repack_meta(Ctx *ctx, const W4Seg *segs, int nseg, int pair, int IC, const KRange &kr, uint8_t *out, cudaStream_t stream);
+cudaError_t repack_meta(Ctx *ctx, const W4Seg *segs, int nseg, int gate_up, int IC, const KRange &kr, uint8_t *out, cudaStream_t stream);
 cudaError_t encode_kv_tmap(CUtensorMap *out, const void *kv, long long rows);
 
 }  // namespace pk
