@@ -7,14 +7,14 @@
 // walk the same GEMV tiles, each over its half of K (see KRange):
 //
 //   producer (1 warp, 1 elected lane)  walks the phases in order and keeps a ring of `nst` TMA stages full.  A stage is either
-//        [16 rows x <=32 groups] of packed int4 weights (one or two 3-D UTMALDG boxes of 16 groups through the [group][row][64 B] view,
-//        16 KiB each; see GemvOp) + the stage's repacked scales|zeros record (one 1536 B UBLKCP), or 64 cached K rows + 64 cached V rows
+//        [32 rows x <=16 groups] of packed int4 weights (one 32 KiB 3-D UTMALDG box through the [group][row][64 B] view, two 16 KiB ones
+//        for gate | up; see GemvOp) + the box's repacked scales|zeros record (one 1536 B UBLKCP), or 64 cached K rows + 64 cached V rows
 //        of the attention phase (four 128B-swizzled 2-D boxes).  It depends on nothing but static data and the token position, so it
 //        runs ahead across every phase boundary.
 //   consumers (16 warps)  per phase: spin on the flag-carrying words of their input vector, quantise it (fused RMSNorm, four int8 planes
-//        per 128-group), run the integer-MMA GEMV over this CTA's tiles (two 128-k groups per warp and stage), or run flash-decoding
+//        per 128-group), run the integer-MMA GEMV over this CTA's tiles (one 128-k group of 32 rows per warp and stage), or run flash-decoding
 //        attention straight out of the ring stages (mma.sync m16n8k16, ldmatrix on the swizzled K/V rows).
-//   epilogue (1 warp)  reduces the 16 consumer partials of every tile and publishes the results as {value, phase tag} words; one CTA of
+//   epilogue (1 warp)  reduces the 16 consumer partials of every 32-row tile (one lane per row) and publishes the results as {value, phase tag} words; one CTA of
 //        the cluster per tile first adds its partner's row sums.
 //
 // There is NO grid barrier between phases.  Every vector that crosses CTAs (q|k|v, attention partials and outputs, SiLU*mul
@@ -169,13 +169,13 @@ struct PSmem {
     float *resid;       // this CTA's copy of the fp32 residual stream: the channels of its K range
     float *gx;          // [max_ng] group steps
     int *gsum;          // [max_ng][2] group sums
-    float *red;         // [kRedBufs][kCW][16] tile partials
+    float *red;         // [kRedBufs][kCW][kTileRows] tile partials
     float *rms;         // [2][kCW] partial sums of squares (rank, warp)
     float *inv;         // [kCW] each consumer warp's 1/rms of the current phase (see hand_tile)
     float *rope;        // cos[128] | sin[128] of the token position
     uint64_t *full, *empty, *red_full, *red_empty;
     uint64_t *rx;       // counts the bytes of the partner's 16 partial sums of squares (RMSNorm)
-    float *prx;         // [kPairSlots][16] tile row sums received from the partner
+    float *prx;         // [kPairSlots][kTileRows] tile row sums received from the partner
     uint64_t *prx_full; // [kPairSlots] completed by the partner's st.async of a slot of `prx`
     uint64_t *pfree;    // [kPairSlots] arrived on by the partner once it has read the row sums this CTA sent into its slot
     int2 *red_pos;      // [kCW] each consumer warp's position in the red-buffer ring between GEMV phases (see consume_gemv)
@@ -201,7 +201,7 @@ TCE_DEVINL PSmem carve(uint8_t *raw, const Args &a) {
     s.gsum = reinterpret_cast<int *>(p);
     p += (size_t)a.max_ng * 8;
     s.red = reinterpret_cast<float *>(p);
-    p += (size_t)kRedBufs * kCW * 16 * 4;
+    p += (size_t)kRedBufs * kCW * kTileRows * 4;
     s.rms = reinterpret_cast<float *>(p);
     p += 32 * 4;
     s.inv = reinterpret_cast<float *>(p);
@@ -209,7 +209,7 @@ TCE_DEVINL PSmem carve(uint8_t *raw, const Args &a) {
     s.rope = reinterpret_cast<float *>(p);
     p += 256 * 4;
     s.prx = reinterpret_cast<float *>(p);
-    p += kPairSlots * 16 * 4;
+    p += kPairSlots * kTileRows * 4;
     s.full = reinterpret_cast<uint64_t *>(p);
     s.empty = s.full + a.nst;
     s.red_full = s.empty + a.nst;
@@ -288,44 +288,40 @@ TCE_DEVINL AttnSplit attn_split(int cta, int ncta, int KVH, int pos) {
 }
 
 // ------------------------------------------------------------------------------------------------------------ producer
-// one weight stage: the next two boxes of this CTA's (tile, box) walk (see KRange), slot b at b * 16 KiB (gate | up: the up rows 8 KiB into
-// it), and their two scale|zero records, which are adjacent in the repacked array
+// one weight stage: the next box of this CTA's (tile, box) walk (see KRange; gate | up: the gate rows' box, the up rows' box 16 KiB into
+// the stage) and its scale|zero record
 TCE_DEVINL void produce_gemv(const GemvOp &op, const CUtensorMap *m0, const uint8_t *meta, const PSmem &sm, Ring &rs, int cta, int ncta, int rank,
                              uint32_t leader, uint64_t policy) {
     int t0, t1;
     partition(op, cta, ncta, t0, t1);
     const KRange kr = k_range(op.NG, rank);
-    const uint32_t box_bytes = 16u * (uint32_t)kr.bw * 64u;  // 16 rows (gate | up: 8 of each matrix) x bw groups x 64 B
+    const uint32_t stage_tx = (uint32_t)kTileRows * (uint32_t)kr.bw * 64u + (uint32_t)kBoxMetaBytes;  // 32 rows (gate | up: 16 of each matrix) x bw groups x 64 B
     const int nbox = (t1 - t0) * kr.nb;
     const uint8_t *rec = meta + (size_t)t0 * kr.nb * kBoxMetaBytes;
     int tile = t0, box = 0;
-    for (int i = 0; i < nbox; i += 2) {
-        const int n = min(2, nbox - i);
+    for (int i = 0; i < nbox; i++) {
         mbar_wait(&sm.empty[rs.stage], rs.phase ^ 1);
         uint64_t *bar = &sm.full[rs.stage];
         uint8_t *dst = sm.ring + (size_t)rs.stage * kStageBytes;
-        mbar_arrive_expect_tx_pred(bar, (uint32_t)n * (box_bytes + kBoxMetaBytes), leader);
-#pragma unroll 1
-        for (int b = 0; b < n; b++) {
-            // the tile's matrix (q|k|v: tiles never straddle two segments; gate | up: the gate map, the up map follows it) and first row
-            int row = op.gate_up ? tile * 8 : tile * 16;
-            const CUtensorMap *m = m0;
-            if (!op.gate_up && op.nseg > 1 && row >= op.rows0) {
-                row -= op.rows0;
-                m = m0 + 1;
-                if (op.nseg > 2 && row >= op.rows1) {
-                    row -= op.rows1;
-                    m = m0 + 2;
-                }
-            }
-            tma_load_3d_pred(dst + b * 16384, m, 0, row, box * kBoxGroups, bar, policy, leader);
-            if (op.gate_up) tma_load_3d_pred(dst + b * 16384 + 8192, m + 1, 0, row, box * kBoxGroups, bar, policy, leader);
-            if (++box == kr.nb) {
-                box = 0;
-                tile++;
+        mbar_arrive_expect_tx_pred(bar, stage_tx, leader);
+        // the tile's matrix (q|k|v: tiles never straddle two segments; gate | up: the gate map, the up map follows it) and first row
+        int row = op.gate_up ? tile * (kTileRows / 2) : tile * kTileRows;
+        const CUtensorMap *m = m0;
+        if (!op.gate_up && op.nseg > 1 && row >= op.rows0) {
+            row -= op.rows0;
+            m = m0 + 1;
+            if (op.nseg > 2 && row >= op.rows1) {
+                row -= op.rows1;
+                m = m0 + 2;
             }
         }
-        bulk_g2s_pred(dst + kMetaOff, rec + (size_t)i * kBoxMetaBytes, (uint32_t)n * kBoxMetaBytes, bar, policy, leader);
+        tma_load_3d_pred(dst, m, 0, row, box * kBoxGroups, bar, policy, leader);
+        if (op.gate_up) tma_load_3d_pred(dst + 16384, m + 1, 0, row, box * kBoxGroups, bar, policy, leader);
+        bulk_g2s_pred(dst + kMetaOff, rec + (size_t)i * kBoxMetaBytes, (uint32_t)kBoxMetaBytes, bar, policy, leader);
+        if (++box == kr.nb) {
+            box = 0;
+            tile++;
+        }
         __syncwarp();
         rs.advance(sm.nst);
     }
@@ -375,7 +371,7 @@ TCE_DEVINL void producer_walk(const Args &a, const PSmem &sm, int cta, int ncta,
 // ------------------------------------------------------------------------------------------------------------ clusters of two CTAs
 // The two CTAs of a cluster walk the same tiles, CTA `rank` over its K range (k_range): each stages, keeps and reads only its own half of the
 // activation planes and of the residual stream.  What crosses between them goes by st.async (remote shared-memory stores that complete
-// transaction bytes on the receiver's mbarrier: no fence, no flag): the 16 partial sums of squares of an RMSNorm, and the 16 row sums of
+// transaction bytes on the receiver's mbarrier: no fence, no flag): the 16 partial sums of squares of an RMSNorm, and the 32 row sums of
 // every tile the partner publishes.
 struct PairCtx {
     uint32_t rank;
@@ -585,36 +581,47 @@ TCE_DEVINL void stage_rms(const Args &a, const GemvOp &op, const PSmem &sm, cons
 }
 
 // ------------------------------------------------------------------------------------------------------------ consumers: GEMV
-// one (16 rows x 128 k) unit; see gemv::unit1 (w4a16_gemv_impl.cuh) for the arithmetic.  All operands by shared address; the loads
-// of both units of a stage are issued before either is consumed.
+// one (32 rows x 128 k) unit; see gemv::unit1 (w4a16_gemv_impl.cuh) for the arithmetic of each 16-row half.  Both halves take the same
+// activation fragment, group sum and step.  All operands by shared address; every load of a stage is issued before the first MMA.
 struct UnitRegs {
-    uint4 wa, wb, xe, xo;
-    uint32_t z;   // zero points of rows g (bits 0..7) and g + 8 (bits 8..15)
-    uint32_t sc;  // half2: scales of rows g, g + 8
+    uint4 wa, wb, wc, wd, xe, xo;  // rows g, g + 8, g + 16, g + 24; the activation planes
+    uint32_t z;    // zero points of rows g, g + 8, g + 16, g + 24 (bytes 0..3)
+    uint2 sc;      // half2 pairs: scales of rows (g, g + 8), (g + 16, g + 24)
     int sxv;
 };
+struct RowSums {
+    float a, b, c, d;  // rows g, g + 8, g + 16, g + 24
+};
 // st_addr: the group's activation step, read after the MMAs are issued (held from the operand loads on, it was spilled to local memory)
-TCE_DEVINL void unit_compute(const UnitRegs &u, uint32_t st_addr, float lscale, float &totA, float &totB) {
+TCE_DEVINL void unit_compute(const UnitRegs &u, uint32_t st_addr, float lscale, RowSums &tot) {
     constexpr uint32_t ML = 0x0f0f0f0fu, MH = 0xf0f0f0f0u;
-    int accL[4], accH[4];
+    int accL[4], accH[4], accL2[4], accH2[4];
     mma_m16n8k32_u8s8_z(accL, u.wa.x & ML, u.wb.x & ML, u.wa.y & ML, u.wb.y & ML, u.xe.x, u.xe.y);
     mma_m16n8k32_u8s8_z(accH, u.wa.x & MH, u.wb.x & MH, u.wa.y & MH, u.wb.y & MH, u.xo.x, u.xo.y);
+    mma_m16n8k32_u8s8_z(accL2, u.wc.x & ML, u.wd.x & ML, u.wc.y & ML, u.wd.y & ML, u.xe.x, u.xe.y);
+    mma_m16n8k32_u8s8_z(accH2, u.wc.x & MH, u.wd.x & MH, u.wc.y & MH, u.wd.y & MH, u.xo.x, u.xo.y);
     mma_m16n8k32_u8s8(accL, u.wa.z & ML, u.wb.z & ML, u.wa.w & ML, u.wb.w & ML, u.xe.z, u.xe.w);
     mma_m16n8k32_u8s8(accH, u.wa.z & MH, u.wb.z & MH, u.wa.w & MH, u.wb.w & MH, u.xo.z, u.xo.w);
-    const float2 sc = h2_to_f2(u.sc);
+    mma_m16n8k32_u8s8(accL2, u.wc.z & ML, u.wd.z & ML, u.wc.w & ML, u.wd.w & ML, u.xe.z, u.xe.w);
+    mma_m16n8k32_u8s8(accH2, u.wc.z & MH, u.wd.z & MH, u.wc.w & MH, u.wd.w & MH, u.xo.z, u.xo.w);
+    const float2 sc01 = h2_to_f2(u.sc.x), sc23 = h2_to_f2(u.sc.y);
     const float st = lds_f32(st_addr) * lscale;
-    const int zAq = (int)(u.z & 0xFFu), zBq = (int)(u.z >> 8);
+    const int z0 = (int)(u.z & 0xFFu), z1 = (int)((u.z >> 8) & 0xFFu), z2 = (int)((u.z >> 16) & 0xFFu), z3 = (int)(u.z >> 24);
     // X = 2^24*p3 + 2^16*p2 + 2^8*p1 + p0; odd slots carry 16 x nibble (exact multiple of 16): c0 * 256 + c1 per parity, then q*X - z*sum X
-    const int vA = (accL[0] << 8) + accL[1] + (((accH[0] << 8) + accH[1]) >> 4) - zAq * u.sxv;
-    const int vB = (accL[2] << 8) + accL[3] + (((accH[2] << 8) + accH[3]) >> 4) - zBq * u.sxv;
-    totA += (sc.x * st) * (float)vA;
-    totB += (sc.y * st) * (float)vB;
+    const int v0 = (accL[0] << 8) + accL[1] + (((accH[0] << 8) + accH[1]) >> 4) - z0 * u.sxv;
+    const int v1 = (accL[2] << 8) + accL[3] + (((accH[2] << 8) + accH[3]) >> 4) - z1 * u.sxv;
+    const int v2 = (accL2[0] << 8) + accL2[1] + (((accH2[0] << 8) + accH2[1]) >> 4) - z2 * u.sxv;
+    const int v3 = (accL2[2] << 8) + accL2[3] + (((accH2[2] << 8) + accH2[3]) >> 4) - z3 * u.sxv;
+    tot.a += (sc01.x * st) * (float)v0;
+    tot.b += (sc01.y * st) * (float)v1;
+    tot.c += (sc23.x * st) * (float)v2;
+    tot.d += (sc23.y * st) * (float)v3;
 }
 
-// Hand one tile's row sums of this warp, times 1/rms, to the epilogue warp (red buffer `cs`).  1/rms is the warp's word sm.inv[cw]; a
+// Hand one tile's 32 row sums of this warp, times 1/rms, to the epilogue warp (red buffer `cs`).  1/rms is the warp's word sm.inv[cw]; a
 // negative word -1 - parity (RMSNorm phase, first tile) means: wait for the partner's sums of squares on the rx barrier, then take 1/rms
 // from all 32.
-TCE_DEVINL void hand_tile(const Args &a, const GemvOp &op, const PSmem &sm, Red &cs, float totA, float totB, int cw, int lane) {
+TCE_DEVINL void hand_tile(const Args &a, const GemvOp &op, const PSmem &sm, Red &cs, RowSums tot, int cw, int lane) {
     const int g = lane >> 2, t = lane & 3;
     float inv = sm.inv[cw];
     if (inv < 0.f) {
@@ -623,23 +630,27 @@ TCE_DEVINL void hand_tile(const Args &a, const GemvOp &op, const PSmem &sm, Red 
         __syncwarp();  // every lane has read the flag
         if (lane == 0) sm.inv[cw] = inv;
     }
-    totA += __shfl_xor_sync(0xffffffffu, totA, 1);  // (p3, p2) share of t = 0 + (p1, p0) share of t = 1
-    totB += __shfl_xor_sync(0xffffffffu, totB, 1);
+    tot.a += __shfl_xor_sync(0xffffffffu, tot.a, 1);  // (p3, p2) share of t = 0 + (p1, p0) share of t = 1
+    tot.b += __shfl_xor_sync(0xffffffffu, tot.b, 1);
+    tot.c += __shfl_xor_sync(0xffffffffu, tot.c, 1);
+    tot.d += __shfl_xor_sync(0xffffffffu, tot.d, 1);
     mbar_wait_u32(sm.redempty_u32 + (uint32_t)cs.rb * 8u, cs.rphase ^ 1);
-    float *rbuf = sm.red + ((size_t)cs.rb * kCW + cw) * 16;
+    float *rbuf = sm.red + ((size_t)cs.rb * kCW + cw) * kTileRows;
     if (t == 0) {
-        rbuf[g] = totA * inv;
-        rbuf[g + 8] = totB * inv;
+        rbuf[g] = tot.a * inv;
+        rbuf[g + 8] = tot.b * inv;
+        rbuf[g + 16] = tot.c * inv;
+        rbuf[g + 24] = tot.d * inv;
     }
     __syncwarp();
     if (lane == 0) mbar_arrive_u32(sm.redfull_u32 + (uint32_t)cs.rb * 8u);
     cs.advance();
 }
 
-// A stage holds two boxes of this CTA's (tile, box) walk (see KRange); warp cw consumes group cw of each (slot 0, and slot 1 16 KiB
-// further).  The two boxes may belong to two tiles, and a tile is handed to the epilogue after its last box.  Group gi of a slot sits at a
-// fixed place whatever the shape, so every operand address is a per-lane constant plus the slot base and the box's place in the planes
-// (+4 KiB planes, +128 B sums, +64 B steps per box): the inner loop carries almost no address arithmetic (the ALU pipe is what bounds it).
+// A stage holds one box of this CTA's (tile, box) walk (see KRange); warp cw consumes group cw of it, all 32 rows, and hands the tile to the
+// epilogue after its last box.  Group gi of a box sits at a fixed place whatever the shape, so every operand address is a per-lane constant
+// plus the stage base and the box's place in the planes (+4 KiB planes, +128 B sums, +64 B steps per box): the inner loop carries almost no
+// address arithmetic (the ALU pipe is what bounds it).
 // Stamps of consumer warp 0 (TCE_PK_DEBUG): 4 first stage landed, 5 last stage released, 6 last tile handed to the epilogue.
 // The warp's red-buffer position, its lane id and 1/rms are taken afresh here (shared memory, %laneid, a shuffle of the same value), not
 // carried in registers across the phase loop: held there, they were spilled to local memory (the attention and staging code set the
@@ -662,11 +673,12 @@ TCE_DEVINL void consume_gemv(const Args &a, const GemvOp &op, const PSmem &sm, R
     const KRange kr = k_range(op.NG, rank);
     const int nb = kr.nb, nbox = (t1 - t0) * nb;
     const int lim = kr.ng - cw;  // box b carries this warp's group when 16 b < lim (the last box of a K range may have fewer than 16)
-    // row g of group cw, this lane's 16-byte chunk: the 16 rows of a group 64 B apart (conflict-free LDS.128), gate | up as two 8-row regions
-    const uint32_t w_lane = (uint32_t)cw * (op.gate_up ? 512u : 1024u) + (uint32_t)g * 64u + (uint32_t)t * 16u;
-    const uint32_t wb_off = op.gate_up ? 8192u : 512u;  // row g + 8
-    const uint32_t m_lane = (uint32_t)kMetaOff + (uint32_t)(cw * 8 + g) * 4u;                            // scales of rows g, g + 8 of group cw
-    const uint32_t z_lane = (uint32_t)kMetaOff + 512u + (uint32_t)(cw * 8 + g) * 2u;
+    // row g of group cw, this lane's 16-byte chunk: the rows of a group 64 B apart (conflict-free LDS.128); gate | up: the 16 gate rows of
+    // the group (1 KiB), its 16 up rows 16 KiB further
+    const uint32_t w_lane = (uint32_t)cw * (op.gate_up ? 1024u : 2048u) + (uint32_t)g * 64u + (uint32_t)t * 16u;
+    const uint32_t wc_off = op.gate_up ? 16384u : 1024u;  // row g + 16 (row g + 8: +512 B, row g + 24: wc_off + 512 B)
+    const uint32_t m_lane = (uint32_t)kMetaOff + (uint32_t)(cw * 8 + g) * 8u;                             // scales of rows g, g + 8, g + 16, g + 24 of group cw
+    const uint32_t z_lane = (uint32_t)kMetaOff + 1024u + (uint32_t)(cw * 8 + g) * 4u;
     const uint32_t x_lane = sm.xs_u32 + (uint32_t)((g >> 1) & 1) * (uint32_t)plane_ic(op.NG) * 2u + (uint32_t)(t * 2 + (g & 1)) * 16u + (uint32_t)cw * 256u;
     const uint32_t s_lane = sm.gsum_u32 + (uint32_t)(2 * cw + (t & 1)) * 4u;
     const uint32_t q_lane = sm.gx_u32 + (uint32_t)cw * 4u;
@@ -676,61 +688,37 @@ TCE_DEVINL void consume_gemv(const Args &a, const GemvOp &op, const PSmem &sm, R
         mbar_wait_u32(sm.full_u32 + (uint32_t)rs.stage * 8u, rs.phase);
         stamp(a, cta, nphase, p, 4);
     }
-    int box = 0;  // box of the next slot within its tile
-    float totA = 0.f, totB = 0.f;
-    for (int left = nbox; left > 0; left -= 2) {
-        const int box0 = box, box1 = (box0 + 1 == nb) ? 0 : box0 + 1;
-        const bool two = left > 1;
-        box = (box1 + 1 == nb) ? 0 : box1 + 1;  // (unused after a lone last box)
-        const bool has0 = box0 * kBoxGroups < lim, has1 = two && box1 * kBoxGroups < lim;  // warp-uniform
+    int box = 0;  // box of the next stage within its tile
+    RowSums tot = {0.f, 0.f, 0.f, 0.f};
+    for (int left = nbox; left > 0; left--) {
+        const bool has = box * kBoxGroups < lim;  // warp-uniform
         mbar_wait_u32(sm.full_u32 + (uint32_t)rs.stage * 8u, rs.phase);
-        const uint32_t base = sm.ring_u32 + (uint32_t)rs.stage * (uint32_t)kStageBytes;
-        const uint32_t wb_ = base + w_lane, mb_ = base + m_lane, zb_ = base + z_lane;
-        UnitRegs u0, u1;
-        u0.xe = u0.xo = u1.xe = u1.xo = make_uint4(0u, 0u, 0u, 0u);
-        if (has0) {
-            const uint32_t xb_ = x_lane + (uint32_t)box0 * 4096u;
-            u0.wa = lds_u4(wb_);
-            u0.wb = lds_u4(wb_ + wb_off);
+        if (has) {
+            const uint32_t base = sm.ring_u32 + (uint32_t)rs.stage * (uint32_t)kStageBytes;
+            const uint32_t wb_ = base + w_lane, xb_ = x_lane + (uint32_t)box * 4096u;
+            UnitRegs u;
+            u.wa = lds_u4(wb_);
+            u.wb = lds_u4(wb_ + 512u);
+            u.wc = lds_u4(wb_ + wc_off);
+            u.wd = lds_u4(wb_ + wc_off + 512u);
+            u.xe = u.xo = make_uint4(0u, 0u, 0u, 0u);
             if (xl) {
-                u0.xe = lds_u4(xb_);
-                u0.xo = lds_u4(xb_ + 128u);
+                u.xe = lds_u4(xb_);
+                u.xo = lds_u4(xb_ + 128u);
             }
-            u0.sc = lds_u32(mb_);
-            u0.z = lds_u16(zb_);
-            u0.sxv = (int)lds_u32(s_lane + (uint32_t)box0 * 128u);
+            u.sc = lds_u2(base + m_lane);
+            u.z = lds_u32(base + z_lane);
+            u.sxv = (int)lds_u32(s_lane + (uint32_t)box * 128u);
+            unit_compute(u, q_lane + (uint32_t)box * 64u, lscale, tot);
         }
-        if (has1) {
-            const uint32_t xb_ = x_lane + (uint32_t)box1 * 4096u;
-            u1.wa = lds_u4(wb_ + 16384u);
-            u1.wb = lds_u4(wb_ + 16384u + wb_off);
-            if (xl) {
-                u1.xe = lds_u4(xb_);
-                u1.xo = lds_u4(xb_ + 128u);
-            }
-            u1.sc = lds_u32(mb_ + (uint32_t)kBoxMetaBytes);
-            u1.z = lds_u16(zb_ + (uint32_t)kBoxMetaBytes);
-            u1.sxv = (int)lds_u32(s_lane + (uint32_t)box1 * 128u);
-        }
-        if (has0) unit_compute(u0, q_lane + (uint32_t)box0 * 64u, lscale, totA, totB);
-        // slot 0 ends a tile: its sums wait in hA / hB while slot 1 starts the next one
-        const bool end0 = box0 + 1 == nb;
-        float hA = 0.f, hB = 0.f;
-        if (end0) {
-            hA = totA;
-            hB = totB;
-            totA = totB = 0.f;
-        }
-        if (has1) unit_compute(u1, q_lane + (uint32_t)box1 * 64u, lscale, totA, totB);
         __syncwarp();
         if (lane == 0) mbar_arrive_u32(sm.empty_u32 + (uint32_t)rs.stage * 8u);
         rs.advance(sm.nst);
-        if (left <= 2 && cw == 0 && lane == 0) stamp(a, cta, nphase, p, 5);
-        const bool end1 = two && box1 + 1 == nb;
-        if (end0) hand_tile(a, op, sm, cs, hA, hB, cw, lane);
-        if (end1) {
-            hand_tile(a, op, sm, cs, totA, totB, cw, lane);
-            totA = totB = 0.f;
+        if (left == 1 && cw == 0 && lane == 0) stamp(a, cta, nphase, p, 5);
+        if (++box == nb) {
+            box = 0;
+            hand_tile(a, op, sm, cs, tot, cw, lane);
+            tot.a = tot.b = tot.c = tot.d = 0.f;
         }
     }
     __syncwarp();  // every lane has read the old position
@@ -748,7 +736,7 @@ struct EpiState {
 // Stamp (TCE_PK_DEBUG): 7 the last tile's partials are in; the caller stamps 3 after its last publish.
 // The lane id is read here (%laneid), as in consume_gemv: passed in, the lane-derived offsets and predicates were hoisted out of the phase
 // loop, spilled, and reloaded on every tile.
-// Rank 0 publishes the first half of the pair's tiles and rank 1 the rest (both epilogue warps publish), adding the partner's 16
+// Rank 0 publishes the first half of the pair's tiles and rank 1 the rest (both epilogue warps publish), adding the partner's 32
 // row sums, received by st.async into a `prx` slot, to its own: the same bits on every run.  Contiguous halves let each direction stream up
 // to kPairSlots tiles ahead; tiles owned alternately made the two epilogues wait for each other on every tile (on H100 the Llama-3-8B step
 // took 2.96 ms instead of 2.01).
@@ -764,15 +752,11 @@ TCE_DEVINL void epilogue_gemv(const Args &a, const GemvOp &op, const PSmem &sm, 
     for (int tile = t0; tile < t1; tile++) {
         mbar_wait_u32(sm.redfull_u32 + (uint32_t)es.rb * 8u, es.rphase);
         if (tile == t1 - 1 && lane == 0) stamp(a, cta, nphase, p, 7);
-        const float *rbuf = sm.red + (size_t)es.rb * kCW * 16;
-        // lane l < 16 sums consumer warps 0..7 of row l, lane l + 16 warps 8..15
+        const float *rbuf = sm.red + (size_t)es.rb * kCW * kTileRows;
+        // lane l sums row l over consumer warps 0..15, in that order
         float v = 0.f;
-        {
-            const int row = lane & 15, w0 = (lane >> 4) * 8;
 #pragma unroll
-            for (int w = 0; w < 8; w++) v += rbuf[(w0 + w) * 16 + row];
-        }
-        v += __shfl_down_sync(0xffffffffu, v, 16);
+        for (int w = 0; w < kCW; w++) v += rbuf[w * kTileRows + lane];
         __syncwarp();
         if (lane == 0) mbar_arrive_u32(sm.redempty_u32 + (uint32_t)es.rb * 8u);
         es.advance();
@@ -781,52 +765,49 @@ TCE_DEVINL void epilogue_gemv(const Args &a, const GemvOp &op, const PSmem &sm, 
         if (!mine) {  // the partner publishes this tile: send it this CTA's row sums
             const uint32_t n = st.nsent++;
             mbar_wait_cluster(smem_u32(sm.pfree + slot), ((n / kPairSlots) & 1u) ^ 1u);
-            if (lane < 16)
-                st_async_b32(map_to_cta(smem_u32(sm.prx + slot * 16 + lane), rank ^ 1u), __float_as_uint(v), map_to_cta(smem_u32(sm.prx_full + slot), rank ^ 1u));
+            st_async_b32(map_to_cta(smem_u32(sm.prx + slot * kTileRows + lane), rank ^ 1u), __float_as_uint(v), map_to_cta(smem_u32(sm.prx_full + slot), rank ^ 1u));
             continue;
         }
         const uint32_t n = st.nrecv++;
         const uint32_t fb = smem_u32(sm.prx_full + slot);
-        if (lane == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(fb), "r"(64u) : "memory");
+        if (lane == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(fb), "r"((uint32_t)kTileRows * 4u) : "memory");
         mbar_wait_u32(fb, (n / kPairSlots) & 1u);
-        v += sm.prx[slot * 16 + (lane & 15)];  // a sum of two terms: the same bits whichever rank publishes
+        v += sm.prx[slot * kTileRows + lane];  // a sum of two terms: the same bits whichever rank publishes
         __syncwarp();
         if (lane == 0) mbar_arrive_remote(map_to_cta(smem_u32(sm.pfree + slot), rank ^ 1u));
         switch (op.epi) {
-            case PE_DELTA_LL:
+            case PE_DELTA_LL: {
                 // o_proj / down_proj output rows: one {float, tag} word each, into slot `rank` of every rank's buffer (NVLink peer stores
                 // when tensor parallel) -- the residual add happens in every reader (stage_rms)
-                if (lane < 16) {
-                    const size_t o = (size_t)a.tp_rank * a.E + (size_t)tile * 16 + lane;
-                    if (tp) {
-                        for (int pr = 0; pr < a.tp_size; pr++) st_ll(a.tp_delta[which][pr] + o, __float_as_uint(v), tag, true);
-                    } else {
-                        st_ll(out_ll + o, __float_as_uint(v), tag, false);
-                    }
+                const size_t o = (size_t)a.tp_rank * a.E + (size_t)tile * kTileRows + lane;
+                if (tp) {
+                    for (int pr = 0; pr < a.tp_size; pr++) st_ll(a.tp_delta[which][pr] + o, __float_as_uint(v), tag, true);
+                } else {
+                    st_ll(out_ll + o, __float_as_uint(v), tag, false);
                 }
                 break;
+            }
             case PE_HALF_LL: {
                 const float hi = __shfl_down_sync(0xffffffffu, v, 1);
-                if (lane < 16 && !(lane & 1)) st_ll(out_ll + (size_t)tile * 8 + (lane >> 1), pack_half2(v, hi), tag, false);
+                if (!(lane & 1)) st_ll(out_ll + (size_t)tile * (kTileRows / 2) + (lane >> 1), pack_half2(v, hi), tag, false);
                 break;
             }
             case PE_SILU_LL: {
-                // rows 0-7 = gate, rows 8-15 = up of the same output channels: y = SiLU(gate) * up
+                // rows 0-15 = gate, rows 16-31 = up of the same 16 output channels: y = SiLU(gate) * up
                 // (reference SiLuMul_half, llm/src/nn_modules/cuda/Int4llamaDecoderLayer.cu:21-30; fp32 here)
-                const float up = __shfl_down_sync(0xffffffffu, v, 8);
+                const float up = __shfl_down_sync(0xffffffffu, v, 16);
                 const float y = v / (1.f + __expf(-v)) * up;
                 const float yhi = __shfl_down_sync(0xffffffffu, y, 1);
-                if (lane < 8 && !(lane & 1)) st_ll(out_ll + (size_t)tile * 4 + (lane >> 1), pack_half2(y, yhi), tag, false);
+                if (lane < 16 && !(lane & 1)) st_ll(out_ll + (size_t)tile * (kTileRows / 4) + (lane >> 1), pack_half2(y, yhi), tag, false);
                 break;
             }
-            case PE_LOGITS:
-                if (lane < 16) {
-                    const int idx = tile * 16 + lane;
-                    a.logits[idx] = v;
-                    const unsigned long long key = argmax_key(v, a.vocab_base + idx);
-                    st.best = key > st.best ? key : st.best;
-                }
+            case PE_LOGITS: {
+                const int idx = tile * kTileRows + lane;
+                a.logits[idx] = v;
+                const unsigned long long key = argmax_key(v, a.vocab_base + idx);
+                st.best = key > st.best ? key : st.best;
                 break;
+            }
         }
     }
 }
@@ -1224,9 +1205,9 @@ __global__ void __launch_bounds__(kThreads, 1) decode_persistent_kernel(const __
 }
 
 // ------------------------------------------------------------------------------------------------------------ repack kernel
-// scales half[rows][sf_w] + zeros u32[rows][zeros_w] (QM_CUDA, llm/tools/quantize_methods.py:370-442) -> one 768-byte record per
-// (16-row tile, 16-group box of the K range [g0, g0 + ng)): scales half[16 groups][8][2] (rows g and g + 8 adjacent), then zero points
-// u8[16 groups][8][2] in the same order.
+// scales half[rows][sf_w] + zeros u32[rows][zeros_w] (QM_CUDA, llm/tools/quantize_methods.py:370-442) -> one 1536-byte record per
+// (32-row tile, 16-group box of the K range [g0, g0 + ng)): scales half[16 groups][8][4] (rows g, g + 8, g + 16, g + 24 adjacent), then
+// zero points u8[16 groups][8][4] in the same order.
 __global__ void repack_meta_kernel(W4Seg s0, W4Seg s1, W4Seg s2, int nseg, int gate_up, int g0, int ng, int nb, int zeros_w, int sf_w, int num_tiles, uint8_t *out) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;  // (tile, box, gi)
     if (idx >= num_tiles * nb * kBoxGroups) return;
@@ -1234,16 +1215,16 @@ __global__ void repack_meta_kernel(W4Seg s0, W4Seg s1, W4Seg s2, int nseg, int g
     const int tile = rb / nb, box = rb - tile * nb;
     const int lg = kBoxGroups * box + gi, G = g0 + lg;
     uint8_t *rec = out + (size_t)rb * kBoxMetaBytes;
-    __half *so = reinterpret_cast<__half *>(rec) + gi * 16;  // [g][2]: rows g and g + 8 adjacent
-    uint8_t *zo = rec + 512 + gi * 16;                         // zero points, same order, one byte each
-    for (int r = 0; r < 16; r++) {
+    __half *so = reinterpret_cast<__half *>(rec) + gi * kTileRows;  // [g][4]: rows g, g + 8, g + 16, g + 24 adjacent
+    uint8_t *zo = rec + 2 * kBoxGroups * kTileRows + gi * kTileRows;  // zero points, same order, one byte each
+    for (int r = 0; r < kTileRows; r++) {
         const W4Seg *seg = &s0;
         int row;
         if (gate_up) {
-            seg = (r < 8) ? &s0 : &s1;
-            row = tile * 8 + (r & 7);
+            seg = (r < kTileRows / 2) ? &s0 : &s1;
+            row = tile * (kTileRows / 2) + (r & 15);
         } else {
-            row = tile * 16 + r;
+            row = tile * kTileRows + r;
             if (nseg > 1 && row >= s0.rows) {
                 row -= s0.rows;
                 seg = &s1;
@@ -1253,7 +1234,7 @@ __global__ void repack_meta_kernel(W4Seg s0, W4Seg s1, W4Seg s2, int nseg, int g
                 }
             }
         }
-        const int slot = (r & 7) * 2 + (r >> 3);
+        const int slot = (r & 7) * 4 + (r >> 3);
         if (lg < ng) {
             so[slot] = seg->scales[(size_t)row * sf_w + G];
             zo[slot] = (uint8_t)((seg->zeros[(size_t)row * zeros_w + (G >> 3)] >> ((G & 7) * 4)) & 0xFu);
@@ -1276,7 +1257,8 @@ int attn_nsplit_max(int ncta, int KVH, int max_ctx) {
 }
 
 static size_t fixed_bytes(const Args &a) {
-    return (size_t)a.xs_bytes + (size_t)resid_floats(a) * 4 + (size_t)a.max_ng * 12 + (size_t)kRedBufs * kCW * 16 * 4 + 32 * 4 + kCW * 4 + 256 * 4 + (size_t)kPairSlots * 16 * 4 +
+    return (size_t)a.xs_bytes + (size_t)resid_floats(a) * 4 + (size_t)a.max_ng * 12 + (size_t)kRedBufs * kCW * kTileRows * 4 + 32 * 4 + kCW * 4 + 256 * 4 +
+           (size_t)kPairSlots * kTileRows * 4 +
            (size_t)(2 * kMaxStages + 2 * kRedBufs + 1 + 2 * kPairSlots) * 8 + (size_t)kCW * 8 + 1024;
 }
 void plan_smem(Args &a, int smem_optin) {
@@ -1292,7 +1274,7 @@ size_t smem_bytes(const Args &a) { return fixed_bytes(a) + (size_t)a.nst * kStag
 cudaError_t repack_meta(Ctx *ctx, const W4Seg *segs, int nseg, int gate_up, int IC, const KRange &kr, uint8_t *out, cudaStream_t stream) {
     int rows = 0;
     for (int i = 0; i < nseg; i++) rows += segs[i].rows;
-    const int num_tiles = rows / 16;
+    const int num_tiles = rows / kTileRows;
     const int zw = zeros_width(IC, kW4Group);
     const int total = num_tiles * kr.nb * kBoxGroups;
     if (total == 0) return cudaSuccess;

@@ -177,7 +177,8 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         if (err) *err = m;
         return cudaErrorNotSupported;
     };
-    if (hd != 128 || nrep > 4 || ncta < KVH || F % 16 || V % 16) return no("shape outside the persistent kernel's envelope");
+    // 32-row tiles (pk::kTileRows; gate | up: 16 channels): with hd = 128 the q|k|v segment boundaries fall on tile boundaries
+    if (hd != 128 || nrep > 4 || ncta < KVH || F % pk::kTileRows || V % pk::kTileRows) return no("shape outside the persistent kernel's envelope");
     // clusters of two CTAs split K (see pk::KRange): an even number of SMs, and two 128-groups or more in every op
     if (ncta % 2) return no("odd SM count: the persistent kernel runs on clusters of two CTAs");
     pk::Args a{};
@@ -185,7 +186,7 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         pk::GemvOp o{};
         o.IC = IC;
         o.NG = IC / kW4Group;
-        o.num_tiles = rows / 16;
+        o.num_tiles = rows / pk::kTileRows;
         o.nseg = nseg;
         o.gate_up = gate_up;
         o.rows0 = rows0;
@@ -235,7 +236,8 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
             for (int i = 0; i < 7; i++) {
                 const pk::GemvOp &o = a.op[opi[i]];
                 const pk::KRange kr = pk::k_range(o.NG, rank);
-                DCK(encode_w4_tmap_units(&maps[rank * nmaps + (size_t)l * 7 + i], t7[i]->w, t7[i]->oc, t7[i]->ic, kr.bw, o.gate_up ? 8 : 16, kr.g0, kr.ng));
+                const int box_rows = o.gate_up ? pk::kTileRows / 2 : pk::kTileRows;  // gate | up: a box of each matrix per stage
+                DCK(encode_w4_tmap_units(&maps[rank * nmaps + (size_t)l * 7 + i], t7[i]->w, t7[i]->oc, t7[i]->ic, kr.bw, box_rows, kr.g0, kr.ng));
             }
         }
         pk::LayerDesc &D = descs[l];
@@ -266,7 +268,7 @@ cudaError_t LlamaDecoder::build_persistent(std::string *err) {
         const W4Seg lm[1] = {seg_of(w_.lm_head)};
         for (int rank = 0; rank < 2; rank++) {
             const pk::KRange kr = pk::k_range(o.NG, rank);
-            DCK(encode_w4_tmap_units(&maps[rank * nmaps + (size_t)Lyr * 7], w_.lm_head.w, w_.lm_head.oc, w_.lm_head.ic, kr.bw, 16, kr.g0, kr.ng));
+            DCK(encode_w4_tmap_units(&maps[rank * nmaps + (size_t)Lyr * 7], w_.lm_head.w, w_.lm_head.oc, w_.lm_head.ic, kr.bw, pk::kTileRows, kr.g0, kr.ng));
             uint8_t *m = (uint8_t *)dalloc((size_t)o.num_tiles * kr.nb * pk::kBoxMetaBytes);
             if (!m) return cudaErrorMemoryAllocation;
             DCK(pk::repack_meta(ctx_, lm, 1, 0, o.IC, kr, m, s));

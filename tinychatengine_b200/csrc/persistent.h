@@ -1,7 +1,7 @@
 // persistent.h -- host/device interface of the persistent Llama decode kernel (decode_persistent.cu).
 //
 // One kernel per decoded token, one CTA per SM, launched as clusters of two CTAs: both CTAs of a cluster walk the same GEMV tiles, each
-// over its half of the 128-groups (k_range), and one CTA per tile adds its partner's 16 row sums (st.async over DSMEM).  Everything a
+// over its half of the 128-groups (k_range), and one CTA per tile adds its partner's 32 row sums (st.async over DSMEM).  Everything a
 // token needs from HBM -- packed weights, their repacked scales/zeros, and the K/V cache rows -- flows through ONE ring of TMA stages per
 // CTA that is filled by a producer warp which depends on nothing but static data, so it runs ahead across all phase boundaries.  Phases
 // hand their results to each other through flag-carrying 8-byte words (value + phase tag, stored and loaded as one unit): there is no
@@ -17,9 +17,10 @@ constexpr int kAuxWarps = 4;                     // warpgroup 0: loader warp, ep
 constexpr int kThreads = 32 * (kAuxWarps + kCW); // 640
 constexpr int kConsumerThreads = 32 * kCW;       // 512
 constexpr int kHalfBytes = 16384;                // 64 K rows or 64 V rows (one half of an attention stage)
-constexpr int kBoxGroups = 16;                   // 128-k groups per weight box; a stage carries two boxes (slots 0 and 1, 16 KiB apart)
-constexpr int kMetaOff = 2 * kHalfBytes;         // per slot (768 B apart): scales half[16 groups][8][2] (rows g, g+8 adjacent) then zero points u8[16][8][2]
-constexpr int kBoxMetaBytes = 768;
+constexpr int kTileRows = 32;                    // rows of a GEMV tile (gate | up: 16 gate rows + 16 up rows of the same 16 channels)
+constexpr int kBoxGroups = 16;                   // 128-k groups per weight box; a stage carries one box (16 groups x 32 rows x 64 B = 32 KiB)
+constexpr int kMetaOff = 2 * kHalfBytes;         // the box's record: scales half[16 groups][8][4] (rows g, g+8, g+16, g+24 adjacent) then zero points u8[16][8][4]
+constexpr int kBoxMetaBytes = 1536;
 constexpr int kStageBytes = 34816;               // 32 KiB + 1.5 KiB meta (+ pad), 1 KiB multiple (128B-swizzle atoms of the K/V boxes)
 constexpr int kMaxStages = 6;
 constexpr int kRedBufs = 3;
@@ -33,17 +34,17 @@ enum OpIdx : int { OPI_QKV = 0, OPI_O = 1, OPI_GATEUP = 2, OPI_DOWN = 3, OPI_LMH
 // shape of one GEMV op; identical for every layer, so it lives in the kernel parameter block.
 struct GemvOp {
     int IC, NG;          // input channels, 128-groups per row
-    int num_tiles;       // 16-row tiles (gate | up: 8 gate rows + 8 up rows)
-    int nseg, gate_up;   // row segments (q|k|v = 3); gate_up: tiles interleave 8 rows of each of the two segments
+    int num_tiles;       // 32-row tiles (gate | up: 16 gate rows + 16 up rows)
+    int nseg, gate_up;   // row segments (q|k|v = 3); gate_up: tiles interleave 16 rows of each of the two segments
     int rows0, rows1;    // rows of segments 0 and 1 (tile -> segment)
     int x_mode, epi;
 };
 
 // The K range a CTA reduces over: cluster rank 0 the first ceil(NG / 2) groups, rank 1 the rest.  Contiguous halves keep every TMA box a
-// plain range of groups of one tensor map, encoded over the half (box width bw), so a box never reads the partner's groups.  The range is walked as `nb` boxes of 16 groups per tile, tile by tile; a ring stage takes two
-// consecutive boxes (slot 0 at 0, slot 1 at 16 KiB), which may belong to two tiles: at NG = 32 a stage holds the halves of two tiles.  Group gi
-// of a slot sits at gi KiB (gate | up: the 8 gate rows at gi * 512 B, the 8 up rows 8 KiB further); a box that runs past the range is
-// zero-filled by TMA and still counts its full bytes.  Scales and zeros follow the same walk: one 768-byte record per (tile, box).
+// plain range of groups of one tensor map, encoded over the half (box width bw), so a box never reads the partner's groups.  The range is
+// walked as `nb` boxes of 16 groups per tile, tile by tile, one box per ring stage: at NG = 32 (IC = 4096) a stage is a whole tile.  Group gi
+// of a box sits at gi * 2 KiB (gate | up: the 16 gate rows at gi KiB, the 16 up rows 16 KiB further); a box that runs past the range is
+// zero-filled by TMA and still counts its full bytes.  Scales and zeros follow the same walk: one 1536-byte record per (tile, box).
 struct KRange {
     int g0, ng;  // first group, groups
     int nb, bw;  // boxes per tile, TMA box width in groups
@@ -62,7 +63,7 @@ __host__ __device__ inline KRange k_range(int NG, int rank) {
 __host__ __device__ inline int plane_ic(int NG) { return k_range(NG, 0).ng * 128; }
 
 struct LayerDesc {       // per layer, global memory
-    const uint8_t *meta[2][4];   // repacked scales|zeros of qkv, o, gate_up, down over the K range of cluster rank 0 / 1: [tile][box][768 B]
+    const uint8_t *meta[2][4];   // repacked scales|zeros of qkv, o, gate_up, down over the K range of cluster rank 0 / 1: [tile][box][1536 B]
     const float *input_norm, *post_norm;
     __half *k_cache, *v_cache;   // [KVH][max_ctx][128] of this layer (append)
     int k_row0, v_row0;          // first row of this layer's K / V slab in the cache tensor map

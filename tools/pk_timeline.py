@@ -108,16 +108,16 @@ def main():
     # the compute of every stage and, where a tile is one box (q|k|v, o_proj, gate|up at Llama-3-8B), the hand-offs of all tiles but the
     # last.  With the stages already in shared memory (q|k|v and o_proj: at most 3 per CTA, loaded while the previous phases ran) it is the
     # consumer-only cost of a ring stage.  Stages per CTA follow the kernel's layout: the two CTAs of a cluster walk the tiles of their pair
-    # (partition over num_sms / 2), each over its half of the 128-groups in boxes of 16 groups (k_range), two boxes per ring stage.
+    # (partition over num_sms / 2), each over its half of the 128-groups in boxes of 16 groups (k_range) of a 32-row tile, one box per ring stage.
     tick = np.gcd.reduce(np.unique(raw[raw > 0] - raw[raw > 0].min()).astype(np.int64))
-    ops = {0: (E, (H + 2 * KVH) * hd // 16), 2: (H * hd, E // 16), 3: (E, 2 * F // 16), 4: (F, E // 16)}  # IC, 16-row tiles
+    ops = {0: (E, (H + 2 * KVH) * hd // 32), 2: (H * hd, E // 32), 3: (E, 2 * F // 32), 4: (F, E // 32)}  # IC, 32-row tiles
     sub = {}
     npair = ncta // 2
     for k, (ic, ntiles) in ops.items():
         ng, h = ic // 128, (ic // 128 + 1) // 2  # groups of a row; rank 0 takes the first h, rank 1 the rest
         tiles = np.array([(ntiles * (c // 2 + 1)) // npair - (ntiles * (c // 2)) // npair for c in range(ncta)])
         nb = np.array([(h if c % 2 == 0 else ng - h) + 15 for c in range(ncta)]) // 16  # boxes per tile
-        nst = (tiles * nb + 1) // 2
+        nst = tiles * nb
         rows = {"first_landed": [], "last_released": [], "handed": [], "epi_last_in": [], "published": [], "per_stage": []}
         for p in range(k, nphase - 1, 5):
             base = T[:, p, 1]
